@@ -18,9 +18,6 @@ int set_error(int code, const std::string& msg) {
   tls_error() = msg;
   return code;
 }
-int launch_attention_tc(const AttnLaunch& a, cudaStream_t s) {
-  return launch_attention_wgmma(a, s);
-}
 
 int num_sms() {  // of the current device (cached per ordinal: one process may hold handles on several GPUs)
   static int n[64] = {};
@@ -80,24 +77,17 @@ ProfScope::~ProfScope() {
 
 namespace {
 
-// fp32 [N, K] -> fp16 hi at [n, 0:K] and (np == 2) lo at [n, K:2K]; rows scaled by `scale` (q scaling fold).
-__global__ void pack_weight_kernel(const float* __restrict__ w, int N, int K, float scale, __half* __restrict__ out, int np) {
+// Element (n, k) of a source weight is w[n * sn + k * sk]: sk = 1 for nn.Linear ([out = N, in = K]), sn = 1 for Conv1D ([in, out],
+// x @ W). Both are packed to the K-major [N, np*K] operand layout, scaled by `scale` (the q scaling fold).
+// fp16 formats: hi at [n, 0:K] and (np == 2) lo at [n, K:2K].
+__global__ void pack_weight_kernel(const float* __restrict__ w, int N, int K, long long sn, long long sk, float scale, __half* __restrict__ out,
+                                   int np) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= static_cast<long long>(N) * K) return;
   const int n = static_cast<int>(i / K), k = static_cast<int>(i % K);
-  const float v = w[i] * scale;
+  const float v = w[n * sn + k * sk] * scale;
   __half hi, lo;
   split_hi_lo(v, hi, lo);
-  out[static_cast<long long>(n) * K * np + k] = hi;
-  if (np == 2) out[static_cast<long long>(n) * K * np + K + k] = lo;
-}
-// Conv1D weights are stored [in = K, out = N] (x @ W); repack to the K-major [N, np*K] operand layout.
-__global__ void pack_weight_t_kernel(const float* __restrict__ w, int N, int K, __half* __restrict__ out, int np) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<long long>(N) * K) return;
-  const int n = static_cast<int>(i / K), k = static_cast<int>(i % K);
-  __half hi, lo;
-  split_hi_lo(w[static_cast<long long>(k) * N + n], hi, lo);
   out[static_cast<long long>(n) * K * np + k] = hi;
   if (np == 2) out[static_cast<long long>(n) * K * np + K + k] = lo;
 }
@@ -105,7 +95,7 @@ __global__ void pack_weight_t_kernel(const float* __restrict__ w, int N, int K, 
 // hi8 = e4m3(hi * t), lo8 = e4m3(lo * 2^11 * t) with ONE power of two t per matrix: the one that puts the largest |hi| of the matrix in
 // (112, 224]. e4m3 is a floating-point format (2^-4 relative precision over 15 binades), so rows much smaller than the largest one
 // keep their precision; a per-row scale would only cost the epilogue a load per output column. w_inv[n] = 1 / t for every n.
-// Element (n, k) of the source is w[n * sn + k * sk] (sk = 1: nn.Linear; sn = 1: Conv1D). Two kernels: matrix |hi| maximum, then pack.
+// Two kernels: matrix |hi| maximum, then pack.
 __global__ void weight_absmax_kernel(const float* __restrict__ w, int N, int K, long long sn, long long sk, float scale,
                                      unsigned int* __restrict__ amax_bits) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -142,13 +132,32 @@ __global__ void pack_weight_f8_kernel(const float* __restrict__ w, int N, int K,
   }
   if (lane == 0) w_inv[n] = 1.f / t;
 }
-// One matrix: absmax pass + pack pass on stream s; `scratch` is one device word per call (kept alive by the caller).
-void launch_pack_weight_f8(const float* w, int N, int K, long long sn, long long sk, float scale, unsigned int* scratch, __half* out,
-                           float* w_inv, cudaStream_t s) {
+// Packs a group of [N, K] weights (w[i] scaled by scale[i]) into consecutive blocks of N operand rows of `out` on stream s, in fp16
+// format (np 1 / 2) or, with `f8_scratch`, in the fp16 + e4m3 format (np 2) with ONE scale t for the whole group: a group is one
+// GEMM operand (q, k and v). w_inv[i * N + n] = 1 / t. `f8_scratch` is one device word per call (kept alive by the caller).
+struct PackSrc {
+  PackSrc(const float* w_, float scale_ = 1.f) : w(w_), scale(scale_) {}
+  const float* w;
+  float scale;
+};
+void pack_weights(std::initializer_list<PackSrc> group, int N, int K, long long sn, long long sk, int np, unsigned int* f8_scratch,
+                  __half* out, float* w_inv, cudaStream_t s) {
   const long long tot = static_cast<long long>(N) * K;
-  cudaMemsetAsync(scratch, 0, sizeof(unsigned int), s);
-  weight_absmax_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, s>>>(w, N, K, sn, sk, scale, scratch);
-  pack_weight_f8_kernel<<<(N + 7) / 8, 256, 0, s>>>(w, N, K, sn, sk, scale, scratch, out, w_inv);
+  const unsigned blocks = static_cast<unsigned>((tot + 255) / 256);
+  if (!f8_scratch) {
+    for (const PackSrc& m : group) {
+      pack_weight_kernel<<<blocks, 256, 0, s>>>(m.w, N, K, sn, sk, m.scale, out, np);
+      out += tot * np;
+    }
+    return;
+  }
+  cudaMemsetAsync(f8_scratch, 0, sizeof(unsigned int), s);
+  for (const PackSrc& m : group) weight_absmax_kernel<<<blocks, 256, 0, s>>>(m.w, N, K, sn, sk, m.scale, f8_scratch);
+  for (const PackSrc& m : group) {
+    pack_weight_f8_kernel<<<(N + 7) / 8, 256, 0, s>>>(m.w, N, K, sn, sk, m.scale, f8_scratch, out, w_inv);
+    out += tot * 2;
+    w_inv += N;
+  }
 }
 __global__ void scale_copy_kernel(const float* __restrict__ src, float* __restrict__ dst, int n, float scale) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -172,13 +181,37 @@ constexpr float S_ATT = 4.f;    // attention output            -> out_proj GEMM
 constexpr float S_GELU = 2.f;   // GELU(fc1) (ESM)             -> fc2 GEMM           (up to 224)
 constexpr float S_RELU2 = 1.f;  // relu(fc1)^2 (Tranception)   -> fc2 GEMM           (up to 448)
 
+// Operand formats of a precision mode (common.h fmt 0 / 1 / 2), fixed at pg_create. Pitches and offsets in fp16 elements.
+struct OpFmt {
+  int np = 1;    // operand row pitch in units of the fp16 hi plane: 1 (fp16) or 2 (hi | lo, or hi | e4m3 planes)
+  int nseg = 1;  // GEMM operand mode: 1 fp16, 3 fp16 hi/lo x3, 2 fp16 + e4m3 cross terms
+  int afmt = 0;  // GEMM inputs (LayerNorm, attention and fc1 outputs): 2 under nseg 2, else 1 when np == 2
+  int qfmt = 0;  // q/k/v rows, read by the attention kernels: fp16 hi [| lo]
+  int pseg = 1;  // nseg of the operands that are fp16 hi [| lo] in every mode (attention, the MSA tied GEMMs): 3 when np == 2
+  int64_t ldd = 0, ldf = 0, ldq = 0;  // pitches of d-, ffn- and 3d-wide rows
+  int64_t lo_d = 0, lo_q = 0;         // offset of the planes after the hi plane in d- and 3d-wide rows (0: none)
+};
+OpFmt op_fmt(const pg_model_desc& D) {
+  OpFmt o;
+  o.np = D.precision == PG_PREC_F16 ? 1 : 2;
+  o.nseg = D.precision == PG_PREC_F16 ? 1 : (D.precision == PG_PREC_F16F8 ? 2 : 3);  // F16D: the fp16 hi/lo x3 plumbing + delta GEMMs
+  o.afmt = o.nseg == 2 ? 2 : o.np - 1;
+  o.qfmt = o.np - 1;
+  o.pseg = o.np == 2 ? 3 : 1;
+  o.ldd = static_cast<int64_t>(D.embed_dim) * o.np;
+  o.ldf = static_cast<int64_t>(D.ffn_dim) * o.np;
+  o.ldq = 3 * o.ldd;
+  o.lo_d = o.np == 2 ? D.embed_dim : 0;
+  o.lo_q = 3 * o.lo_d;
+  return o;
+}
+
 }  // namespace
 }  // namespace pg
 
 struct pg_handle_s {
   pg_model_desc desc{};
-  int np = 1;    // operand row pitch in units of the fp16 hi plane: 1 (fp16) or 2 (hi | lo, or hi | e4m3 planes)
-  int nseg = 1;  // GEMM operand mode: 1 fp16, 3 fp16 hi/lo x3, 2 fp16 + e4m3 cross terms
+  pg::OpFmt op;
   bool loaded = false;
   std::string err;
   std::vector<void*> allocs;
@@ -216,7 +249,7 @@ struct pg_handle_s {
   // `allocs`) and the compact exact q/k/v rows of the masked positions
   bool delta = false;
   float* base = nullptr;
-  size_t base_floats = 0;  // bytes allocated for `base`
+  size_t base_alloc_bytes = 0;  // allocated for `base`
   int base_T = 0;
   __half* cq = nullptr;
 };
@@ -248,29 +281,96 @@ __global__ void row_select_kernel(const int32_t* positions, const int32_t* win_s
   sel[i] = tok - (win_start ? win_start[gp] : 0);
 }
 
-// One linear layer of the model: A in the handle's operand format (common.h: fmt 0 / 1 / 2 by precision mode).
-struct Lin {
-  const __half* a; int64_t lda; float a_scale;  // a_scale: scale of A's e4m3 planes (PG_PREC_F16F8)
-  const __half* w; const float* w_inv; const float* bias;
-  int M, N, K, epi;
-  __half* out = nullptr; int out_fmt = 0; float out_scale = 0.f;  // epi != 2
-  float* resid = nullptr;                                          // epi == 2
-};
-int run_lin(pg_handle h, int cat, const Lin& L, cudaStream_t s, int rot_T = 0) {
-  const int np = h->np;
+// ---- block helpers: every operand they write or read is in the handle's formats (h->op) ------------------------------------
+
+// ESM embedding of the copies [p_offset, p_offset + P) of a window of T tokens into h->x (force_mask_scale: see EmbedLaunch).
+int embed(pg_handle h, const int32_t* tokens, int n_tokens, const int32_t* positions, const int32_t* win_start, int p_offset, int P,
+          int T, cudaStream_t s, int force_mask_scale = 0) {
+  const pg_model_desc& D = h->desc;
+  EmbedLaunch e{};
+  e.tokens = tokens; e.n_tokens = n_tokens; e.positions = positions; e.win_start = win_start;
+  e.P = P; e.T = T; e.d = D.embed_dim; e.embed = h->embed; e.pos_table = h->pos;  // null for ESM2 (rotary)
+  e.lnb_gamma = D.emb_ln_before ? h->lnbg : nullptr; e.lnb_beta = D.emb_ln_before ? h->lnbb : nullptr;
+  e.token_dropout = D.token_dropout; e.mask_idx = 32; e.p_offset = p_offset; e.x = h->x; e.force_mask_scale = force_mask_scale;
+  ProfScope ps(CAT_EMBED, s);
+  return launch_embed(e, s);
+}
+
+// LayerNorm of M fp32 rows x (pitch d) into operand rows `out` in the GEMM-input format (perm_R / perm_C: launch_layernorm_f16).
+int ln(pg_handle h, const float* x, const float* g, const float* b, int M, __half* out, cudaStream_t s, int perm_R = 0, int perm_C = 0) {
+  const int d = h->desc.embed_dim;
+  ProfScope ps(CAT_LN, s);
+  return launch_layernorm_f16(x, d, g, b, M, d, out, h->op.ldd, h->op.lo_d, s, h->op.afmt, S_LN, perm_R, perm_C);
+}
+
+// The projections of a Layer, each profiled in its own GEMM category.
+enum Proj { QKV = CAT_GEMM_QKV, OUT = CAT_GEMM_OUT, FC1 = CAT_GEMM_FC1, FC2 = CAT_GEMM_FC2 };
+// Projection p of layer L on M operand rows `a` in the GEMM-input format (a_scale: the e4m3 scale their producer applied).
+GemmLaunch proj_gemm(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int M) {
+  const int d = h->desc.embed_dim, f = h->desc.ffn_dim;
   GemmLaunch g{};
-  g.a = L.a; g.lda = L.lda; g.w = L.w; g.ldw = static_cast<int64_t>(L.K) * np; g.bias = L.bias;
-  g.M = L.M; g.N = L.N; g.K = L.K; g.nseg = h->nseg; g.epi = L.epi;
-  g.a_scale = L.a_scale; g.w_inv = L.w_inv; g.w_uniform = 1;  // pg_load_weights: one e4m3 scale per (fused) weight matrix
-  if (L.epi == 2) {
-    g.resid = L.resid; g.ldr = L.N;
-  } else {
-    g.out = L.out; g.ldo = static_cast<int64_t>(L.N) * np; g.out_fmt = L.out_fmt; g.out_lo_off = L.out_fmt ? L.N : 0;
-    g.out_scale = L.out_scale;
+  switch (p) {
+    case QKV: g.w = L.wqkv; g.w_inv = L.iqkv; g.bias = L.bqkv; g.N = 3 * d; g.K = d; break;
+    case OUT: g.w = L.wo; g.w_inv = L.io; g.bias = L.bo; g.N = d; g.K = d; break;
+    case FC1: g.w = L.w1; g.w_inv = L.i1; g.bias = L.b1; g.N = f; g.K = d; break;
+    case FC2: g.w = L.w2; g.w_inv = L.i2; g.bias = L.b2; g.N = d; g.K = f; break;
   }
-  if (L.epi == 3) { g.rot_cos = h->rot_cos; g.rot_sin = h->rot_sin; g.rot_T = rot_T; g.rot_dim = h->desc.embed_dim; }
-  ProfScope ps(cat, s);
+  g.a = a; g.lda = static_cast<int64_t>(g.K) * h->op.np; g.ldw = g.lda; g.M = M; g.nseg = h->op.nseg;
+  g.a_scale = a_scale; g.w_uniform = 1;  // pg_load_weights: one e4m3 scale per (fused) weight matrix
+  return g;
+}
+// ... written as operand rows to `out` through epilogue `epi`: q/k/v in the q/k/v format (epi 0, or 3: rotary embedding over windows of
+// rot_T rows), fc1 in the GEMM-input format (epi: the MLP's activation, out_scale: the e4m3 scale of its output).
+int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int M, __half* out, cudaStream_t s, int epi = 0,
+        float out_scale = 0.f, int rot_T = 0) {
+  GemmLaunch g = proj_gemm(h, L, p, a, a_scale, M);
+  g.epi = epi;
+  g.out = out; g.ldo = static_cast<int64_t>(g.N) * h->op.np; g.out_fmt = p == QKV ? h->op.qfmt : h->op.afmt;
+  g.out_lo_off = g.out_fmt ? g.N : 0; g.out_scale = out_scale;
+  if (epi == 3) { g.rot_cos = h->rot_cos; g.rot_sin = h->rot_sin; g.rot_T = rot_T; g.rot_dim = h->desc.embed_dim; }
+  ProfScope ps(p, s);
   return launch_gemm(g, s);
+}
+// ... added into the fp32 rows `resid` (pitch N): out_proj and fc2 into the residual stream, and the base rows of the delta mode.
+int lin_add(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int M, float* resid, cudaStream_t s) {
+  GemmLaunch g = proj_gemm(h, L, p, a, a_scale, M);
+  g.epi = 2; g.resid = resid; g.ldr = g.N;
+  ProfScope ps(p, s);
+  return launch_gemm(g, s);
+}
+
+// MLP block on M fp32 residual rows x: x += fc2(act(fc1(LN2(x)))), through operand rows `ab` (LayerNorm output) and `fb` (hidden
+// layer). act: fc1's activation epilogue (1 GELU, 4 relu^2); act_scale: the e4m3 scale of its output (S_GELU, S_RELU2).
+int mlp(pg_handle h, const Layer& L, float* x, int M, __half* ab, __half* fb, int act, float act_scale, cudaStream_t s) {
+  int rc = ln(h, x, L.ln2g, L.ln2b, M, ab, s);
+  if (!rc) rc = lin(h, L, FC1, ab, S_LN, M, fb, s, act, act_scale);
+  if (!rc) rc = lin_add(h, L, FC2, fb, act_scale, M, x, s);
+  return rc;
+}
+
+// Attention over B sequences of T rows, q/k/v rows `qkv` -> operand rows `out` in the GEMM-input format; bidirectional and without
+// bias. The caller sets the causal / ALiBi / prefix / column (perm_C) / delta-operand fields.
+AttnLaunch attn_args(pg_handle h, const __half* qkv, __half* out, int B, int T) {
+  const OpFmt& o = h->op;
+  AttnLaunch a{};
+  a.qkv = qkv; a.ld = o.ldq; a.lo_off = o.lo_q;
+  a.out = out; a.ldo = o.ldd; a.out_lo_off = o.lo_d; a.out_fmt = o.afmt; a.out_scale = S_ATT;
+  a.B = B; a.T = T; a.heads = h->desc.heads; a.nseg = o.pseg; a.causal = 0; a.alibi_slopes = nullptr;
+  return a;
+}
+
+// Exact pruning of the final ESM layer, after its q/k/v projection into h->qkv: one query row per sequence (emit_rows[b] of sequence b)
+// from here on; out_proj and the MLP run on the Bc compact residual rows h->xc. `gather`: fill h->xc from h->x first (otherwise the
+// caller already holds those rows there).
+int last_layer(pg_handle h, const Layer& L, const int32_t* emit_rows, int Bc, int T, bool gather, cudaStream_t s) {
+  const OpFmt& o = h->op;
+  int rc;
+  { ProfScope ps(CAT_ATTN, s, gather ? 2 : 1);
+    rc = launch_attn_single_query(h->qkv, o.ldq, o.lo_q, emit_rows, Bc, T, h->desc.heads, h->cabuf, o.ldd, o.lo_d, s, o.afmt, S_ATT);
+    if (!rc && gather) rc = launch_gather_rows(h->x, emit_rows, Bc, T, h->desc.embed_dim, h->xc, s); }
+  if (!rc) rc = lin_add(h, L, OUT, h->cabuf, S_ATT, Bc, h->xc, s);
+  if (!rc) rc = mlp(h, L, h->xc, Bc, h->cabuf, h->cfbuf, 1, S_GELU, s);
+  return rc;
 }
 
 // `emit_rows` (device, [Bc]) = the one row per sequence the caller will read, or null when every row is needed. When given,
@@ -278,73 +378,20 @@ int run_lin(pg_handle h, int cat, const Lin& L, cudaStream_t s, int rot_T = 0) {
 int forward_rows(pg_handle h, const int32_t* tokens, int n_tokens, const int32_t* positions, const int32_t* win_start,
                  int p_offset, int Bc, int T, cudaStream_t s, const int32_t* emit_rows = nullptr) {
   const pg_model_desc& D = h->desc;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->np;
-  const int afmt = h->nseg == 2 ? 2 : (np == 2 ? 1 : 0);  // operand format of GEMM inputs
-  const int qfmt = np == 2 ? 1 : 0;                        // q/k/v for the attention kernel: fp16 hi [| lo]
-  const int64_t ldd = static_cast<int64_t>(d) * np, ldf = static_cast<int64_t>(f) * np, ldq = static_cast<int64_t>(3 * d) * np;
   const int rows = Bc * T;
-  EmbedLaunch e{};
-  e.tokens = tokens; e.n_tokens = n_tokens; e.positions = positions; e.win_start = win_start;
-  e.P = Bc; e.T = T; e.d = d; e.embed = h->embed; e.pos_table = (D.arch == PG_ARCH_ESM1B) ? h->pos : nullptr;
-  e.lnb_gamma = D.emb_ln_before ? h->lnbg : nullptr; e.lnb_beta = D.emb_ln_before ? h->lnbb : nullptr;
-  e.token_dropout = D.token_dropout; e.mask_idx = 32; e.p_offset = p_offset; e.x = h->x;
-  int rc;
-  { ProfScope ps(CAT_EMBED, s); rc = launch_embed(e, s); }
-  if (rc) return rc;
   const bool rotary = (D.arch == PG_ARCH_ESM2);
-  auto ln = [&](const float* x, const float* g, const float* b, int nrows, __half* out) {
-    ProfScope ps(CAT_LN, s);
-    return launch_layernorm_f16(x, d, g, b, nrows, d, out, ldd, np == 2 ? d : 0, s, afmt, S_LN);
-  };
+  int rc = embed(h, tokens, n_tokens, positions, win_start, p_offset, Bc, T, s);
+  if (rc) return rc;
   for (int l = 0; l < D.layers; ++l) {
     const Layer& L = h->layers[l];
-    rc = ln(h->x, L.ln1g, L.ln1b, rows, h->abuf);
+    if ((rc = ln(h, h->x, L.ln1g, L.ln1b, rows, h->abuf, s))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s, rotary ? 3 : 0, 0.f, T))) return rc;
+    if (emit_rows && l == D.layers - 1) return last_layer(h, L, emit_rows, Bc, T, true, s);
+    const AttnLaunch a = attn_args(h, h->qkv, h->abuf, Bc, T);
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
-    Lin q{h->abuf, ldd, S_LN, L.wqkv, L.iqkv, L.bqkv, rows, 3 * d, d, rotary ? 3 : 0};
-    q.out = h->qkv; q.out_fmt = qfmt;
-    rc = run_lin(h, CAT_GEMM_QKV, q, s, T);
-    if (rc) return rc;
-    if (emit_rows && l == D.layers - 1) {
-      // exact pruning of the final layer: one query row per sequence from here on
-      { ProfScope ps(CAT_ATTN, s, 2);
-        rc = launch_attn_single_query(h->qkv, ldq, np == 2 ? 3 * d : 0, emit_rows, Bc, T, D.heads, h->cabuf, ldd, np == 2 ? d : 0, s,
-                                      afmt, S_ATT);
-        if (!rc) rc = launch_gather_rows(h->x, emit_rows, Bc, T, d, h->xc, s); }
-      if (rc) return rc;
-      Lin o{h->cabuf, ldd, S_ATT, L.wo, L.io, L.bo, Bc, d, d, 2};
-      o.resid = h->xc;
-      rc = run_lin(h, CAT_GEMM_OUT, o, s);
-      if (rc) return rc;
-      rc = ln(h->xc, L.ln2g, L.ln2b, Bc, h->cabuf);
-      if (rc) return rc;
-      Lin f1{h->cabuf, ldd, S_LN, L.w1, L.i1, L.b1, Bc, f, d, 1};
-      f1.out = h->cfbuf; f1.out_fmt = afmt; f1.out_scale = S_GELU;
-      rc = run_lin(h, CAT_GEMM_FC1, f1, s);
-      if (rc) return rc;
-      Lin f2{h->cfbuf, ldf, S_GELU, L.w2, L.i2, L.b2, Bc, d, f, 2};
-      f2.resid = h->xc;
-      return run_lin(h, CAT_GEMM_FC2, f2, s);
-    }
-    AttnLaunch a{};
-    a.qkv = h->qkv; a.ld = ldq; a.lo_off = np == 2 ? 3 * d : 0;
-    a.out = h->abuf; a.ldo = ldd; a.out_lo_off = np == 2 ? d : 0; a.out_fmt = afmt; a.out_scale = S_ATT;
-    a.B = Bc; a.T = T; a.heads = D.heads; a.nseg = np == 2 ? 3 : 1; a.causal = 0; a.alibi_slopes = nullptr;
-    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_tc(a, s); }
-    if (rc) return rc;
-    Lin o{h->abuf, ldd, S_ATT, L.wo, L.io, L.bo, rows, d, d, 2};
-    o.resid = h->x;
-    rc = run_lin(h, CAT_GEMM_OUT, o, s);
-    if (rc) return rc;
-    rc = ln(h->x, L.ln2g, L.ln2b, rows, h->abuf);
-    if (rc) return rc;
-    Lin f1{h->abuf, ldd, S_LN, L.w1, L.i1, L.b1, rows, f, d, 1};
-    f1.out = h->fbuf; f1.out_fmt = afmt; f1.out_scale = S_GELU;
-    rc = run_lin(h, CAT_GEMM_FC1, f1, s);
-    if (rc) return rc;
-    Lin f2{h->fbuf, ldf, S_GELU, L.w2, L.i2, L.b2, rows, d, f, 2};
-    f2.resid = h->x;
-    rc = run_lin(h, CAT_GEMM_FC2, f2, s);
-    if (rc) return rc;
+    if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
+    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, 1, S_GELU, s))) return rc;
   }
   return PG_OK;
 }
@@ -361,16 +408,16 @@ int forward_rows(pg_handle h, const int32_t* tokens, int n_tokens, const int32_t
 //   base rows per layer, T rows each. Inputs of the four GEMMs, as ONE fp16 plane (any fixed reference works as long as the matching
 //   output rows were computed from exactly these values): a0 = rn16(LN1 output), o0 = rn16(attention output), b0 = rn16(LN2 output),
 //   f0 = rn16(GELU output). Their images, fp32: bqkv = Wqkv a0 + b, bout = Wo o0 + b, bfc1 = W1 b0 + b (pre-GELU), bfc2 = W2 f0 + b.
-struct BaseRows { const float *bqkv, *bout, *bfc1, *bfc2; const __half *a0, *o0, *b0, *f0; };
+struct BaseRows { float *bqkv, *bout, *bfc1, *bfc2; __half *a0, *o0, *b0, *f0; };
 size_t base_bytes(const pg_model_desc& D, int T) {
   const size_t d = D.embed_dim, f = D.ffn_dim;
   return static_cast<size_t>(D.layers) * T * (4 * (5 * d + f) + 2 * (3 * d + f));
 }
 BaseRows base_rows(pg_handle h, int l) {
   const long long T = h->base_T, d = h->desc.embed_dim, f = h->desc.ffn_dim;
-  const float* p = h->base + static_cast<long long>(l) * T * (5 * d + f);
-  const __half* q = reinterpret_cast<const __half*>(h->base + static_cast<long long>(h->desc.layers) * T * (5 * d + f)) +
-                    static_cast<long long>(l) * T * (3 * d + f);
+  float* p = h->base + static_cast<long long>(l) * T * (5 * d + f);
+  __half* q = reinterpret_cast<__half*>(h->base + static_cast<long long>(h->desc.layers) * T * (5 * d + f)) +
+              static_cast<long long>(l) * T * (3 * d + f);
   BaseRows b;
   b.bqkv = p; b.bout = p + T * 3 * d; b.bfc1 = p + T * 4 * d; b.bfc2 = p + T * (4 * d + f);
   b.a0 = q; b.o0 = q + T * d; b.b0 = q + T * 2 * d; b.f0 = q + T * 3 * d;
@@ -381,75 +428,48 @@ BaseRows base_rows(pg_handle h, int l) {
 // the base rows of every layer. Uses the pass workspace (T rows of it) before the passes start.
 int forward_base(pg_handle h, const int32_t* tokens, int n_tokens, int T, cudaStream_t s) {
   const pg_model_desc& D = h->desc;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->np;
-  const int64_t ldd = static_cast<int64_t>(d) * np, ldf = static_cast<int64_t>(f) * np, ldq = static_cast<int64_t>(3 * d) * np;
+  const OpFmt& o = h->op;
+  const int d = D.embed_dim, f = D.ffn_dim;
   const size_t need = base_bytes(D, T);
-  if (need > h->base_floats) {  // (base_floats counts bytes)
+  if (need > h->base_alloc_bytes) {
     if (h->base) cudaFree(h->base);
-    h->base = nullptr; h->base_floats = 0;
+    h->base = nullptr; h->base_alloc_bytes = 0;
     cudaError_t e = cudaMalloc(&h->base, need);
     if (e != cudaSuccess) return set_error(PG_ERR_CUDA, std::string("forward_base: cudaMalloc: ") + cudaGetErrorString(e));
-    h->base_floats = need;
+    h->base_alloc_bytes = need;
   }
   h->base_T = T;
   PG_CUDA_OK(cudaMemsetAsync(h->base, 0, need, s));  // the tap GEMMs reduce-add into zero
-  EmbedLaunch e{};
-  e.tokens = tokens; e.n_tokens = n_tokens; e.positions = nullptr; e.win_start = nullptr;
-  e.P = 1; e.T = T; e.d = d; e.embed = h->embed; e.pos_table = h->pos;
-  e.lnb_gamma = D.emb_ln_before ? h->lnbg : nullptr; e.lnb_beta = D.emb_ln_before ? h->lnbb : nullptr;
-  e.token_dropout = D.token_dropout; e.mask_idx = 32; e.p_offset = 0; e.x = h->x; e.force_mask_scale = 1;
-  int rc;
-  { ProfScope ps(CAT_EMBED, s); rc = launch_embed(e, s); }
+  int rc = embed(h, tokens, n_tokens, nullptr, nullptr, 0, 1, T, s, 1);
   if (rc) return rc;
-  auto ln = [&](const float* g, const float* b) {
-    ProfScope ps(CAT_LN, s);
-    return launch_layernorm_f16(h->x, d, g, b, T, d, h->abuf, ldd, d, s, 1, 0.f);
-  };
-  auto tap = [&](int cat, const __half* a, int64_t lda, const __half* w, const float* bias, int N, int K, const float* dst) {
-    Lin t{a, lda, 0.f, w, nullptr, bias, T, N, K, 2};
-    t.resid = const_cast<float*>(dst);
-    return run_lin(h, cat, t, s);
-  };
-  // The base row of a GEMM input is its fp16 hi plane: zero the lo plane of the T rows (the tap GEMM then multiplies exactly that
-  // plane by the full hi/lo weights) and keep a copy of the hi plane.
-  auto fix_base = [&](__half* buf, int64_t ld, int n, const __half* dst) -> int {
+  // The base row of a GEMM input is its fp16 hi plane: zero the lo plane of the T rows (the tap GEMM, lin_add into the base rows,
+  // then multiplies exactly that plane by the full hi/lo weights) and keep a copy of the hi plane.
+  auto fix_base = [&](__half* buf, int64_t ld, int n, __half* dst) -> int {
     ProfScope ps(CAT_OTHER, s);
     PG_CUDA_OK(cudaMemset2DAsync(buf + n, ld * 2, 0, static_cast<size_t>(n) * 2, T, s));
-    PG_CUDA_OK(cudaMemcpy2DAsync(const_cast<__half*>(dst), static_cast<size_t>(n) * 2, buf, ld * 2, static_cast<size_t>(n) * 2, T,
-                                 cudaMemcpyDeviceToDevice, s));
+    PG_CUDA_OK(cudaMemcpy2DAsync(dst, static_cast<size_t>(n) * 2, buf, ld * 2, static_cast<size_t>(n) * 2, T, cudaMemcpyDeviceToDevice, s));
     return PG_OK;
   };
   for (int l = 0; l < D.layers; ++l) {
     const Layer& L = h->layers[l];
     const BaseRows B = base_rows(h, l);
-    if ((rc = ln(L.ln1g, L.ln1b))) return rc;
-    Lin q{h->abuf, ldd, 0.f, L.wqkv, nullptr, L.bqkv, T, 3 * d, d, 0};
-    q.out = h->qkv; q.out_fmt = 1;
-    if ((rc = run_lin(h, CAT_GEMM_QKV, q, s))) return rc;
-    if ((rc = fix_base(h->abuf, ldd, d, B.a0))) return rc;
-    if ((rc = tap(CAT_GEMM_QKV, h->abuf, ldd, L.wqkv, L.bqkv, 3 * d, d, B.bqkv))) return rc;
-    AttnLaunch a{};
-    a.qkv = h->qkv; a.ld = ldq; a.lo_off = 3 * d;
-    a.out = h->abuf; a.ldo = ldd; a.out_lo_off = d; a.out_fmt = 1;
-    a.B = 1; a.T = T; a.heads = D.heads; a.nseg = 3; a.causal = 0; a.alibi_slopes = nullptr;
-    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_tc(a, s); }
+    if ((rc = ln(h, h->x, L.ln1g, L.ln1b, T, h->abuf, s))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, T, h->qkv, s))) return rc;
+    if ((rc = fix_base(h->abuf, o.ldd, d, B.a0))) return rc;
+    if ((rc = lin_add(h, L, QKV, h->abuf, S_LN, T, B.bqkv, s))) return rc;
+    const AttnLaunch a = attn_args(h, h->qkv, h->abuf, 1, T);
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
-    Lin o{h->abuf, ldd, 0.f, L.wo, nullptr, L.bo, T, d, d, 2};
-    o.resid = h->x;
-    if ((rc = run_lin(h, CAT_GEMM_OUT, o, s))) return rc;
-    if ((rc = fix_base(h->abuf, ldd, d, B.o0))) return rc;
-    if ((rc = tap(CAT_GEMM_OUT, h->abuf, ldd, L.wo, L.bo, d, d, B.bout))) return rc;
-    if ((rc = ln(L.ln2g, L.ln2b))) return rc;
-    Lin f1{h->abuf, ldd, 0.f, L.w1, nullptr, L.b1, T, f, d, 1};
-    f1.out = h->fbuf; f1.out_fmt = 1;
-    if ((rc = run_lin(h, CAT_GEMM_FC1, f1, s))) return rc;
-    if ((rc = fix_base(h->abuf, ldd, d, B.b0))) return rc;
-    if ((rc = tap(CAT_GEMM_FC1, h->abuf, ldd, L.w1, L.b1, f, d, B.bfc1))) return rc;
-    Lin f2{h->fbuf, ldf, 0.f, L.w2, nullptr, L.b2, T, d, f, 2};
-    f2.resid = h->x;
-    if ((rc = run_lin(h, CAT_GEMM_FC2, f2, s))) return rc;
-    if ((rc = fix_base(h->fbuf, ldf, f, B.f0))) return rc;
-    if ((rc = tap(CAT_GEMM_FC2, h->fbuf, ldf, L.w2, L.b2, d, f, B.bfc2))) return rc;
+    if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, T, h->x, s))) return rc;
+    if ((rc = fix_base(h->abuf, o.ldd, d, B.o0))) return rc;
+    if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, T, B.bout, s))) return rc;
+    if ((rc = ln(h, h->x, L.ln2g, L.ln2b, T, h->abuf, s))) return rc;
+    if ((rc = lin(h, L, FC1, h->abuf, S_LN, T, h->fbuf, s, 1, S_GELU))) return rc;
+    if ((rc = fix_base(h->abuf, o.ldd, d, B.b0))) return rc;
+    if ((rc = lin_add(h, L, FC1, h->abuf, S_LN, T, B.bfc1, s))) return rc;
+    if ((rc = lin_add(h, L, FC2, h->fbuf, S_GELU, T, h->x, s))) return rc;
+    if ((rc = fix_base(h->fbuf, o.ldf, f, B.f0))) return rc;
+    if ((rc = lin_add(h, L, FC2, h->fbuf, S_GELU, T, B.bfc2, s))) return rc;
   }
   return PG_OK;
 }
@@ -459,7 +479,7 @@ int run_lin_delta(pg_handle h, int cat, const __half* a, int64_t lda, const __ha
                   const __half* base_post, int T, const int32_t* mask_pos, __half* out, int64_t ldo, int out_fmt, float* resid,
                   cudaStream_t s) {
   GemmLaunch g{};
-  g.a = a; g.lda = lda; g.w = w; g.ldw = static_cast<int64_t>(K) * h->np; g.bias = nullptr;  // W: the hi plane of the hi/lo rows
+  g.a = a; g.lda = lda; g.w = w; g.ldw = static_cast<int64_t>(K) * h->op.np; g.bias = nullptr;  // W: the hi plane of the hi/lo rows
   g.M = M; g.N = N; g.K = K; g.nseg = 1; g.epi = epi;
   g.base_pre = base_pre; g.base_post = base_post; g.base_T = T; g.mask_pos = mask_pos;
   if (epi == 2) {
@@ -475,26 +495,18 @@ int run_lin_delta(pg_handle h, int cat, const __half* a, int64_t lda, const __ha
 int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const int32_t* positions, const int32_t* win_start,
                        int p_offset, int Bc, int T, cudaStream_t s, const int32_t* emit_rows) {
   const pg_model_desc& D = h->desc;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->np;
-  const int64_t ldd = static_cast<int64_t>(d) * np, ldf = static_cast<int64_t>(f) * np, ldq = static_cast<int64_t>(3 * d) * np;
+  const OpFmt& o = h->op;
+  const int d = D.embed_dim, f = D.ffn_dim;
   const int rows = Bc * T;
-  EmbedLaunch e{};
-  e.tokens = tokens; e.n_tokens = n_tokens; e.positions = positions; e.win_start = win_start;
-  e.P = Bc; e.T = T; e.d = d; e.embed = h->embed; e.pos_table = h->pos;
-  e.lnb_gamma = D.emb_ln_before ? h->lnbg : nullptr; e.lnb_beta = D.emb_ln_before ? h->lnbb : nullptr;
-  e.token_dropout = D.token_dropout; e.mask_idx = 32; e.p_offset = p_offset; e.x = h->x;
-  int rc;
-  { ProfScope ps(CAT_EMBED, s); rc = launch_embed(e, s); }
+  int rc = embed(h, tokens, n_tokens, positions, win_start, p_offset, Bc, T, s);
   if (rc) return rc;
   { ProfScope ps(CAT_OTHER, s); rc = launch_gather_rows(h->x, emit_rows, Bc, T, d, h->xc, s); }  // xc = the masked rows, kept exact
   if (rc) return rc;
+  // The masked rows (h->xc, through h->cabuf / h->cfbuf) take the compact exact path of the block helpers: in this mode their
+  // operand formats are the fp16 hi / lo pairs (fmt 1) and the e4m3 scales are unread.
   auto ln_delta = [&](const float* g, const float* b, const __half* base) {   // all rows: LN(x) - base[t] -> abuf (fp16, pitch ldd)
     ProfScope ps(CAT_LN, s);
-    return launch_layernorm_f16(h->x, d, g, b, rows, d, h->abuf, ldd, 0, s, 0, 0.f, 0, 0, base, T);
-  };
-  auto ln_compact = [&](const float* g, const float* b) {                     // masked rows: LN(xc) -> cabuf (hi | lo)
-    ProfScope ps(CAT_LN, s);
-    return launch_layernorm_f16(h->xc, d, g, b, Bc, d, h->cabuf, ldd, d, s, 1, 0.f);
+    return launch_layernorm_f16(h->x, d, g, b, rows, d, h->abuf, o.ldd, 0, s, 0, 0.f, 0, 0, base, T);
   };
   auto put_back = [&]() {                                                    // x[masked rows] <- xc
     ProfScope ps(CAT_OTHER, s);
@@ -505,55 +517,30 @@ int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const i
     const BaseRows B = base_rows(h, l);
     // q/k/v: all rows from the difference, the masked rows exactly
     if ((rc = ln_delta(L.ln1g, L.ln1b, B.a0))) return rc;
-    if ((rc = run_lin_delta(h, CAT_GEMM_QKV, h->abuf, ldd, L.wqkv, rows, 3 * d, d, 0, B.bqkv, nullptr, T, nullptr, h->qkv, ldq, 1, nullptr, s)))
+    if ((rc = run_lin_delta(h, CAT_GEMM_QKV, h->abuf, o.ldd, L.wqkv, rows, 3 * d, d, 0, B.bqkv, nullptr, T, nullptr, h->qkv, o.ldq, 1, nullptr, s)))
       return rc;
-    if ((rc = ln_compact(L.ln1g, L.ln1b))) return rc;
-    Lin cq{h->cabuf, ldd, 0.f, L.wqkv, nullptr, L.bqkv, Bc, 3 * d, d, 0};
-    cq.out = h->cq; cq.out_fmt = 1;
-    if ((rc = run_lin(h, CAT_GEMM_QKV, cq, s))) return rc;
+    if ((rc = ln(h, h->xc, L.ln1g, L.ln1b, Bc, h->cabuf, s))) return rc;
+    if ((rc = lin(h, L, QKV, h->cabuf, S_LN, Bc, h->cq, s))) return rc;
     { ProfScope ps(CAT_OTHER, s);
-      rc = launch_scatter_rows(h->cq, ldq * 2, h->qkv, ldq * 2, emit_rows, Bc, T, static_cast<int>(ldq * 2), s); }
+      rc = launch_scatter_rows(h->cq, o.ldq * 2, h->qkv, o.ldq * 2, emit_rows, Bc, T, static_cast<int>(o.ldq * 2), s); }
     if (rc) return rc;
-    if (l == D.layers - 1) {
-      // exact pruning of the final layer, as in forward_rows: one query row per copy from here on, x3 GEMMs on full values
-      { ProfScope ps(CAT_ATTN, s, 2);
-        rc = launch_attn_single_query(h->qkv, ldq, 3 * d, emit_rows, Bc, T, D.heads, h->cabuf, ldd, d, s, 1, 0.f); }
-      if (rc) return rc;
-      Lin o{h->cabuf, ldd, 0.f, L.wo, nullptr, L.bo, Bc, d, d, 2};
-      o.resid = h->xc;
-      if ((rc = run_lin(h, CAT_GEMM_OUT, o, s))) return rc;
-      if ((rc = ln_compact(L.ln2g, L.ln2b))) return rc;
-      Lin f1{h->cabuf, ldd, 0.f, L.w1, nullptr, L.b1, Bc, f, d, 1};
-      f1.out = h->cfbuf; f1.out_fmt = 1;
-      if ((rc = run_lin(h, CAT_GEMM_FC1, f1, s))) return rc;
-      Lin f2{h->cfbuf, ldf, 0.f, L.w2, nullptr, L.b2, Bc, d, f, 2};
-      f2.resid = h->xc;
-      return run_lin(h, CAT_GEMM_FC2, f2, s);
-    }
-    // attention on full-value q/k/v; output as difference rows, the masked rows' exact output to cabuf
-    AttnLaunch a{};
-    a.qkv = h->qkv; a.ld = ldq; a.lo_off = 3 * d;
-    a.out = h->abuf; a.ldo = ldd; a.out_lo_off = 0; a.out_fmt = 0;
-    a.B = Bc; a.T = T; a.heads = D.heads; a.nseg = 3; a.causal = 0; a.alibi_slopes = nullptr;
-    a.base_o = B.o0; a.mask_pos = emit_rows; a.cout = h->cabuf; a.ldc = ldd; a.c_lo_off = d;
-    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_tc(a, s); }
+    if (l == D.layers - 1) return last_layer(h, L, emit_rows, Bc, T, false, s);
+    // attention on full-value q/k/v; output as difference rows (one fp16 plane), the masked rows' exact output to cabuf
+    AttnLaunch a = attn_args(h, h->qkv, h->abuf, Bc, T);
+    a.out_lo_off = 0; a.out_fmt = 0;
+    a.base_o = B.o0; a.mask_pos = emit_rows; a.cout = h->cabuf; a.ldc = o.ldd; a.c_lo_off = d;
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
-    if ((rc = run_lin_delta(h, CAT_GEMM_OUT, h->abuf, ldd, L.wo, rows, d, d, 2, B.bout, nullptr, T, emit_rows, nullptr, 0, 0, h->x, s))) return rc;
-    Lin o{h->cabuf, ldd, 0.f, L.wo, nullptr, L.bo, Bc, d, d, 2};
-    o.resid = h->xc;
-    if ((rc = run_lin(h, CAT_GEMM_OUT, o, s))) return rc;
+    if ((rc = run_lin_delta(h, CAT_GEMM_OUT, h->abuf, o.ldd, L.wo, rows, d, d, 2, B.bout, nullptr, T, emit_rows, nullptr, 0, 0, h->x, s))) return rc;
+    if ((rc = lin_add(h, L, OUT, h->cabuf, S_ATT, Bc, h->xc, s))) return rc;
     if ((rc = put_back())) return rc;
     // MLP
     if ((rc = ln_delta(L.ln2g, L.ln2b, B.b0))) return rc;
-    if ((rc = run_lin_delta(h, CAT_GEMM_FC1, h->abuf, ldd, L.w1, rows, f, d, 1, B.bfc1, B.f0, T, nullptr, h->fbuf, ldf, 0, nullptr, s))) return rc;
-    if ((rc = ln_compact(L.ln2g, L.ln2b))) return rc;
-    Lin f1{h->cabuf, ldd, 0.f, L.w1, nullptr, L.b1, Bc, f, d, 1};
-    f1.out = h->cfbuf; f1.out_fmt = 1;
-    if ((rc = run_lin(h, CAT_GEMM_FC1, f1, s))) return rc;
-    if ((rc = run_lin_delta(h, CAT_GEMM_FC2, h->fbuf, ldf, L.w2, rows, d, f, 2, B.bfc2, nullptr, T, emit_rows, nullptr, 0, 0, h->x, s))) return rc;
-    Lin f2{h->cfbuf, ldf, 0.f, L.w2, nullptr, L.b2, Bc, d, f, 2};
-    f2.resid = h->xc;
-    if ((rc = run_lin(h, CAT_GEMM_FC2, f2, s))) return rc;
+    if ((rc = run_lin_delta(h, CAT_GEMM_FC1, h->abuf, o.ldd, L.w1, rows, f, d, 1, B.bfc1, B.f0, T, nullptr, h->fbuf, o.ldf, 0, nullptr, s))) return rc;
+    if ((rc = ln(h, h->xc, L.ln2g, L.ln2b, Bc, h->cabuf, s))) return rc;
+    if ((rc = lin(h, L, FC1, h->cabuf, S_LN, Bc, h->cfbuf, s, 1, S_GELU))) return rc;
+    if ((rc = run_lin_delta(h, CAT_GEMM_FC2, h->fbuf, o.ldf, L.w2, rows, d, f, 2, B.bfc2, nullptr, T, emit_rows, nullptr, 0, 0, h->x, s))) return rc;
+    if ((rc = lin_add(h, L, FC2, h->cfbuf, S_GELU, Bc, h->xc, s))) return rc;
     if ((rc = put_back())) return rc;
   }
   return PG_OK;
@@ -566,56 +553,31 @@ int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const i
 // wild type's: depthwise-conv look-back and the keys / values of the prefix come from the caches.
 int forward_tranception(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, int mode = 0, int start = 0) {
   const pg_model_desc& D = h->desc;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->np;
-  const int afmt = h->nseg == 2 ? 2 : (np == 2 ? 1 : 0);
-  const int qfmt = np == 2 ? 1 : 0;
-  const int64_t ldd = static_cast<int64_t>(d) * np, ldf = static_cast<int64_t>(f) * np, ldq = static_cast<int64_t>(3 * d) * np;
+  const int64_t ldq = h->op.ldq;
   const int rows = B * T;
   int rc;
-  { ProfScope ps(CAT_EMBED, s); rc = launch_gather_embed(ids, h->embed, rows, d, D.vocab, h->x, s); }
+  { ProfScope ps(CAT_EMBED, s); rc = launch_gather_embed(ids, h->embed, rows, D.embed_dim, D.vocab, h->x, s); }
   if (rc) return rc;
-  auto ln = [&](const float* g, const float* b) {
-    ProfScope ps(CAT_LN, s);
-    return launch_layernorm_f16(h->x, d, g, b, rows, d, h->abuf, ldd, np == 2 ? d : 0, s, afmt, S_LN);
-  };
   for (int l = 0; l < D.layers; ++l) {
     const Layer& L = h->layers[l];
-    rc = ln(L.ln1g, L.ln1b);
-    if (rc) return rc;
-    Lin q{h->abuf, ldd, S_LN, L.wqkv, L.iqkv, L.bqkv, rows, 3 * d, d, 0};
-    q.out = h->qkv; q.out_fmt = qfmt;
-    rc = run_lin(h, CAT_GEMM_QKV, q, s);
-    if (rc) return rc;
+    if ((rc = ln(h, h->x, L.ln1g, L.ln1b, rows, h->abuf, s))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s))) return rc;
     const size_t layer_off = static_cast<size_t>(l) * h->prefix_cap * ldq;
     if (mode == 1)
       PG_CUDA_OK(cudaMemcpyAsync(h->raw_cache + layer_off, h->qkv, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     { ProfScope ps(CAT_OTHER, s);
-      rc = launch_qkv_conv(h->qkv, h->qkv2, ldq, np == 2 ? 3 * d : 0, B, T, D.heads, L.conv_taps, 0.125f, s,
+      rc = launch_qkv_conv(h->qkv, h->qkv2, ldq, h->op.lo_q, B, T, D.heads, L.conv_taps, 0.125f, s,
                            mode == 2 ? h->raw_cache + layer_off + static_cast<size_t>(start - 6) * ldq : nullptr); }
     if (rc) return rc;
     if (mode == 1)
       PG_CUDA_OK(cudaMemcpyAsync(h->kv_cache + layer_off, h->qkv2, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
-    AttnLaunch a{};
-    a.qkv = h->qkv2; a.ld = ldq; a.lo_off = np == 2 ? 3 * d : 0;
-    a.out = h->abuf; a.ldo = ldd; a.out_lo_off = np == 2 ? d : 0; a.out_fmt = afmt; a.out_scale = S_ATT;
-    a.B = B; a.T = T; a.heads = D.heads; a.nseg = np == 2 ? 3 : 1; a.causal = 1; a.alibi_slopes = h->slopes;
+    AttnLaunch a = attn_args(h, h->qkv2, h->abuf, B, T);
+    a.causal = 1; a.alibi_slopes = h->slopes;
     if (mode == 2) { a.prefix = h->kv_cache + layer_off; a.prefix_len = start; }
-    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_tc(a, s); }
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
-    Lin o{h->abuf, ldd, S_ATT, L.wo, L.io, L.bo, rows, d, d, 2};
-    o.resid = h->x;
-    rc = run_lin(h, CAT_GEMM_OUT, o, s);
-    if (rc) return rc;
-    rc = ln(L.ln2g, L.ln2b);
-    if (rc) return rc;
-    Lin f1{h->abuf, ldd, S_LN, L.w1, L.i1, L.b1, rows, f, d, 4};
-    f1.out = h->fbuf; f1.out_fmt = afmt; f1.out_scale = S_RELU2;
-    rc = run_lin(h, CAT_GEMM_FC1, f1, s);
-    if (rc) return rc;
-    Lin f2{h->fbuf, ldf, S_RELU2, L.w2, L.i2, L.b2, rows, d, f, 2};
-    f2.resid = h->x;
-    rc = run_lin(h, CAT_GEMM_FC2, f2, s);
-    if (rc) return rc;
+    if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
+    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, 4, S_RELU2, s))) return rc;
   }
   return PG_OK;
 }
@@ -631,10 +593,8 @@ int forward_tranception(pg_handle h, const int32_t* ids, int B, int T, cudaStrea
 int forward_msa(pg_handle h, const int32_t* tokens, int R, int Cfull, const int32_t* positions, const int32_t* win_start, int p_offset,
                 int Bc, int Cw, cudaStream_t s, const int32_t* sel) {
   const pg_model_desc& D = h->desc;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->np, H = D.heads;
-  const int afmt = h->nseg == 2 ? 2 : (np == 2 ? 1 : 0);
-  const int qfmt = np == 2 ? 1 : 0;
-  const int64_t ldd = static_cast<int64_t>(d) * np, ldf = static_cast<int64_t>(f) * np, ldq = static_cast<int64_t>(3 * d) * np;
+  const OpFmt& o = h->op;
+  const int d = D.embed_dim, np = o.np, H = D.heads;
   const int rows = Bc * R * Cw;
   // tied-attention workspace: Q' / K' [G*Cp, Nt*np] (Q' doubles as the context buffer), V' [G*Nt, Kp*np], S fp32 [G*Cp, Kp], P [G*Cp, Kp*np]
   const int G = Bc * H, Cp = (Cw + 127) / 128 * 128, Kp = (Cw + 63) / 64 * 64, Nt = R * 64;
@@ -663,76 +623,44 @@ int forward_msa(pg_handle h, const int32_t* tokens, int R, int Cfull, const int3
   e.gamma = h->lnbg; e.beta = h->lnbb; e.mask_idx = 32; e.x = h->x;
   { ProfScope ps(CAT_EMBED, s); rc = launch_msa_embed(e, s); }
   if (rc) return rc;
-  auto ln = [&](const float* g, const float* b, int pR, int pC) {
-    ProfScope ps(CAT_LN, s);
-    return launch_layernorm_f16(h->x, d, g, b, rows, d, h->abuf, ldd, np == 2 ? d : 0, s, afmt, S_LN, pR, pC);
-  };
   const float row_scale = 1.0f / sqrtf(static_cast<float>(R));  // align_scaling (axial_attention.py:78-80); head_dim^-1/2 is in the weights
   for (int l = 0; l < D.layers; ++l) {
     const Layer& L = h->layers[l];
     const Layer& CL = h->col_layers[l];
     // ---- tied row attention
-    rc = ln(L.ln1g, L.ln1b, 0, 0);
-    if (rc) return rc;
-    Lin q{h->abuf, ldd, S_LN, L.wqkv, L.iqkv, L.bqkv, rows, 3 * d, d, 0};
-    q.out = h->qkv; q.out_fmt = qfmt;
-    rc = run_lin(h, CAT_GEMM_QKV, q, s);
-    if (rc) return rc;
+    if ((rc = ln(h, h->x, L.ln1g, L.ln1b, rows, h->abuf, s))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s))) return rc;
     if (l == D.layers - 1) {
       // ---- pruned last layer (exact)
       const int BR = Bc * R;
       uint8_t* fb = reinterpret_cast<uint8_t*>(h->fbuf);  // the MLP hidden buffer is idle here: compact residual / operand / q-k-v rows
       float* xr = reinterpret_cast<float*>(fb);
       __half* cab = reinterpret_cast<__half*>(fb + al(static_cast<size_t>(BR) * d * 4));
-      __half* cqkv = reinterpret_cast<__half*>(fb + al(static_cast<size_t>(BR) * d * 4) + al(static_cast<size_t>(BR) * ldd * 2));
+      __half* cqkv = reinterpret_cast<__half*>(fb + al(static_cast<size_t>(BR) * d * 4) + al(static_cast<size_t>(BR) * o.ldd * 2));
       { ProfScope ps(CAT_TIED, s, 3);
-        rc = launch_tied_col_attention(h->qkv, ldq, np == 2 ? 3 * d : 0, sel, Bc, R, Cw, H, row_scale, S, cab, ldd, np == 2 ? d : 0, afmt,
-                                       S_ATT, s); }
+        rc = launch_tied_col_attention(h->qkv, o.ldq, o.lo_q, sel, Bc, R, Cw, H, row_scale, S, cab, o.ldd, o.lo_d, o.afmt, S_ATT, s); }
       if (rc) return rc;
       { ProfScope ps(CAT_REGROUP, s);
         rc = launch_msa_gather_col(h->x, sel, Bc, R, Cw, d, xr, s); }
       if (rc) return rc;
-      Lin o{cab, ldd, S_ATT, L.wo, L.io, L.bo, BR, d, d, 2};
-      o.resid = xr;
-      rc = run_lin(h, CAT_GEMM_OUT, o, s);
+      if ((rc = lin_add(h, L, OUT, cab, S_ATT, BR, xr, s))) return rc;
+      if ((rc = ln(h, xr, CL.ln1g, CL.ln1b, BR, cab, s))) return rc;
+      if ((rc = lin(h, CL, QKV, cab, S_LN, BR, cqkv, s))) return rc;
+      const AttnLaunch a = attn_args(h, cqkv, cab, Bc, R);
+      { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
       if (rc) return rc;
-      { ProfScope ps(CAT_LN, s);
-        rc = launch_layernorm_f16(xr, d, CL.ln1g, CL.ln1b, BR, d, cab, ldd, np == 2 ? d : 0, s, afmt, S_LN); }
+      if ((rc = lin_add(h, CL, OUT, cab, S_ATT, BR, xr, s))) return rc;
+      rc = launch_gather_rows(xr, h->row_sel + h->head_cap, Bc, R, d, h->xc, s);  // row 0 of every alignment (counted by the head)
       if (rc) return rc;
-      Lin q2{cab, ldd, S_LN, CL.wqkv, CL.iqkv, CL.bqkv, BR, 3 * d, d, 0};
-      q2.out = cqkv; q2.out_fmt = qfmt;
-      rc = run_lin(h, CAT_GEMM_QKV, q2, s);
-      if (rc) return rc;
-      AttnLaunch a{};
-      a.qkv = cqkv; a.ld = ldq; a.lo_off = np == 2 ? 3 * d : 0;
-      a.out = cab; a.ldo = ldd; a.out_lo_off = np == 2 ? d : 0; a.out_fmt = afmt; a.out_scale = S_ATT;
-      a.B = Bc; a.T = R; a.heads = H; a.nseg = np == 2 ? 3 : 1; a.causal = 0; a.alibi_slopes = nullptr;
-      { ProfScope ps(CAT_ATTN, s); rc = launch_attention_tc(a, s); }
-      if (rc) return rc;
-      Lin o2{cab, ldd, S_ATT, CL.wo, CL.io, CL.bo, BR, d, d, 2};
-      o2.resid = xr;
-      rc = run_lin(h, CAT_GEMM_OUT, o2, s);
-      if (rc) return rc;
-      rc = launch_gather_rows(xr, h->row_sel + h->head_cap, Bc, R, d, h->xc, s);  // row 0 of every alignment
-      if (rc) return rc;
-      { ProfScope ps(CAT_LN, s);
-        rc = launch_layernorm_f16(h->xc, d, L.ln2g, L.ln2b, Bc, d, h->cabuf, ldd, np == 2 ? d : 0, s, afmt, S_LN); }
-      if (rc) return rc;
-      Lin f1{h->cabuf, ldd, S_LN, L.w1, L.i1, L.b1, Bc, f, d, 1};
-      f1.out = h->cfbuf; f1.out_fmt = afmt; f1.out_scale = S_GELU;
-      rc = run_lin(h, CAT_GEMM_FC1, f1, s);
-      if (rc) return rc;
-      Lin f2{h->cfbuf, ldf, S_GELU, L.w2, L.i2, L.b2, Bc, d, f, 2};
-      f2.resid = h->xc;
-      return run_lin(h, CAT_GEMM_FC2, f2, s);
+      return mlp(h, L, h->xc, Bc, h->cabuf, h->cfbuf, 1, S_GELU, s);
     }
     { ProfScope ps(CAT_REGROUP, s, 2);
-      rc = launch_tied_gather_qk(h->qkv, ldq, np == 2 ? 3 * d : 0, Bc, R, Cw, H, Cp, tq, tk, ldt, s);
-      if (!rc) rc = launch_tied_transpose_v(h->qkv, ldq, np == 2 ? 3 * d : 0, Bc, R, Cw, H, Kp, tv, ldv, s); }
+      rc = launch_tied_gather_qk(h->qkv, o.ldq, o.lo_q, Bc, R, Cw, H, Cp, tq, tk, ldt, s);
+      if (!rc) rc = launch_tied_transpose_v(h->qkv, o.ldq, o.lo_q, Bc, R, Cw, H, Kp, tv, ldv, s); }
     if (rc) return rc;
     PG_CUDA_OK(cudaMemsetAsync(S, 0, b_s, s));
     { GemmLaunch g{};
-      g.a = tq; g.lda = ldt; g.w = tk; g.ldw = ldt; g.M = G * Cp; g.N = Cw; g.K = Nt; g.nseg = np == 2 ? 3 : 1; g.epi = 2;
+      g.a = tq; g.lda = ldt; g.w = tk; g.ldw = ldt; g.M = G * Cp; g.N = Cw; g.K = Nt; g.nseg = o.pseg; g.epi = 2;
       g.resid = S; g.ldr = lds; g.grp_rows_a = Cp; g.grp_rows_b = Cp;
       ProfScope ps(CAT_TIED, s);
       rc = launch_gemm(g, s); }
@@ -741,47 +669,26 @@ int forward_msa(pg_handle h, const int32_t* tokens, int R, int Cfull, const int3
       rc = launch_tied_softmax(S, lds, G, Cw, Cp, Kp, row_scale, P, ldp, np, s); }
     if (rc) return rc;
     { GemmLaunch g{};
-      g.a = P; g.lda = ldp; g.w = tv; g.ldw = ldv; g.M = G * Cp; g.N = Nt; g.K = Kp; g.nseg = np == 2 ? 3 : 1; g.epi = 0;
-      g.out = tq; g.ldo = ldt; g.out_fmt = afmt; g.out_lo_off = afmt ? Nt : 0; g.out_scale = S_ATT;
+      g.a = P; g.lda = ldp; g.w = tv; g.ldw = ldv; g.M = G * Cp; g.N = Nt; g.K = Kp; g.nseg = o.pseg; g.epi = 0;
+      g.out = tq; g.ldo = ldt; g.out_fmt = o.afmt; g.out_lo_off = o.afmt ? Nt : 0; g.out_scale = S_ATT;
       g.grp_rows_a = Cp; g.grp_rows_b = Nt;
       ProfScope ps(CAT_TIED, s);
       rc = launch_gemm(g, s); }
     if (rc) return rc;
     { ProfScope ps(CAT_REGROUP, s);
-      rc = launch_tied_scatter_out(tq, ldt, h->abuf, ldd, afmt, Bc, R, Cw, H, Cp, s); }
+      rc = launch_tied_scatter_out(tq, ldt, h->abuf, o.ldd, o.afmt, Bc, R, Cw, H, Cp, s); }
     if (rc) return rc;
-    Lin o{h->abuf, ldd, S_ATT, L.wo, L.io, L.bo, rows, d, d, 2};
-    o.resid = h->x;
-    rc = run_lin(h, CAT_GEMM_OUT, o, s);
-    if (rc) return rc;
+    if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
     // ---- column attention: rows regrouped to (b, c, r) by the LayerNorm, back to (b, r, c) by the attention kernel
-    rc = ln(CL.ln1g, CL.ln1b, R, Cw);
+    if ((rc = ln(h, h->x, CL.ln1g, CL.ln1b, rows, h->abuf, s, R, Cw))) return rc;
+    if ((rc = lin(h, CL, QKV, h->abuf, S_LN, rows, h->qkv, s))) return rc;
+    AttnLaunch a = attn_args(h, h->qkv, h->abuf, Bc * Cw, R);
+    a.perm_C = Cw;
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
-    Lin q2{h->abuf, ldd, S_LN, CL.wqkv, CL.iqkv, CL.bqkv, rows, 3 * d, d, 0};
-    q2.out = h->qkv; q2.out_fmt = qfmt;
-    rc = run_lin(h, CAT_GEMM_QKV, q2, s);
-    if (rc) return rc;
-    AttnLaunch a{};
-    a.qkv = h->qkv; a.ld = ldq; a.lo_off = np == 2 ? 3 * d : 0;
-    a.out = h->abuf; a.ldo = ldd; a.out_lo_off = np == 2 ? d : 0; a.out_fmt = afmt; a.out_scale = S_ATT;
-    a.B = Bc * Cw; a.T = R; a.heads = H; a.nseg = np == 2 ? 3 : 1; a.causal = 0; a.alibi_slopes = nullptr; a.perm_C = Cw;
-    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_tc(a, s); }
-    if (rc) return rc;
-    Lin o2{h->abuf, ldd, S_ATT, CL.wo, CL.io, CL.bo, rows, d, d, 2};
-    o2.resid = h->x;
-    rc = run_lin(h, CAT_GEMM_OUT, o2, s);
-    if (rc) return rc;
+    if ((rc = lin_add(h, CL, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
     // ---- feed-forward
-    rc = ln(L.ln2g, L.ln2b, 0, 0);
-    if (rc) return rc;
-    Lin f1{h->abuf, ldd, S_LN, L.w1, L.i1, L.b1, rows, f, d, 1};
-    f1.out = h->fbuf; f1.out_fmt = afmt; f1.out_scale = S_GELU;
-    rc = run_lin(h, CAT_GEMM_FC1, f1, s);
-    if (rc) return rc;
-    Lin f2{h->fbuf, ldf, S_GELU, L.w2, L.i2, L.b2, rows, d, f, 2};
-    f2.resid = h->x;
-    rc = run_lin(h, CAT_GEMM_FC2, f2, s);
-    if (rc) return rc;
+    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, 1, S_GELU, s))) return rc;
   }
   return PG_OK;
 }
@@ -793,6 +700,48 @@ HeadLaunch head_args(pg_handle h, int T) {
   hl.ln_g = h->hlng; hl.ln_b = h->hlnb; hl.out_w = h->embed; hl.out_b = h->hbias; hl.vocab = h->desc.vocab;
   hl.scratch_a = h->hs_a; hl.scratch_b = h->hs_b;
   return hl;
+}
+
+// Sequences per pass: as many as the workspace holds, then evened out over the passes that needs — 512 copies of a 514-token window
+// against the default 131 072-row workspace are 171 + 171 + 170, not 255 + 255 + 2 (a 2-sequence pass pays all 33 layers' launch
+// latencies and partial waves for 0.4 % of the rows). Results do not depend on the split (rows are independent; tested).
+long long balanced_per(long long total, long long cap) {
+  if (cap < 1) cap = 1;
+  if (total <= cap) return total > 0 ? total : 1;
+  const long long passes = (total + cap - 1) / cap;
+  return (total + passes - 1) / passes;
+}
+
+// LM head on the Bc rows a pruned last layer left compacted in h->xc -> out [Bc, vocab]. `launches`: the head's own and the pass's
+// launches no other scope counts.
+int compact_head(pg_handle h, int T, int Bc, float* out, int launches, cudaStream_t s) {
+  ProfScope ps(CAT_HEAD, s, launches);
+  HeadLaunch hl = head_args(h, T);
+  hl.x = h->xc; hl.P = Bc; hl.all_rows = 1;
+  hl.out = out;
+  return launch_head(hl, s);
+}
+
+// The Tranception passes over B sequences of T rows (forward_tranception mode 0, or mode 2 after the recorded prefix at `start`), as
+// many sequences per pass as the workspace holds, each followed by the head on its rows.
+int ar_passes(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, int mode, int start, const ArFusion& fusion,
+              float* out_sum_logp, cudaStream_t s) {
+  const long long per = balanced_per(B, h->max_rows / T);
+  for (int b0 = 0; b0 < B; b0 += static_cast<int>(per)) {
+    const int Bc = (B - b0) < per ? (B - b0) : static_cast<int>(per);
+    const long long off = static_cast<long long>(b0) * T;
+    int rc = forward_tranception(h, ids + off, Bc, T, s, mode, start);
+    if (rc) return fail(h, rc, tls_error());
+    ProfScope ps(CAT_HEAD, s, 2);
+    ArFusion fc = fusion;
+    if (fc.prior_row) fc.prior_row += off;
+    if (fc.prior_row2) fc.prior_row2 += off;
+    if (fc.out_logprobs) fc.out_logprobs += off * h->desc.vocab;
+    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->lnag, h->lnab, h->embed, fc, h->tok_logp,
+                        out_sum_logp + b0, s);
+    if (rc) return fail(h, rc, tls_error());
+  }
+  return PG_OK;
 }
 
 }  // namespace
@@ -863,12 +812,11 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   if (prop.major != 9 || prop.minor != 0) return set_error(PG_ERR_UNSUPPORTED, "pg_create: device is not sm_90 (the kernels are built for sm_90a: wgmma, TMA)");
   pg_handle h = new pg_handle_s();
   h->desc = D;
-  h->np = (D.precision == PG_PREC_F16) ? 1 : 2;
-  h->nseg = (D.precision == PG_PREC_F16) ? 1 : (D.precision == PG_PREC_F16F8 ? 2 : 3);  // F16D: the fp16 hi/lo x3 plumbing + delta GEMMs
+  h->op = op_fmt(D);
   h->delta = (D.precision == PG_PREC_F16D);
   h->max_rows = D.max_rows > 0 ? D.max_rows : 131072;
   h->head_cap = 8192;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->np;
+  const int d = D.embed_dim, f = D.ffn_dim, np = h->op.np;
   int rc = PG_OK;
   auto A = [&](auto** p, size_t n) { if (!rc) rc = dev_alloc(h, p, n); };
   h->layers.resize(D.layers);
@@ -877,7 +825,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     A(&L.w1, static_cast<size_t>(f) * d * np); A(&L.w2, static_cast<size_t>(d) * f * np);
     A(&L.bqkv, 3 * d); A(&L.bo, d); A(&L.b1, f); A(&L.b2, d);
     A(&L.ln1g, d); A(&L.ln1b, d); A(&L.ln2g, d); A(&L.ln2b, d);
-    if (h->nseg == 2) { A(&L.iqkv, 3 * d); A(&L.io, d); A(&L.i1, f); A(&L.i2, d); }
+    if (h->op.nseg == 2) { A(&L.iqkv, 3 * d); A(&L.io, d); A(&L.i1, f); A(&L.i2, d); }
     if (D.arch == PG_ARCH_TRANCEPTION) A(&L.conv_taps, 3 * 4 * 64 * 8);
   }
   if (D.arch == PG_ARCH_MSA) {
@@ -885,7 +833,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     for (auto& L : h->col_layers) {
       A(&L.wqkv, static_cast<size_t>(3) * d * d * np); A(&L.wo, static_cast<size_t>(d) * d * np);
       A(&L.bqkv, 3 * d); A(&L.bo, d); A(&L.ln1g, d); A(&L.ln1b, d);
-      if (h->nseg == 2) { A(&L.iqkv, 3 * d); A(&L.io, d); }
+      if (h->op.nseg == 2) { A(&L.iqkv, 3 * d); A(&L.io, d); }
     }
     A(&h->row_pos, static_cast<size_t>(1024) * d);
   }
@@ -894,7 +842,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     A(&h->tok_logp, static_cast<size_t>(h->max_rows));
     A(&h->slopes, D.heads);
   }
-  if (h->nseg == 2) A(&h->pack_scratch, static_cast<size_t>(D.layers) * 6);
+  if (h->op.nseg == 2) A(&h->pack_scratch, static_cast<size_t>(D.layers) * 6);
   A(&h->embed, static_cast<size_t>(D.vocab) * d);
   if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA) A(&h->pos, static_cast<size_t>(D.max_positions + 2) * d);
   A(&h->lnbg, d); A(&h->lnbb, d); A(&h->lnag, d); A(&h->lnab, d);
@@ -934,7 +882,7 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
   if (!h || !tensors) return set_error(PG_ERR_ARG, "pg_load_weights: null argument");
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
   const pg_model_desc& D = h->desc;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->np;
+  const int d = D.embed_dim, f = D.ffn_dim, np = h->op.np;
   std::map<std::string, const pg_tensor*> by_name;
   for (int i = 0; i < n; ++i) by_name[tensors[i].name] = &tensors[i];
   std::string missing;
@@ -948,32 +896,26 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     if (!src) return;
     scale_copy_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256>>>(src, dst, static_cast<int>(cnt), scale);
   };
-  const bool f8 = h->nseg == 2;
-  // inv: where the per-row 1/t_n of this matrix go (PG_PREC_F16F8 only)
-  auto pack = [&](__half* dst, float* inv, const float* src, int N, int K, float scale = 1.f) {
-    if (!src) return;
-    const long long tot = static_cast<long long>(N) * K;
-    if (f8) launch_pack_weight_f8(src, N, K, K, 1, scale, h->pack_scratch + (h->pack_used++ % (D.layers * 6)), dst, inv, 0);
-    else pack_weight_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(src, N, K, scale, dst, np);
-  };
-  auto pack_t = [&](__half* dst, float* inv, const float* src, int N, int K) {
-    if (!src) return;
-    const long long tot = static_cast<long long>(N) * K;
-    if (f8) launch_pack_weight_f8(src, N, K, 1, N, 1.f, h->pack_scratch + (h->pack_used++ % (D.layers * 6)), dst, inv, 0);
-    else pack_weight_t_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(src, N, K, dst, np);
+  // A group of [N, K] weights that form one GEMM operand, packed into dst (inv: where the per-row 1/t of PG_PREC_F16F8 go).
+  // Conv1D weights are stored [in = K, out = N].
+  auto pack = [&](__half* dst, float* inv, std::initializer_list<PackSrc> group, int N, int K, bool conv1d = false) {
+    for (const PackSrc& m : group)
+      if (!m.w) return;
+    unsigned int* f8_scratch = h->op.nseg == 2 ? h->pack_scratch + (h->pack_used++ % (D.layers * 6)) : nullptr;
+    pack_weights(group, N, K, conv1d ? 1 : K, conv1d ? N : 1, np, f8_scratch, dst, inv, 0);
   };
   if (D.arch == PG_ARCH_TRANCEPTION) {
-    // HF GPT2-style names with the "transformer." prefix stripped by the host; Conv1D weights are [in, out].
+    // HF GPT2-style names with the "transformer." prefix stripped by the host
     for (int l = 0; l < D.layers; ++l) {
       Layer& L = h->layers[l];
       const std::string p = "h." + std::to_string(l) + ".";
-      pack_t(L.wqkv, L.iqkv, get(p + "attn.c_attn.weight", d, 3 * d), 3 * d, d);
+      pack(L.wqkv, L.iqkv, {get(p + "attn.c_attn.weight", d, 3 * d)}, 3 * d, d, true);
       copy(L.bqkv, get(p + "attn.c_attn.bias", 3 * d, 1), 3 * d);
-      pack_t(L.wo, L.io, get(p + "attn.c_proj.weight", d, d), d, d);
+      pack(L.wo, L.io, {get(p + "attn.c_proj.weight", d, d)}, d, d, true);
       copy(L.bo, get(p + "attn.c_proj.bias", d, 1), d);
-      pack_t(L.w1, L.i1, get(p + "mlp.c_fc.weight", d, f), f, d);
+      pack(L.w1, L.i1, {get(p + "mlp.c_fc.weight", d, f)}, f, d, true);
       copy(L.b1, get(p + "mlp.c_fc.bias", f, 1), f);
-      pack_t(L.w2, L.i2, get(p + "mlp.c_proj.weight", f, d), d, f);
+      pack(L.w2, L.i2, {get(p + "mlp.c_proj.weight", f, d)}, d, f, true);
       copy(L.b2, get(p + "mlp.c_proj.bias", d, 1), d);
       copy(L.ln1g, get(p + "ln_1.weight", d, 1), d);
       copy(L.ln1b, get(p + "ln_1.bias", d, 1), d);
@@ -985,98 +927,78 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     copy(h->lnag, get("ln_f.weight", d, 1), d);
     copy(h->lnab, get("ln_f.bias", d, 1), d);
     copy(h->slopes, get("alibi_slopes", D.heads, 1), D.heads);
-    if (!missing.empty()) return fail(h, PG_ERR_ARG, "pg_load_weights: missing or mis-shaped tensors: " + missing);
-    PG_CUDA_OK(cudaGetLastError());
-    PG_CUDA_OK(cudaDeviceSynchronize());
-    h->loaded = true;
-    return PG_OK;
-  }
-  const float qscale = 0.125f;  // head_dim^-1/2 with head_dim == 64 (multihead_attention.py:103,261); exact power of two
-  // one attention block: q/k/v/out projections at `pa` ("...self_attn." / "...row_self_attention.layer."), its LayerNorm at `pl`
-  auto load_attn = [&](Layer& L, const std::string& pa, const std::string& pl) {
-    const size_t dd = static_cast<size_t>(d) * d * np;
-    if (f8) {  // q, k, v form ONE GEMM operand: one common e4m3 scale (matrix maximum over the three, q already scaled)
+  } else {
+    const float qscale = 0.125f;  // head_dim^-1/2 with head_dim == 64 (multihead_attention.py:103,261); exact power of two
+    // one attention block: q/k/v/out projections at `pa` ("...self_attn." / "...row_self_attention.layer."), its LayerNorm at `pl`
+    auto load_attn = [&](Layer& L, const std::string& pa, const std::string& pl) {
+      // q, k, v form ONE GEMM operand: one common e4m3 scale (matrix maximum over the three, q already scaled)
       const float* wq = get(pa + "q_proj.weight", d, d);
       const float* wk = get(pa + "k_proj.weight", d, d);
       const float* wv = get(pa + "v_proj.weight", d, d);
-      if (wq && wk && wv) {
-        unsigned int* word = h->pack_scratch + (h->pack_used++ % (D.layers * 6));
-        const unsigned nb = static_cast<unsigned>((static_cast<long long>(d) * d + 255) / 256);
-        cudaMemsetAsync(word, 0, sizeof(unsigned int), 0);
-        weight_absmax_kernel<<<nb, 256>>>(wq, d, d, d, 1, qscale, word);
-        weight_absmax_kernel<<<nb, 256>>>(wk, d, d, d, 1, 1.f, word);
-        weight_absmax_kernel<<<nb, 256>>>(wv, d, d, d, 1, 1.f, word);
-        pack_weight_f8_kernel<<<(d + 7) / 8, 256>>>(wq, d, d, d, 1, qscale, word, L.wqkv, L.iqkv);
-        pack_weight_f8_kernel<<<(d + 7) / 8, 256>>>(wk, d, d, d, 1, 1.f, word, L.wqkv + dd, L.iqkv + d);
-        pack_weight_f8_kernel<<<(d + 7) / 8, 256>>>(wv, d, d, d, 1, 1.f, word, L.wqkv + 2 * dd, L.iqkv + 2 * d);
+      pack(L.wqkv, L.iqkv, {{wq, qscale}, wk, wv}, d, d);
+      copy(L.bqkv, get(pa + "q_proj.bias", d, 1), d, qscale);
+      copy(L.bqkv + d, get(pa + "k_proj.bias", d, 1), d);
+      copy(L.bqkv + 2 * d, get(pa + "v_proj.bias", d, 1), d);
+      pack(L.wo, L.io, {get(pa + "out_proj.weight", d, d)}, d, d);
+      copy(L.bo, get(pa + "out_proj.bias", d, 1), d);
+      copy(L.ln1g, get(pl + "weight", d, 1), d);
+      copy(L.ln1b, get(pl + "bias", d, 1), d);
+    };
+    auto load_ffn = [&](Layer& L, const std::string& pf, const std::string& pl) {
+      pack(L.w1, L.i1, {get(pf + "fc1.weight", f, d)}, f, d);
+      copy(L.b1, get(pf + "fc1.bias", f, 1), f);
+      pack(L.w2, L.i2, {get(pf + "fc2.weight", d, f)}, d, f);
+      copy(L.b2, get(pf + "fc2.bias", d, 1), d);
+      copy(L.ln2g, get(pl + "weight", d, 1), d);
+      copy(L.ln2b, get(pl + "bias", d, 1), d);
+    };
+    for (int l = 0; l < D.layers; ++l) {
+      const std::string p = "layers." + std::to_string(l) + ".";
+      if (D.arch == PG_ARCH_MSA) {  // AxialTransformerLayer (modules.py:194-196): three NormalizedResidualBlocks {layer, layer_norm}
+        load_attn(h->layers[l], p + "row_self_attention.layer.", p + "row_self_attention.layer_norm.");
+        load_attn(h->col_layers[l], p + "column_self_attention.layer.", p + "column_self_attention.layer_norm.");
+        load_ffn(h->layers[l], p + "feed_forward_layer.layer.", p + "feed_forward_layer.layer_norm.");
+      } else {
+        load_attn(h->layers[l], p + "self_attn.", p + "self_attn_layer_norm.");
+        load_ffn(h->layers[l], p, p + "final_layer_norm.");
       }
-    } else {
-      pack(L.wqkv, nullptr, get(pa + "q_proj.weight", d, d), d, d, qscale);
-      pack(L.wqkv + dd, nullptr, get(pa + "k_proj.weight", d, d), d, d);
-      pack(L.wqkv + 2 * dd, nullptr, get(pa + "v_proj.weight", d, d), d, d);
     }
-    copy(L.bqkv, get(pa + "q_proj.bias", d, 1), d, qscale);
-    copy(L.bqkv + d, get(pa + "k_proj.bias", d, 1), d);
-    copy(L.bqkv + 2 * d, get(pa + "v_proj.bias", d, 1), d);
-    pack(L.wo, L.io, get(pa + "out_proj.weight", d, d), d, d);
-    copy(L.bo, get(pa + "out_proj.bias", d, 1), d);
-    copy(L.ln1g, get(pl + "weight", d, 1), d);
-    copy(L.ln1b, get(pl + "bias", d, 1), d);
-  };
-  auto load_ffn = [&](Layer& L, const std::string& pf, const std::string& pl) {
-    pack(L.w1, L.i1, get(pf + "fc1.weight", f, d), f, d);
-    copy(L.b1, get(pf + "fc1.bias", f, 1), f);
-    pack(L.w2, L.i2, get(pf + "fc2.weight", d, f), d, f);
-    copy(L.b2, get(pf + "fc2.bias", d, 1), d);
-    copy(L.ln2g, get(pl + "weight", d, 1), d);
-    copy(L.ln2b, get(pl + "bias", d, 1), d);
-  };
-  for (int l = 0; l < D.layers; ++l) {
-    const std::string p = "layers." + std::to_string(l) + ".";
-    if (D.arch == PG_ARCH_MSA) {  // AxialTransformerLayer (modules.py:194-196): three NormalizedResidualBlocks {layer, layer_norm}
-      load_attn(h->layers[l], p + "row_self_attention.layer.", p + "row_self_attention.layer_norm.");
-      load_attn(h->col_layers[l], p + "column_self_attention.layer.", p + "column_self_attention.layer_norm.");
-      load_ffn(h->layers[l], p + "feed_forward_layer.layer.", p + "feed_forward_layer.layer_norm.");
-    } else {
-      load_attn(h->layers[l], p + "self_attn.", p + "self_attn_layer_norm.");
-      load_ffn(h->layers[l], p, p + "final_layer_norm.");
+    if (D.arch == PG_ARCH_MSA) {
+      auto it = by_name.find("msa_position_embedding");  // host-expanded to [1024, d] (the first release stores a 1-wide table)
+      if (it != by_name.end()) {
+        if (it->second->shape[0] != 1024 || it->second->shape[1] != d) missing += "msa_position_embedding(shape) ";
+        else copy(h->row_pos, static_cast<const float*>(it->second->data), static_cast<size_t>(1024) * d);
+      } else {
+        h->row_pos = nullptr;  // embed_positions_msa off (msa_transformer.py:106-114)
+      }
     }
-  }
-  if (D.arch == PG_ARCH_MSA) {
-    auto it = by_name.find("msa_position_embedding");  // host-expanded to [1024, d] (the first release stores a 1-wide table)
-    if (it != by_name.end()) {
-      if (it->second->shape[0] != 1024 || it->second->shape[1] != d) missing += "msa_position_embedding(shape) ";
-      else copy(h->row_pos, static_cast<const float*>(it->second->data), static_cast<size_t>(1024) * d);
-    } else {
-      h->row_pos = nullptr;  // embed_positions_msa off (msa_transformer.py:106-114)
+    copy(h->embed, get("embed_tokens.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA)
+      copy(h->pos, get("embed_positions.weight", D.max_positions + 2, d), static_cast<size_t>(D.max_positions + 2) * d);
+    if (D.emb_ln_before || D.arch == PG_ARCH_MSA) {
+      copy(h->lnbg, get("emb_layer_norm_before.weight", d, 1), d);
+      copy(h->lnbb, get("emb_layer_norm_before.bias", d, 1), d);
     }
-  }
-  copy(h->embed, get("embed_tokens.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-  if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA)
-    copy(h->pos, get("embed_positions.weight", D.max_positions + 2, d), static_cast<size_t>(D.max_positions + 2) * d);
-  if (D.emb_ln_before || D.arch == PG_ARCH_MSA) {
-    copy(h->lnbg, get("emb_layer_norm_before.weight", d, 1), d);
-    copy(h->lnbb, get("emb_layer_norm_before.bias", d, 1), d);
-  }
-  copy(h->lnag, get("emb_layer_norm_after.weight", d, 1), d);
-  copy(h->lnab, get("emb_layer_norm_after.bias", d, 1), d);
-  copy(h->hdw, get("lm_head.dense.weight", d, d), static_cast<size_t>(d) * d);
-  copy(h->hdb, get("lm_head.dense.bias", d, 1), d);
-  copy(h->hlng, get("lm_head.layer_norm.weight", d, 1), d);
-  copy(h->hlnb, get("lm_head.layer_norm.bias", d, 1), d);
-  copy(h->hbias, get("lm_head.bias", D.vocab, 1), D.vocab);
-  if (D.arch == PG_ARCH_ESM2) {
-    auto it = by_name.find("rotary.cos");
-    auto is = by_name.find("rotary.sin");
-    if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != 32 || is->second->shape[0] != it->second->shape[0]) {
-      missing += "rotary.cos/rotary.sin[T,32] ";
-    } else {
-      h->rot_rows = static_cast<int>(it->second->shape[0]);
-      int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
-      if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
-      if (rc) return rc;
-      copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * 32);
-      copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * 32);
+    copy(h->lnag, get("emb_layer_norm_after.weight", d, 1), d);
+    copy(h->lnab, get("emb_layer_norm_after.bias", d, 1), d);
+    copy(h->hdw, get("lm_head.dense.weight", d, d), static_cast<size_t>(d) * d);
+    copy(h->hdb, get("lm_head.dense.bias", d, 1), d);
+    copy(h->hlng, get("lm_head.layer_norm.weight", d, 1), d);
+    copy(h->hlnb, get("lm_head.layer_norm.bias", d, 1), d);
+    copy(h->hbias, get("lm_head.bias", D.vocab, 1), D.vocab);
+    if (D.arch == PG_ARCH_ESM2) {
+      auto it = by_name.find("rotary.cos");
+      auto is = by_name.find("rotary.sin");
+      if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != 32 || is->second->shape[0] != it->second->shape[0]) {
+        missing += "rotary.cos/rotary.sin[T,32] ";
+      } else {
+        h->rot_rows = static_cast<int>(it->second->shape[0]);
+        int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
+        if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
+        if (rc) return rc;
+        copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * 32);
+        copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * 32);
+      }
     }
   }
   if (!missing.empty()) return fail(h, PG_ERR_ARG, "pg_load_weights: missing or mis-shaped tensors: " + missing);
@@ -1084,16 +1006,6 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
   PG_CUDA_OK(cudaDeviceSynchronize());  // caller may free its tensors on return
   h->loaded = true;
   return PG_OK;
-}
-
-// Sequences per pass: as many as the workspace holds, then evened out over the passes that needs — 512 copies of a 514-token window
-// against the default 131 072-row workspace are 171 + 171 + 170, not 255 + 255 + 2 (a 2-sequence pass pays all 33 layers' launch
-// latencies and partial waves for 0.4 % of the rows). Results do not depend on the split (rows are independent; tested).
-static long long balanced_per(long long total, long long cap) {
-  if (cap < 1) cap = 1;
-  if (total <= cap) return total > 0 ? total : 1;
-  const long long passes = (total + cap - 1) / cap;
-  return (total + passes - 1) / passes;
 }
 
 int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, const int32_t* positions, const int32_t* win_start,
@@ -1125,11 +1037,7 @@ int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, co
     int rc = delta ? forward_rows_delta(h, tokens, n_tokens, positions, win_start, p0, Bc, T, s, h->row_sel)
                    : forward_rows(h, tokens, n_tokens, positions, win_start, p0, Bc, T, s, h->row_sel);
     if (rc) return fail(h, rc, tls_error());
-    ProfScope ps(CAT_HEAD, s, 4);
-    HeadLaunch hl = head_args(h, T);
-    hl.x = h->xc; hl.P = Bc; hl.all_rows = 1;  // the pruned last layer left exactly the rows to emit, compacted
-    hl.out = out_logprobs + static_cast<long long>(p0) * h->desc.vocab;
-    rc = launch_head(hl, s);
+    rc = compact_head(h, T, Bc, out_logprobs + static_cast<long long>(p0) * h->desc.vocab, 4, s);  // + row_select_kernel
     if (rc) return fail(h, rc, tls_error());
   }
   return PG_OK;
@@ -1157,11 +1065,7 @@ int pg_msa_masked_marginals(pg_handle h, const int32_t* tokens, int32_t R, int32
     row_select_kernel<<<(Bc + 255) / 256, 256, 0, s>>>(positions, win_start, nullptr, p0, Bc, h->row_sel);
     int rc = forward_msa(h, tokens, R, C_full, positions, win_start, p0, Bc, Cw, s, h->row_sel);
     if (rc) return fail(h, rc, tls_error());
-    ProfScope ps(CAT_HEAD, s, 5);
-    HeadLaunch hl = head_args(h, 1);
-    hl.x = h->xc; hl.P = Bc; hl.all_rows = 1;
-    hl.out = out_logprobs + static_cast<long long>(p0) * h->desc.vocab;
-    rc = launch_head(hl, s);
+    rc = compact_head(h, 1, Bc, out_logprobs + static_cast<long long>(p0) * h->desc.vocab, 5, s);  // + row_select_kernel, row-0 gather
     if (rc) return fail(h, rc, tls_error());
   }
   return PG_OK;
@@ -1220,24 +1124,7 @@ int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int
   if (T > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_ar_loglik: sequence longer than n_ctx");
   if (T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_ar_loglik: sequence longer than workspace");
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const long long per = balanced_per(B, h->max_rows / T);
-  for (int b0 = 0; b0 < B; b0 += static_cast<int>(per)) {
-    const int Bc = (B - b0) < per ? (B - b0) : static_cast<int>(per);
-    const long long off = static_cast<long long>(b0) * T;
-    const int32_t* idc = ids + off;
-    int rc = forward_tranception(h, idc, Bc, T, s);
-    if (rc) return fail(h, rc, tls_error());
-    ProfScope ps(CAT_HEAD, s, 2);
-    ArFusion fc = base;
-    if (fc.prior_row) fc.prior_row += off;
-    if (fc.prior_row2) fc.prior_row2 += off;
-    if (fc.out_logprobs) fc.out_logprobs += off * h->desc.vocab;
-    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, idc, lens + b0, h->lnag, h->lnab, h->embed, fc, h->tok_logp,
-                        out_sum_logp + b0, s);
-    if (rc) return fail(h, rc, tls_error());
-  }
-  return PG_OK;
+  return ar_passes(h, ids, lens, B, T, 0, 0, base, out_sum_logp, static_cast<cudaStream_t>(stream));
 }
 
 int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_fusion* f, float* out_tok_logp, pg_stream stream) {
@@ -1251,7 +1138,7 @@ int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_f
   if (rc) return rc;
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const size_t ldq = static_cast<size_t>(3) * h->desc.embed_dim * h->np;
+  const size_t ldq = static_cast<size_t>(h->op.ldq);
   if (h->prefix_cap < h->desc.max_positions) {  // first use: [layers][n_ctx][3d*np] fp16, twice
     const size_t n = static_cast<size_t>(h->desc.layers) * h->desc.max_positions * ldq;
     rc = dev_alloc(h, &h->raw_cache, n);
@@ -1288,23 +1175,7 @@ int pg_ar_loglik_prefix(pg_handle h, const int32_t* ids, const int32_t* lens, in
   int rc = ar_fusion_args(h, f, &base);
   if (rc) return rc;
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const long long per = balanced_per(B, h->max_rows / T);
-  for (int b0 = 0; b0 < B; b0 += static_cast<int>(per)) {
-    const int Bc = (B - b0) < per ? (B - b0) : static_cast<int>(per);
-    const long long off = static_cast<long long>(b0) * T;
-    rc = forward_tranception(h, ids + off, Bc, T, s, 2, start);
-    if (rc) return fail(h, rc, tls_error());
-    ProfScope ps(CAT_HEAD, s, 2);
-    ArFusion fc = base;
-    if (fc.prior_row) fc.prior_row += off;
-    if (fc.prior_row2) fc.prior_row2 += off;
-    if (fc.out_logprobs) fc.out_logprobs += off * h->desc.vocab;
-    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->lnag, h->lnab, h->embed, fc, h->tok_logp,
-                        out_sum_logp + b0, s);
-    if (rc) return fail(h, rc, tls_error());
-  }
-  return PG_OK;
+  return ar_passes(h, ids, lens, B, T, 2, start, base, out_sum_logp, static_cast<cudaStream_t>(stream));
 }
 
 int pg_ar_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, const float* log_prior,
@@ -1357,7 +1228,6 @@ int pg_layernorm_f16(const float* x, int64_t ldx, const float* gamma, const floa
 int pg_pack_weight(const float* w, int32_t N, int32_t K, int32_t fmt, void* out, float* w_inv, pg_stream stream) {
   if (!w || !out || N <= 0 || K <= 0) return set_error(PG_ERR_ARG, "pg_pack_weight: bad arguments");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const long long tot = static_cast<long long>(N) * K;
   if (fmt == 2) {
     if (!w_inv) return set_error(PG_ERR_ARG, "pg_pack_weight: fmt 2 needs w_inv[N]");
     // the matrix maximum is accumulated in w_inv[0]'s storage (as bits) before the pack kernel overwrites it with 1 / t... a separate
@@ -1367,9 +1237,9 @@ int pg_pack_weight(const float* w, int32_t N, int32_t K, int32_t fmt, void* out,
     PG_CUDA_OK(cudaGetDevice(&dev));
     if (dev >= 64) return set_error(PG_ERR_UNSUPPORTED, "pg_pack_weight: device ordinal >= 64");
     if (!scratch[dev]) PG_CUDA_OK(cudaMalloc(&scratch[dev], 256));
-    launch_pack_weight_f8(w, N, K, K, 1, 1.f, scratch[dev], static_cast<__half*>(out), w_inv, s);
+    pack_weights({w}, N, K, K, 1, 2, scratch[dev], static_cast<__half*>(out), w_inv, s);
   } else if (fmt == 0 || fmt == 1) {
-    pack_weight_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, s>>>(w, N, K, 1.f, static_cast<__half*>(out), fmt + 1);
+    pack_weights({w}, N, K, K, 1, fmt + 1, nullptr, static_cast<__half*>(out), nullptr, s);
   } else {
     return set_error(PG_ERR_ARG, "pg_pack_weight: fmt must be 0, 1 or 2");
   }
@@ -1387,7 +1257,7 @@ int pg_attention(const pg_attn_args* a, pg_stream stream) {
   l.base_o = static_cast<const __half*>(a->base_o); l.mask_pos = a->mask_pos; l.cout = static_cast<__half*>(a->cout); l.ldc = a->ldc; l.c_lo_off = a->c_lo_off;
   if ((l.base_o || l.mask_pos) && a->impl != 0) return set_error(PG_ERR_UNSUPPORTED, "pg_attention: the delta-operand form needs impl 0");
   ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream));
-  if (a->impl == 0) return launch_attention_tc(l, static_cast<cudaStream_t>(stream));   // the model's kernel (wgmma)
+  if (a->impl == 0) return launch_attention_wgmma(l, static_cast<cudaStream_t>(stream));   // the model's kernel
   if (a->impl != 1) return set_error(PG_ERR_ARG, "pg_attention: impl must be 0 (the model's wgmma kernel) or 1 (mma.sync cross-check)");
   if (l.out_fmt == 2) return set_error(PG_ERR_UNSUPPORTED, "pg_attention: the mma.sync cross-check kernel writes fp16 planes only");
   return launch_attention(l, static_cast<cudaStream_t>(stream));

@@ -142,8 +142,7 @@ int make_tmap_f16_2d(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t co
 // General form: elem_bytes 2 (fp16) / 4 (fp32) / 1 (bytes), swizzle 128 or 64 bytes. Encoded maps are cached per host thread.
 int make_tmap_2d(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t box_cols,
                  int elem_bytes, int swizzle);
-int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s);  // wgmma/TMA attention, 64-query x 64-key blocks (attention_wgmma.cu)
-int launch_attention_tc(const AttnLaunch& a, cudaStream_t s);     // the model's attention (attention_wgmma.cu)
+int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s);  // the model's attention: wgmma/TMA, 64-query x 64-key blocks
 }  // namespace pg
 
 namespace pg {

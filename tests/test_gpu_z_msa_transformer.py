@@ -1,6 +1,6 @@
 """GPU (-m gpu): the MSA Transformer path (tied row attention as grouped wgmma GEMMs, column attention through the wgmma attention
 kernel, pg_msa_masked_marginals) against golden vectors of the unmodified reference and the CPU oracle. Tolerance: 1e-3 abs per mutant
-score in the parity modes (north_star's bar)."""
+score in the parity modes (north_star's bar); f16 is held to the bound of tests/test_gpu_z_msa_fp64.py."""
 import os
 import subprocess
 import sys
@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from conftest import ROOT
+from msa_fp64_cases import BOUND
 from msa_transformer_cases import case_dir, have, load_case
 from oracle import msa_oracle as MO
 from proteingym_b200 import _lib, checkpoint, msa_engine, synth
@@ -39,8 +40,8 @@ def test_golden_table_and_scores(name, precision):
     sc.close()
     et, es = np.abs(tab - c["table"]).max(), np.abs(got - c["df"][col].to_numpy()).max()
     print(f"\nMSA Transformer {name} {precision}: max|dlogp|={et:.2e} max|dscore|={es:.2e}")
-    if precision == "f16":
-        assert es < 0.2
+    if precision == "f16":  # a score is a difference of two log-probs
+        assert et < BOUND["f16"] and es < 2 * BOUND["f16"]
     else:
         assert et < TOL and es < TOL
 

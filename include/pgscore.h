@@ -50,7 +50,7 @@ typedef struct {
   int32_t arch;            /* pg_arch */
   int32_t layers;          /* args.layers / cfg.encoder_layers */
   int32_t embed_dim;       /* args.embed_dim */
-  int32_t heads;           /* args.attention_heads; head_dim must be 64 */
+  int32_t heads;           /* args.attention_heads; head_dim = embed_dim / heads must be 64, except ESM2: any even head_dim <= 64 */
   int32_t ffn_dim;         /* args.ffn_embed_dim (ESM2: 4*embed_dim, esm2.py:52) */
   int32_t vocab;           /* 33 */
   int32_t max_positions;   /* learned-position table rows - 2 (ESM-1b: 1024) */

@@ -1,4 +1,5 @@
 // C-ABI of libpgscore.so (include/pgscore.h): model handle, weight repacking, and the batched masked-marginal forward.
+#include <cmath>
 #include <cstdlib>
 #include <map>
 #include <mutex>
@@ -182,14 +183,17 @@ constexpr float S_GELU = 2.f;   // GELU(fc1) (ESM)             -> fc2 GEMM      
 constexpr float S_RELU2 = 1.f;  // relu(fc1)^2 (Tranception)   -> fc2 GEMM           (up to 448)
 
 // Operand formats of a precision mode (common.h fmt 0 / 1 / 2), fixed at pg_create. Pitches and offsets in fp16 elements.
+// Widths (DESIGN.md §3): residual rows d; GEMM-input rows of width d (LayerNorm outputs) dk = d rounded up to 64, zero-padded; q/k/v
+// and attention outputs da = heads * 64, head h in the slot [64h, 64h + 64), zeros after its head_dim columns. All d for hd 64.
 struct OpFmt {
   int np = 1;    // operand row pitch in units of the fp16 hi plane: 1 (fp16) or 2 (hi | lo, or hi | e4m3 planes)
   int nseg = 1;  // GEMM operand mode: 1 fp16, 3 fp16 hi/lo x3, 2 fp16 + e4m3 cross terms
   int afmt = 0;  // GEMM inputs (LayerNorm, attention and fc1 outputs): 2 under nseg 2, else 1 when np == 2
   int qfmt = 0;  // q/k/v rows, read by the attention kernels: fp16 hi [| lo]
   int pseg = 1;  // nseg of the operands that are fp16 hi [| lo] in every mode (attention, the MSA tied GEMMs): 3 when np == 2
-  int64_t ldd = 0, ldf = 0, ldq = 0;  // pitches of d-, ffn- and 3d-wide rows
-  int64_t lo_d = 0, lo_q = 0;         // offset of the planes after the hi plane in d- and 3d-wide rows (0: none)
+  int dk = 0, da = 0;                          // plane widths of GEMM-input rows of width d, and of attention rows (see above)
+  int64_t ldd = 0, ldf = 0, ldat = 0, ldq = 0;  // pitches of dk-, ffn-, da- and 3da-wide rows
+  int64_t lo_d = 0, lo_at = 0, lo_q = 0;        // offset of the planes after the hi plane in dk-, da- and 3da-wide rows (0: none)
 };
 OpFmt op_fmt(const pg_model_desc& D) {
   OpFmt o;
@@ -198,12 +202,38 @@ OpFmt op_fmt(const pg_model_desc& D) {
   o.afmt = o.nseg == 2 ? 2 : o.np - 1;
   o.qfmt = o.np - 1;
   o.pseg = o.np == 2 ? 3 : 1;
-  o.ldd = static_cast<int64_t>(D.embed_dim) * o.np;
+  o.dk = (D.embed_dim + 63) / 64 * 64;
+  o.da = D.heads * 64;
+  o.ldd = static_cast<int64_t>(o.dk) * o.np;
   o.ldf = static_cast<int64_t>(D.ffn_dim) * o.np;
-  o.ldq = 3 * o.ldd;
-  o.lo_d = o.np == 2 ? D.embed_dim : 0;
-  o.lo_q = 3 * o.lo_d;
+  o.ldat = static_cast<int64_t>(o.da) * o.np;
+  o.ldq = 3 * o.ldat;
+  o.lo_d = o.np == 2 ? o.dk : 0;
+  o.lo_at = o.np == 2 ? o.da : 0;
+  o.lo_q = 3 * o.lo_at;
   return o;
+}
+
+// Slot maps: index i of a padded width -> source index, or -1 (zero). SL_PAD: i < n (dk columns). SL_HEAD: dim c of head h at 64h + c
+// (v rows, out_proj columns). SL_ROT (q/k rows): dims c < hd/2 at 64h + c, the others at 64h + 32 + (c - hd/2), so ESM2's rotate-half
+// partners (c, c + hd/2) sit on the pair (c', c' + 32) the GEMM's rotary epilogue rotates; q.k is unchanged.
+enum SlotMap { SL_PAD = 0, SL_HEAD, SL_ROT };
+__device__ __forceinline__ int slot_src(int i, int map, int n, int hd) {
+  if (map == SL_PAD) return i < n ? i : -1;
+  const int h = i >> 6, c = i & 63;
+  if (map == SL_HEAD) return c < hd ? h * hd + c : -1;
+  const int half = hd >> 1;
+  if (c < half) return h * hd + c;
+  if (c >= 32 && c < 32 + half) return h * hd + half + (c - 32);
+  return -1;
+}
+// dst [N, K] = src [n_src, k_src] (row-major) with its rows placed by map rmap and its columns by cmap, zeros elsewhere.
+__global__ void expand_slots_kernel(const float* __restrict__ src, int n_src, int k_src, float* __restrict__ dst, int N, int K, int rmap,
+                                    int cmap, int hd) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(N) * K) return;
+  const int r = slot_src(static_cast<int>(i / K), rmap, n_src, hd), c = slot_src(static_cast<int>(i % K), cmap, k_src, hd);
+  dst[i] = (r >= 0 && c >= 0) ? src[static_cast<long long>(r) * k_src + c] : 0.f;
 }
 
 }  // namespace
@@ -300,19 +330,19 @@ int embed(pg_handle h, const int32_t* tokens, int n_tokens, const int32_t* posit
 int ln(pg_handle h, const float* x, const float* g, const float* b, int M, __half* out, cudaStream_t s, int perm_R = 0, int perm_C = 0) {
   const int d = h->desc.embed_dim;
   ProfScope ps(CAT_LN, s);
-  return launch_layernorm_f16(x, d, g, b, M, d, out, h->op.ldd, h->op.lo_d, s, h->op.afmt, S_LN, perm_R, perm_C);
+  return launch_layernorm_f16(x, d, g, b, M, d, out, h->op.ldd, h->op.lo_d, s, h->op.afmt, S_LN, perm_R, perm_C, nullptr, 0, h->op.dk);
 }
 
 // The projections of a Layer, each profiled in its own GEMM category.
 enum Proj { QKV = CAT_GEMM_QKV, OUT = CAT_GEMM_OUT, FC1 = CAT_GEMM_FC1, FC2 = CAT_GEMM_FC2 };
 // Projection p of layer L on M operand rows `a` in the GEMM-input format (a_scale: the e4m3 scale their producer applied).
 GemmLaunch proj_gemm(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int M) {
-  const int d = h->desc.embed_dim, f = h->desc.ffn_dim;
+  const int d = h->desc.embed_dim, f = h->desc.ffn_dim, dk = h->op.dk, da = h->op.da;
   GemmLaunch g{};
   switch (p) {
-    case QKV: g.w = L.wqkv; g.w_inv = L.iqkv; g.bias = L.bqkv; g.N = 3 * d; g.K = d; break;
-    case OUT: g.w = L.wo; g.w_inv = L.io; g.bias = L.bo; g.N = d; g.K = d; break;
-    case FC1: g.w = L.w1; g.w_inv = L.i1; g.bias = L.b1; g.N = f; g.K = d; break;
+    case QKV: g.w = L.wqkv; g.w_inv = L.iqkv; g.bias = L.bqkv; g.N = 3 * da; g.K = dk; break;
+    case OUT: g.w = L.wo; g.w_inv = L.io; g.bias = L.bo; g.N = d; g.K = da; break;
+    case FC1: g.w = L.w1; g.w_inv = L.i1; g.bias = L.b1; g.N = f; g.K = dk; break;
     case FC2: g.w = L.w2; g.w_inv = L.i2; g.bias = L.b2; g.N = d; g.K = f; break;
   }
   g.a = a; g.lda = static_cast<int64_t>(g.K) * h->op.np; g.ldw = g.lda; g.M = M; g.nseg = h->op.nseg;
@@ -327,7 +357,7 @@ int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int
   g.epi = epi;
   g.out = out; g.ldo = static_cast<int64_t>(g.N) * h->op.np; g.out_fmt = p == QKV ? h->op.qfmt : h->op.afmt;
   g.out_lo_off = g.out_fmt ? g.N : 0; g.out_scale = out_scale;
-  if (epi == 3) { g.rot_cos = h->rot_cos; g.rot_sin = h->rot_sin; g.rot_T = rot_T; g.rot_dim = h->desc.embed_dim; }
+  if (epi == 3) { g.rot_cos = h->rot_cos; g.rot_sin = h->rot_sin; g.rot_T = rot_T; g.rot_dim = h->op.da; }  // q and k slots
   ProfScope ps(p, s);
   return launch_gemm(g, s);
 }
@@ -354,7 +384,7 @@ AttnLaunch attn_args(pg_handle h, const __half* qkv, __half* out, int B, int T) 
   const OpFmt& o = h->op;
   AttnLaunch a{};
   a.qkv = qkv; a.ld = o.ldq; a.lo_off = o.lo_q;
-  a.out = out; a.ldo = o.ldd; a.out_lo_off = o.lo_d; a.out_fmt = o.afmt; a.out_scale = S_ATT;
+  a.out = out; a.ldo = o.ldat; a.out_lo_off = o.lo_at; a.out_fmt = o.afmt; a.out_scale = S_ATT;
   a.B = B; a.T = T; a.heads = h->desc.heads; a.nseg = o.pseg; a.causal = 0; a.alibi_slopes = nullptr;
   return a;
 }
@@ -366,7 +396,7 @@ int last_layer(pg_handle h, const Layer& L, const int32_t* emit_rows, int Bc, in
   const OpFmt& o = h->op;
   int rc;
   { ProfScope ps(CAT_ATTN, s, gather ? 2 : 1);
-    rc = launch_attn_single_query(h->qkv, o.ldq, o.lo_q, emit_rows, Bc, T, h->desc.heads, h->cabuf, o.ldd, o.lo_d, s, o.afmt, S_ATT);
+    rc = launch_attn_single_query(h->qkv, o.ldq, o.lo_q, emit_rows, Bc, T, h->desc.heads, h->cabuf, o.ldat, o.lo_at, s, o.afmt, S_ATT);
     if (!rc && gather) rc = launch_gather_rows(h->x, emit_rows, Bc, T, h->desc.embed_dim, h->xc, s); }
   if (!rc) rc = lin_add(h, L, OUT, h->cabuf, S_ATT, Bc, h->xc, s);
   if (!rc) rc = mlp(h, L, h->xc, Bc, h->cabuf, h->cfbuf, 1, S_GELU, s);
@@ -794,8 +824,14 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   const pg_model_desc& D = *desc;
   if (D.layers <= 0 || D.embed_dim <= 0 || D.heads <= 0 || D.ffn_dim <= 0 || D.vocab <= 0)
     return set_error(PG_ERR_ARG, "pg_create: non-positive model dimension");
-  if (D.embed_dim != D.heads * 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: head_dim must be 64");
-  if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
+  if (D.arch == PG_ARCH_ESM2) {  // narrow heads in 64-wide slots, widths padded to 64 (OpFmt)
+    if (D.embed_dim % D.heads || (D.embed_dim / D.heads) % 2 || D.embed_dim / D.heads > 64)
+      return set_error(PG_ERR_UNSUPPORTED, "pg_create: ESM2 head_dim must be even and at most 64");
+    if (D.embed_dim % 4 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ESM2 needs embed_dim % 4 == 0 and ffn_dim % 64 == 0");
+  } else {
+    if (D.embed_dim != D.heads * 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: head_dim must be 64");
+    if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
+  }
   if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA)
     return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
   if (D.arch == PG_ARCH_TRANCEPTION && D.heads % 4) return set_error(PG_ERR_UNSUPPORTED, "pg_create: Tranception needs heads % 4 == 0 (model_pytorch.py:129-131)");
@@ -816,24 +852,25 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   h->delta = (D.precision == PG_PREC_F16D);
   h->max_rows = D.max_rows > 0 ? D.max_rows : 131072;
   h->head_cap = 8192;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->op.np;
+  const int d = D.embed_dim, f = D.ffn_dim, np = h->op.np, dk = h->op.dk, da = h->op.da;
+  const int dw = dk > da ? dk : da;  // abuf / cabuf hold both LayerNorm outputs (dk) and attention outputs (da)
   int rc = PG_OK;
   auto A = [&](auto** p, size_t n) { if (!rc) rc = dev_alloc(h, p, n); };
   h->layers.resize(D.layers);
   for (auto& L : h->layers) {
-    A(&L.wqkv, static_cast<size_t>(3) * d * d * np); A(&L.wo, static_cast<size_t>(d) * d * np);
-    A(&L.w1, static_cast<size_t>(f) * d * np); A(&L.w2, static_cast<size_t>(d) * f * np);
-    A(&L.bqkv, 3 * d); A(&L.bo, d); A(&L.b1, f); A(&L.b2, d);
+    A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
+    A(&L.w1, static_cast<size_t>(f) * dk * np); A(&L.w2, static_cast<size_t>(d) * f * np);
+    A(&L.bqkv, 3 * da); A(&L.bo, d); A(&L.b1, f); A(&L.b2, d);
     A(&L.ln1g, d); A(&L.ln1b, d); A(&L.ln2g, d); A(&L.ln2b, d);
-    if (h->op.nseg == 2) { A(&L.iqkv, 3 * d); A(&L.io, d); A(&L.i1, f); A(&L.i2, d); }
+    if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); A(&L.i1, f); A(&L.i2, d); }
     if (D.arch == PG_ARCH_TRANCEPTION) A(&L.conv_taps, 3 * 4 * 64 * 8);
   }
   if (D.arch == PG_ARCH_MSA) {
     h->col_layers.resize(D.layers);
     for (auto& L : h->col_layers) {
-      A(&L.wqkv, static_cast<size_t>(3) * d * d * np); A(&L.wo, static_cast<size_t>(d) * d * np);
-      A(&L.bqkv, 3 * d); A(&L.bo, d); A(&L.ln1g, d); A(&L.ln1b, d);
-      if (h->op.nseg == 2) { A(&L.iqkv, 3 * d); A(&L.io, d); }
+      A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
+      A(&L.bqkv, 3 * da); A(&L.bo, d); A(&L.ln1g, d); A(&L.ln1b, d);
+      if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); }
     }
     A(&h->row_pos, static_cast<size_t>(1024) * d);
   }
@@ -848,14 +885,14 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   A(&h->lnbg, d); A(&h->lnbb, d); A(&h->lnag, d); A(&h->lnab, d);
   A(&h->hdw, static_cast<size_t>(d) * d); A(&h->hdb, d); A(&h->hlng, d); A(&h->hlnb, d); A(&h->hbias, D.vocab);
   A(&h->x, static_cast<size_t>(h->max_rows) * d);
-  A(&h->abuf, static_cast<size_t>(h->max_rows) * d * np);
-  A(&h->qkv, static_cast<size_t>(h->max_rows) * 3 * d * np);
+  A(&h->abuf, static_cast<size_t>(h->max_rows) * dw * np);
+  A(&h->qkv, static_cast<size_t>(h->max_rows) * 3 * da * np);
   A(&h->fbuf, static_cast<size_t>(h->max_rows) * f * np);
   A(&h->hs_a, static_cast<size_t>(h->head_cap) * d);
   A(&h->hs_b, static_cast<size_t>(h->head_cap) * d);
   A(&h->row_sel, 2 * static_cast<size_t>(h->head_cap));  // second half: zeros (row 0 of every compacted sequence)
   A(&h->xc, static_cast<size_t>(h->head_cap) * d);
-  A(&h->cabuf, static_cast<size_t>(h->head_cap) * d * np);
+  A(&h->cabuf, static_cast<size_t>(h->head_cap) * dw * np);
   A(&h->cfbuf, static_cast<size_t>(h->head_cap) * f * np);
   if (h->delta) A(&h->cq, static_cast<size_t>(h->head_cap) * 3 * d * np);
   if (rc) {
@@ -892,6 +929,11 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     if (it->second->shape[0] != r || it->second->shape[1] != c) { missing += name + "(shape) "; return nullptr; }
     return static_cast<const float*>(it->second->data);
   };
+  struct Scratch {  // weights expanded to the padded operand layout (ESM2 head slots); cudaFree waits for the packing kernels
+    std::vector<float*> p;
+    ~Scratch() { for (float* q : p) cudaFree(q); }
+  } expanded;
+  cudaError_t exp_err = cudaSuccess;
   auto copy = [&](float* dst, const float* src, size_t cnt, float scale = 1.f) {
     if (!src) return;
     scale_copy_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256>>>(src, dst, static_cast<int>(cnt), scale);
@@ -928,24 +970,41 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     copy(h->lnab, get("ln_f.bias", d, 1), d);
     copy(h->slopes, get("alibi_slopes", D.heads, 1), D.heads);
   } else {
-    const float qscale = 0.125f;  // head_dim^-1/2 with head_dim == 64 (multihead_attention.py:103,261); exact power of two
+    const int hd = d / D.heads, dk = h->op.dk, da = h->op.da;
+    // head_dim^-1/2 (multihead_attention.py:103,261), folded into the fp32 q weights and bias: 0.125 (exact) for head_dim 64
+    const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(hd)));
+    // A [n_src, k_src] source weight placed in the padded operand layout [N, K] (OpFmt, slot maps rmap / cmap), in a scratch buffer
+    // freed on return; the source itself when the layout is unpadded.
+    auto slots = [&](const float* w, int n_src, int k_src, int N, int K, int rmap, int cmap) -> const float* {
+      if (!w || (N == n_src && K == k_src)) return w;
+      float* p = nullptr;
+      const cudaError_t e = cudaMalloc(&p, static_cast<size_t>(N) * K * sizeof(float));
+      if (e != cudaSuccess) {
+        if (!exp_err) exp_err = e;
+        return nullptr;
+      }
+      expanded.p.push_back(p);
+      const long long tot = static_cast<long long>(N) * K;
+      expand_slots_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(w, n_src, k_src, p, N, K, rmap, cmap, hd);
+      return p;
+    };
     // one attention block: q/k/v/out projections at `pa` ("...self_attn." / "...row_self_attention.layer."), its LayerNorm at `pl`
     auto load_attn = [&](Layer& L, const std::string& pa, const std::string& pl) {
       // q, k, v form ONE GEMM operand: one common e4m3 scale (matrix maximum over the three, q already scaled)
-      const float* wq = get(pa + "q_proj.weight", d, d);
-      const float* wk = get(pa + "k_proj.weight", d, d);
-      const float* wv = get(pa + "v_proj.weight", d, d);
-      pack(L.wqkv, L.iqkv, {{wq, qscale}, wk, wv}, d, d);
-      copy(L.bqkv, get(pa + "q_proj.bias", d, 1), d, qscale);
-      copy(L.bqkv + d, get(pa + "k_proj.bias", d, 1), d);
-      copy(L.bqkv + 2 * d, get(pa + "v_proj.bias", d, 1), d);
-      pack(L.wo, L.io, {get(pa + "out_proj.weight", d, d)}, d, d);
+      const float* wq = slots(get(pa + "q_proj.weight", d, d), d, d, da, dk, SL_ROT, SL_PAD);
+      const float* wk = slots(get(pa + "k_proj.weight", d, d), d, d, da, dk, SL_ROT, SL_PAD);
+      const float* wv = slots(get(pa + "v_proj.weight", d, d), d, d, da, dk, SL_HEAD, SL_PAD);
+      pack(L.wqkv, L.iqkv, {{wq, qscale}, wk, wv}, da, dk);
+      copy(L.bqkv, slots(get(pa + "q_proj.bias", d, 1), d, 1, da, 1, SL_ROT, SL_PAD), da, qscale);
+      copy(L.bqkv + da, slots(get(pa + "k_proj.bias", d, 1), d, 1, da, 1, SL_ROT, SL_PAD), da);
+      copy(L.bqkv + 2 * da, slots(get(pa + "v_proj.bias", d, 1), d, 1, da, 1, SL_HEAD, SL_PAD), da);
+      pack(L.wo, L.io, {slots(get(pa + "out_proj.weight", d, d), d, d, d, da, SL_PAD, SL_HEAD)}, d, da);
       copy(L.bo, get(pa + "out_proj.bias", d, 1), d);
       copy(L.ln1g, get(pl + "weight", d, 1), d);
       copy(L.ln1b, get(pl + "bias", d, 1), d);
     };
     auto load_ffn = [&](Layer& L, const std::string& pf, const std::string& pl) {
-      pack(L.w1, L.i1, {get(pf + "fc1.weight", f, d)}, f, d);
+      pack(L.w1, L.i1, {slots(get(pf + "fc1.weight", f, d), f, d, f, dk, SL_PAD, SL_PAD)}, f, dk);
       copy(L.b1, get(pf + "fc1.bias", f, 1), f);
       pack(L.w2, L.i2, {get(pf + "fc2.weight", d, f)}, d, f);
       copy(L.b2, get(pf + "fc2.bias", d, 1), d);
@@ -987,20 +1046,25 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     copy(h->hlnb, get("lm_head.layer_norm.bias", d, 1), d);
     copy(h->hbias, get("lm_head.bias", D.vocab, 1), D.vocab);
     if (D.arch == PG_ARCH_ESM2) {
+      // cos / sin [T, hd/2] (checkpoint.rotary_tables) or [T, 32] -> device tables [T, 32], zero after column hd/2
       auto it = by_name.find("rotary.cos");
       auto is = by_name.find("rotary.sin");
-      if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != 32 || is->second->shape[0] != it->second->shape[0]) {
-        missing += "rotary.cos/rotary.sin[T,32] ";
+      const int64_t rw = it == by_name.end() ? 0 : it->second->shape[1];
+      if (it == by_name.end() || is == by_name.end() || (rw != 32 && rw != hd / 2) || is->second->shape[1] != rw ||
+          is->second->shape[0] != it->second->shape[0]) {
+        missing += "rotary.cos/rotary.sin[T,head_dim/2] ";
       } else {
         h->rot_rows = static_cast<int>(it->second->shape[0]);
         int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
         if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
         if (rc) return rc;
-        copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * 32);
-        copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * 32);
+        for (auto [dst, src] : {std::make_pair(h->rot_cos, it->second->data), std::make_pair(h->rot_sin, is->second->data)})
+          expand_slots_kernel<<<(h->rot_rows * 32 + 255) / 256, 256>>>(static_cast<const float*>(src), h->rot_rows, static_cast<int>(rw), dst,
+                                                                       h->rot_rows, 32, SL_PAD, SL_PAD, hd);
       }
     }
   }
+  if (exp_err != cudaSuccess) return fail(h, PG_ERR_CUDA, std::string("pg_load_weights: cudaMalloc: ") + cudaGetErrorString(exp_err));
   if (!missing.empty()) return fail(h, PG_ERR_ARG, "pg_load_weights: missing or mis-shaped tensors: " + missing);
   PG_CUDA_OK(cudaGetLastError());
   PG_CUDA_OK(cudaDeviceSynchronize());  // caller may free its tensors on return

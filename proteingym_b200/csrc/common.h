@@ -71,9 +71,10 @@ void set_gemm_cta2(int v);      // 1: clusters of two CTAs sharing the W tile (T
 
 // fmt / scale as above (fmt 0 when lo_off == 0).
 // base (optional, fp16 [base_T, d]): the output is LN(x[row]) - base[row % base_T] (delta-operand mode).
+// dp: width of each output plane (0 = d); columns [d, dp) of every plane are written as zeros.
 int launch_layernorm_f16(const float* x, int64_t ldx, const float* gamma, const float* beta, int rows, int d, __half* out,
                          int64_t ldo, int64_t lo_off, cudaStream_t s, int fmt = -1, float scale = 0.f, int perm_R = 0, int perm_C = 0,
-                         const __half* base = nullptr, int base_T = 0);
+                         const __half* base = nullptr, int base_T = 0, int dp = 0);
 // dst row (b * T + row_sel[b]) <- src row b, row_bytes each (a multiple of 16): the compact exact rows back into the full buffers
 int launch_scatter_rows(const void* src, int64_t src_pitch_bytes, void* dst, int64_t dst_pitch_bytes, const int32_t* row_sel, int B, int T,
                         int row_bytes, cudaStream_t s);

@@ -37,12 +37,15 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
 // ---------------------------------------------------------------------------------------------------------------
 // K2: one warp per row. Two-pass (mean, then centred variance) like torch.nn.LayerNorm; eps = 1e-5
 // (esm/modules.py:68-81). Reads 4*d bytes, writes 2*d (hi) [+ 2*d (lo)] bytes per row.
-template <int MAXV>  // float4 vectors per lane; d <= MAXV*128
+// Each output plane is dp >= d wide: columns [d, dp) of every plane written are zeros (the K padding of the next GEMM when d is
+// not a multiple of 64; statistics are over d only).
+template <int MAXV, bool PAD>  // float4 vectors per lane, d <= MAXV*128; PAD: dp > d (a separate instance keeps the unpadded one lean)
 __global__ void layernorm_f16_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ gamma,
-                                     const float* __restrict__ beta, int rows, int d, __half* __restrict__ out,
+                                     const float* __restrict__ beta, int rows, int d, int dp_, __half* __restrict__ out,
                                      long long ldo, long long lo_off, int fmt, float scale, int perm_R, int perm_C,
                                      const __half* __restrict__ base, int base_T) {
   const int warps_per_block = blockDim.x >> 5;
+  const int dp = PAD ? dp_ : d;
   const long long row = static_cast<long long>(blockIdx.x) * warps_per_block + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -108,9 +111,20 @@ __global__ void layernorm_f16_kernel(const float* __restrict__ x, long long ldx,
         *reinterpret_cast<uint32_t*>(f8 + idx * 4) =
             pack4_e4m3((y[0] - __half2float(h[0])) * sl, (y[1] - __half2float(h[1])) * sl, (y[2] - __half2float(h[2])) * sl,
                        (y[3] - __half2float(h[3])) * sl);
-        *reinterpret_cast<uint32_t*>(f8 + d + idx * 4) =
+        *reinterpret_cast<uint32_t*>(f8 + dp + idx * 4) =
             pack4_e4m3(__half2float(h[0]) * scale, __half2float(h[1]) * scale, __half2float(h[2]) * scale, __half2float(h[3]) * scale);
       }
+    }
+  }
+  if (!PAD) return;
+  for (int c = d + lane * 4; c < dp; c += 128) {  // padding columns, 4 per lane (d and dp are multiples of 4)
+    *reinterpret_cast<uint2*>(orow + c) = make_uint2(0u, 0u);
+    if (fmt == 1) {
+      *reinterpret_cast<uint2*>(orow + lo_off + c) = make_uint2(0u, 0u);
+    } else if (fmt == 2) {
+      uint8_t* f8 = reinterpret_cast<uint8_t*>(orow + lo_off);
+      *reinterpret_cast<uint32_t*>(f8 + c) = 0u;
+      *reinterpret_cast<uint32_t*>(f8 + dp + c) = 0u;
     }
   }
 }
@@ -401,19 +415,27 @@ int launch_scatter_rows(const void* src, int64_t src_pitch_bytes, void* dst, int
 
 int launch_layernorm_f16(const float* x, int64_t ldx, const float* gamma, const float* beta, int rows, int d, __half* out,
                          int64_t ldo, int64_t lo_off, cudaStream_t s, int fmt, float scale, int perm_R, int perm_C, const __half* base,
-                         int base_T) {
+                         int base_T, int dp) {
   if (rows <= 0) return PG_OK;
   if (base && (base_T <= 0 || perm_C > 0)) return set_error(PG_ERR_ARG, "layernorm: a base needs base_T > 0 and no row permutation");
   if (perm_C > 0 && (perm_R <= 0 || rows % (perm_R * perm_C))) return set_error(PG_ERR_ARG, "layernorm: rows must be whole [R, C] alignments");
-  if (d % 4 || ldx % 4 || ldo % 4 || lo_off % 4) return set_error(PG_ERR_ARG, "layernorm: d and pitches must be multiples of 4");
+  if (dp <= 0) dp = d;
+  if (d % 4 || dp % 4 || dp < d || ldx % 4 || ldo % 4 || lo_off % 4) return set_error(PG_ERR_ARG, "layernorm: d, the plane width and pitches must be multiples of 4");
+  if (base && dp != d) return set_error(PG_ERR_ARG, "layernorm: a base needs unpadded rows");
   if (fmt < 0) fmt = lo_off > 0 ? 1 : 0;
   if (fmt > 2 || (fmt >= 1 && lo_off <= 0) || (fmt == 2 && !(scale > 0.f))) return set_error(PG_ERR_ARG, "layernorm: bad output format");
   const int wpb = 8;
   const int grid = (rows + wpb - 1) / wpb;
-  if (d <= 128 * 4) layernorm_f16_kernel<4><<<grid, wpb * 32, 0, s>>>(x, ldx, gamma, beta, rows, d, out, ldo, lo_off, fmt, scale, perm_R, perm_C, base, base_T);
-  else if (d <= 128 * 10) layernorm_f16_kernel<10><<<grid, wpb * 32, 0, s>>>(x, ldx, gamma, beta, rows, d, out, ldo, lo_off, fmt, scale, perm_R, perm_C, base, base_T);
-  else if (d <= 128 * 20) layernorm_f16_kernel<20><<<grid, wpb * 32, 0, s>>>(x, ldx, gamma, beta, rows, d, out, ldo, lo_off, fmt, scale, perm_R, perm_C, base, base_T);
-  else if (d <= 128 * 40) layernorm_f16_kernel<40><<<grid, wpb * 32, 0, s>>>(x, ldx, gamma, beta, rows, d, out, ldo, lo_off, fmt, scale, perm_R, perm_C, base, base_T);
+#define PG_LN(MAXV)                                                                                                               \
+  (dp > d ? layernorm_f16_kernel<MAXV, true><<<grid, wpb * 32, 0, s>>>(x, ldx, gamma, beta, rows, d, dp, out, ldo, lo_off, fmt, scale, \
+                                                                       perm_R, perm_C, base, base_T)                                 \
+          : layernorm_f16_kernel<MAXV, false><<<grid, wpb * 32, 0, s>>>(x, ldx, gamma, beta, rows, d, dp, out, ldo, lo_off, fmt, scale, \
+                                                                        perm_R, perm_C, base, base_T))
+  if (d <= 128 * 4) PG_LN(4);
+  else if (d <= 128 * 10) PG_LN(10);
+  else if (d <= 128 * 20) PG_LN(20);
+  else if (d <= 128 * 40) PG_LN(40);
+#undef PG_LN
   else return set_error(PG_ERR_UNSUPPORTED, "layernorm: d > 5120");
   PG_CUDA_OK(cudaGetLastError());
   return PG_OK;

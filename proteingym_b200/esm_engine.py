@@ -32,7 +32,7 @@ def choose_precision(config: EsmConfig, mutants=None, strategy: str = "masked-ma
     for the ESM-1b / ESM-1v masked-marginal pass over ONE shared window) measures 6.8e-5 mean / 3.9e-4 max on the same BLAT golden
     (286 residues). Its error scales with the size of the perturbation one mask causes, i.e. ~1/L: on a 96-residue protein it is
     7.6e-4 / 8.8e-4 / 1.5e-3 for 1 / 2 / 3 sites (f16f8: 3.4e-4 / 5.6e-4 / 6.0e-4; test_multi_site_error_growth_650m_vs_oracle), so
-    short proteins stay on f16f8.
+    short proteins stay on f16f8. ESM2 8M / 35M / 150M stay within 6.1e-4 in f16f8 (tests/test_gpu_esm2_small.py).
     Rule: for models up to 1280 wide when no mutant has more than two sites — f16d if the architecture and the strategy allow it and
     192 <= ``seq_len`` (residues; + 2 tokens must fit the 1024-token window), else f16f8; f16x3 otherwise."""
     if config.embed_dim > 1280:

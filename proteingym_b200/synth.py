@@ -39,6 +39,9 @@ class EsmArch:
 
 ESM1V_650M = EsmArch("esm1v", 33, 1280, 20, 5120)
 ESM1B_650M = EsmArch("esm1v", 33, 1280, 20, 5120, emb_layer_norm_before=True)
+ESM2_8M = EsmArch("esm2", 6, 320, 20, 1280)      # head_dim 16
+ESM2_35M = EsmArch("esm2", 12, 480, 20, 1920)    # head_dim 24, width not a multiple of 64
+ESM2_150M = EsmArch("esm2", 30, 640, 20, 2560)   # head_dim 32
 ESM2_650M = EsmArch("esm2", 33, 1280, 20, 5120)
 ESM2_3B = EsmArch("esm2", 36, 2560, 40, 10240)
 

@@ -17,8 +17,9 @@ def main():
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    big = len(sys.argv) > 1 and sys.argv[1] == "650m"
-    arch = synth.ESM1V_650M if big else synth.EsmArch("esm1v", 3, 256, 4, 1024)
+    which = sys.argv[1] if len(sys.argv) > 1 else ""
+    big = which == "650m"
+    arch = {"650m": synth.ESM1V_650M, "esm2_8m": synth.ESM2_8M}.get(which, synth.EsmArch("esm1v", 3, 256, 4, 1024))
     conf = config_from_synth(arch)
     state = sharding.broadcast_state(normalise_synth_state(arch, synth.make_esm_state(arch, seed=0)) if rank == 0 else None, src=0,
                                      device=torch.device("cuda", local))

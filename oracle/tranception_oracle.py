@@ -50,21 +50,42 @@ def layer_norm(x, w, b, eps):
     return (x - mu) / torch.sqrt(var + eps) * w + b
 
 
-def depthwise_causal_conv(x, w, b):
+def depthwise_causal_conv(x, w, b, tile=0):
     """SpatialDepthWiseConvolution (model_pytorch.py:73-88): Conv1d(groups=hd, padding=k-1) then drop the last k-1 outputs
-    => out[t] = b + sum_j w[:, j] * x[t - (k-1) + j]. x: [B, h, T, hd]; w: [hd, 1, k]; b: [hd]."""
+    => out[t] = b + sum_j w[:, j] * x[t - (k-1) + j]. x: [B, h, T, hd]; w: [hd, 1, k]; b: [hd].
+    ``tile`` > 0 (emulated fault): a look-back term is dropped when its input row lies in an earlier tile of ``tile`` rows."""
     k = w.shape[-1]
     B, h, T, hd = x.shape
     xp = torch.cat([x.new_zeros(B, h, k - 1, hd), x], dim=2)
     out = x.new_zeros(B, h, T, hd) + b
     for j in range(k):
-        out = out + xp[:, :, j:j + T, :] * w[:, 0, j]
+        term = xp[:, :, j:j + T, :] * w[:, 0, j]
+        if tile:
+            term = term * (torch.arange(T) % tile >= k - 1 - j).to(x.dtype)[:, None]
+        out = out + term
     return out
 
 
-def forward(st, ids, layers, heads, ln_eps=1e-5, dtype=torch.float32, rnd=None):
+# Emulated kernel faults, for measuring how far a test bound is from a real bug. None (the default) is the model itself.
+#   attn_qkv_f16          the conv'd (q / sqrt(hd)), k, v rounded to fp16 before QK^T and PV (a dropped lo plane)
+#   attn_p_f16            the softmax P rounded to fp16 before PV
+#   conv_in_f16           the raw q / k / v rounded to fp16 before the depthwise conv
+#   conv_tile_edge        conv look-back taps that cross a multiple of 64 rows dropped (a lost halo between conv tiles, or a
+#                         wrong look-back pointer into the wild-type prefix)
+#   alibi_slope_by_group  head h takes slopes[h // (heads / 4)], its conv group, instead of its own slope
+FAULTS = ("attn_qkv_f16", "attn_p_f16", "conv_in_f16", "conv_tile_edge", "alibi_slope_by_group")
+
+
+def _f16(t):
+    return t.to(torch.float16).to(t.dtype)
+
+
+def forward(st, ids, layers, heads, ln_eps=1e-5, dtype=torch.float32, rnd=None, fault=None):
     """logits [B, T, V] for right-padded ids [B, T] of EQUAL real length (callers group by length; padding never influences
-    earlier positions under the causal mask, so per-length evaluation equals the reference's padded batches)."""
+    earlier positions under the causal mask, so per-length evaluation equals the reference's padded batches).
+    ``fault``: one of FAULTS, applied in every layer."""
+    if fault is not None and fault not in FAULTS:
+        raise ValueError(f"unknown fault {fault!r}")
     rnd = rnd or (lambda t: t)
     W = lambda n: st[n].to(dtype)
     wte = W("transformer.wte.weight")
@@ -73,7 +94,10 @@ def forward(st, ids, layers, heads, ln_eps=1e-5, dtype=torch.float32, rnd=None):
     hd = d // heads
     g = heads // 4
     x = wte[ids]
-    slopes = torch.tensor(get_slopes(heads), dtype=dtype)
+    slopes = get_slopes(heads)
+    if fault == "alibi_slope_by_group":
+        slopes = [slopes[h // g] for h in range(heads)]
+    slopes = torch.tensor(slopes, dtype=dtype)
     alibi = slopes[:, None, None] * torch.arange(T, dtype=dtype)[None, None, :]  # [h, 1, T]  (model_pytorch.py:376-380)
     causal = torch.tril(torch.ones(T, T, dtype=torch.bool))
     for i in range(layers):
@@ -81,18 +105,25 @@ def forward(st, ids, layers, heads, ln_eps=1e-5, dtype=torch.float32, rnd=None):
         h_ = rnd(layer_norm(x, W(p + "ln_1.weight"), W(p + "ln_1.bias"), ln_eps))
         qkv = h_ @ rnd(W(p + "attn.c_attn.weight")) + W(p + "attn.c_attn.bias")  # Conv1D: x @ W[in,out] + b (:224)
         q, k, v = [t.view(B, T, heads, hd).permute(0, 2, 1, 3) for t in qkv.split(d, dim=2)]
+        if fault == "conv_in_f16":
+            q, k, v = _f16(q), _f16(k), _f16(v)
+        tile = 64 if fault == "conv_tile_edge" else 0
         def conv_groups(t, nm):  # :240-251: heads [0,g) untouched; groups 1..3 get kernels 3,5,7
             parts = [t[:, :g]]
             for ki in range(3):
                 parts.append(depthwise_causal_conv(t[:, (ki + 1) * g:(ki + 2) * g], W(p + f"attn.{nm}_depthwiseconv.{ki}.conv.weight"),
-                                                   W(p + f"attn.{nm}_depthwiseconv.{ki}.conv.bias")))
+                                                   W(p + f"attn.{nm}_depthwiseconv.{ki}.conv.bias"), tile))
             return torch.cat(parts, dim=1)
         q, k, v = conv_groups(q, "query"), conv_groups(k, "key"), conv_groups(v, "value")
         q, k, v = rnd(q / float(hd) ** 0.5), rnd(k), rnd(v)  # (scale applied to q here; algebraically = :158-159)
+        if fault == "attn_qkv_f16":
+            q, k, v = _f16(q), _f16(k), _f16(v)
         s = q @ k.transpose(-1, -2)
         s = torch.where(causal, s, torch.tensor(-1e4, dtype=dtype))  # :162-165
         s = s + alibi[None]                                          # :167-168
         a = torch.softmax(s, dim=-1)
+        if fault == "attn_p_f16":
+            a = _f16(a)
         o = rnd((rnd(a) @ v).permute(0, 2, 1, 3).reshape(B, T, d))
         x = x + o @ rnd(W(p + "attn.c_proj.weight")) + W(p + "attn.c_proj.bias")
         h_ = rnd(layer_norm(x, W(p + "ln_2.weight"), W(p + "ln_2.bias"), ln_eps))
@@ -125,6 +156,17 @@ def sequence_logprob(st, seq, layers, heads, ln_eps=1e-5, dtype=torch.float32, l
             lp = fused
     labels = ids[0, 1:]
     return lp.gather(1, labels[:, None]).sum().item()
+
+
+def logprob_rows(st, seqs, layers, heads, ln_eps=1e-5, dtype=torch.float64, fault=None):
+    """Per string in ``seqs``: the log-softmax rows [len(s) + 1, V] (numpy) of every predicted position of ``[CLS] s [SEP]``
+    (row t predicts token t + 1), unfused. ``fault``: one of FAULTS."""
+    out = []
+    with torch.no_grad():
+        for s in seqs:
+            ids = torch.tensor([tokenize(s)], dtype=torch.int64)
+            out.append(torch.log_softmax(forward(st, ids, layers, heads, ln_eps, dtype, fault=fault)[0, :-1], dim=-1).numpy())
+    return out
 
 
 def fused_logprob_rows(st, seq, layers, heads, ln_eps=1e-5, log_prior=None, prior_row=None, alpha=0.0, log_prior2=None, prior_row2=None,

@@ -7,7 +7,8 @@
 #include <vector>
 
 #include "common.h"
-#include "ptx.cuh"
+#include "operand.cuh"
+#include "reduce.cuh"
 
 namespace pg {
 
@@ -86,11 +87,7 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, int N, int K, lo
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= static_cast<long long>(N) * K) return;
   const int n = static_cast<int>(i / K), k = static_cast<int>(i % K);
-  const float v = w[n * sn + k * sk] * scale;
-  __half hi, lo;
-  split_hi_lo(v, hi, lo);
-  out[static_cast<long long>(n) * K * np + k] = hi;
-  if (np == 2) out[static_cast<long long>(n) * K * np + K + k] = lo;
+  store_operand_one(out + static_cast<long long>(n) * K * np, K, 0, np == 2 ? 1 : 0, 0.f, k, w[n * sn + k * sk] * scale);
 }
 // Weights in the fp16 + e4m3 format of gemm_tc.cu (nseg 2): row n = [hi fp16 (K) | hi8 (K bytes) | lo8 (K bytes)], pitch 4K bytes,
 // hi8 = e4m3(hi * t), lo8 = e4m3(lo * 2^11 * t) with ONE power of two t per matrix: the one that puts the largest |hi| of the matrix in
@@ -102,8 +99,7 @@ __global__ void weight_absmax_kernel(const float* __restrict__ w, int N, int K, 
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   float a = 0.f;
   if (i < static_cast<long long>(N) * K) a = fabsf(__half2float(f2h_sat(w[(i / K) * sn + (i % K) * sk] * scale)));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+  a = warp_max(a);
   if ((threadIdx.x & 31) == 0 && a > 0.f) atomicMax(amax_bits, __float_as_uint(a));  // non-negative floats order like their bit patterns
 }
 __global__ void pack_weight_f8_kernel(const float* __restrict__ w, int N, int K, long long sn, long long sk, float scale,
@@ -121,16 +117,7 @@ __global__ void pack_weight_f8_kernel(const float* __restrict__ w, int N, int K,
   }
   const float* wr = w + static_cast<long long>(n) * sn;
   __half* orow = out + static_cast<long long>(n) * K * 2;
-  uint8_t* f8 = reinterpret_cast<uint8_t*>(orow + K);
-  for (int k = lane; k < K; k += 32) {
-    const float v = wr[k * sk] * scale;
-    __half hi, lo;
-    split_hi_lo(v, hi, lo);
-    const float hf = __half2float(hi);
-    orow[k] = hi;
-    f8[k] = static_cast<uint8_t>(cvt_e4m3x2(hf * t, 0.f) & 0xff);
-    f8[K + k] = static_cast<uint8_t>(cvt_e4m3x2((v - hf) * t * 2048.f, 0.f) & 0xff);
-  }
+  for (int k = lane; k < K; k += 32) store_weight_f8_one(orow, K, t, k, wr[k * sk] * scale);
   if (lane == 0) w_inv[n] = 1.f / t;
 }
 // Packs a group of [N, K] weights (w[i] scaled by scale[i]) into consecutive blocks of N operand rows of `out` on stream s, in fp16

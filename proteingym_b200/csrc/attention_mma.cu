@@ -6,7 +6,7 @@
 // It is the correctness baseline for the attention path; the wgmma version (attention_wgmma.cu) is the hot kernel.
 // With NSEG == 3 every operand is an fp16 hi+lo pair and each product runs three passes (hi*hi + lo*hi + hi*lo).
 #include "common.h"
-#include "ptx.cuh"
+#include "operand.cuh"
 
 namespace pg {
 
@@ -184,31 +184,23 @@ __global__ void __launch_bounds__(128) attn_mma_kernel(AttnLaunch a) {
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
   const float r0 = 1.f / l0, r1 = 1.f / l1;
-  __half* orow0 = a.out + (static_cast<long long>(b) * a.T + qrow0) * a.ldo + head * 64;
-  __half* orow1 = a.out + (static_cast<long long>(b) * a.T + qrow1) * a.ldo + head * 64;
+  __half* orow0 = a.out + (static_cast<long long>(b) * a.T + qrow0) * a.ldo;
+  __half* orow1 = a.out + (static_cast<long long>(b) * a.T + qrow1) * a.ldo;
 #pragma unroll
   for (int n = 0; n < 8; ++n) {
-    const int col = n * 8 + 2 * t;
-    __half h0, h1, e0, e1;
-    if (qrow0 < a.T) {
-      split_hi_lo(o[n][0] * r0, h0, e0);
-      split_hi_lo(o[n][1] * r0, h1, e1);
-      *reinterpret_cast<uint32_t*>(orow0 + col) = pack_h2(h0, h1);
-      if (a.out_lo_off > 0) *reinterpret_cast<uint32_t*>(orow0 + a.out_lo_off + col) = pack_h2(e0, e1);
-    }
-    if (qrow1 < a.T) {
-      split_hi_lo(o[n][2] * r1, h0, e0);
-      split_hi_lo(o[n][3] * r1, h1, e1);
-      *reinterpret_cast<uint32_t*>(orow1 + col) = pack_h2(h0, h1);
-      if (a.out_lo_off > 0) *reinterpret_cast<uint32_t*>(orow1 + a.out_lo_off + col) = pack_h2(e0, e1);
-    }
+    const int col = head * 64 + n * 8 + 2 * t;
+    if (qrow0 < a.T) store_operand_pair(orow0, a.out_lo_off, 0, a.out_fmt, 0.f, col, o[n][0] * r0, o[n][1] * r0);
+    if (qrow1 < a.T) store_operand_pair(orow1, a.out_lo_off, 0, a.out_fmt, 0.f, col, o[n][2] * r1, o[n][3] * r1);
   }
 }
 
 }  // namespace
 
-int launch_attention(const AttnLaunch& a, cudaStream_t s) {
-  if (a.B <= 0 || a.T <= 0) return PG_OK;
+int launch_attention(const AttnLaunch& al, cudaStream_t s) {
+  if (al.B <= 0 || al.T <= 0) return PG_OK;
+  AttnLaunch a = al;
+  if (int rc = resolve_out_fmt(a.out_fmt, a.out_lo_off, a.out_scale, "attention")) return rc;
+  if (a.out_fmt == 2) return set_error(PG_ERR_UNSUPPORTED, "attention: the mma.sync kernel writes fp16 planes only");
   if (a.perm_C) return set_error(PG_ERR_UNSUPPORTED, "attention: the column-attention row order is only in the wgmma kernel (attention_wgmma.cu)");
   if (a.ld % 8 || a.lo_off % 8 || a.ldo % 2 || a.out_lo_off % 2) return set_error(PG_ERR_ARG, "attention: misaligned pitches");
   if (a.nseg != 1 && a.nseg != 3) return set_error(PG_ERR_ARG, "attention: nseg must be 1 or 3");

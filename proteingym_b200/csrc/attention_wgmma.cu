@@ -9,7 +9,7 @@
 #include <cstdlib>
 
 #include "common.h"
-#include "ptx.cuh"
+#include "operand.cuh"
 
 namespace pg {
 
@@ -47,12 +47,6 @@ __device__ __forceinline__ float ex2a(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ uint32_t cvt2h(float lo_elem, float hi_elem) {
-  uint32_t d;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi_elem), "f"(lo_elem));
-  return d;
-}
-__device__ __forceinline__ float2 h2f(uint32_t h) { return __half22float2(*reinterpret_cast<const __half2*>(&h)); }
 
 template <int NP, int DELTA>
 __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tm,
@@ -166,10 +160,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
         const int r = u & 1;
         const float e0 = ex2a(s[i] - mref[r]), e1 = ex2a(s[i + 1] - mref[r]);
         l[r] += e0 + e1;
-        ph[kk][u] = cvt2h(e0, e1);
+        ph[kk][u] = cvt_f16x2_rn_inf(e0, e1);
         if (NP == 2) {
-          const float2 hf = h2f(ph[kk][u]);
-          pl[kk][u] = cvt2h(e0 - hf.x, e1 - hf.y);
+          const float2 hf = unpack_h2(ph[kk][u]);
+          pl[kk][u] = cvt_f16x2_rn_inf(e0 - hf.x, e1 - hf.y);
         }
       }
     }
@@ -201,9 +195,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
     const float rl = 1.f / l[r];
     long long orow_idx = static_cast<long long>(b) * p.Tq + (qidx - p.s_blocks * KT);
     if (p.perm_C > 0) orow_idx = (static_cast<long long>(b / p.perm_C) * p.Tq + qidx) * p.perm_C + b % p.perm_C;
+    // operand.cuh's column-pair store written out, for the same reason as in the GEMM epilogue (gemm_tc.cu)
     __half* orow = p.out + orow_idx * p.ldo + h * 64;
     uint8_t* f8 = reinterpret_cast<uint8_t*>(p.out + orow_idx * p.ldo + p.out_lo_off) + h * 64;
-    const float sh = p.out_scale, sl = p.out_scale * 2048.f;
+    const float sh = p.out_scale, sl = p.out_scale * LO8_GAIN;
     // delta-operand mode (DELTA): this row's exact value also goes to cout[b] when it is the masked row; base row to subtract
     const bool crow = DELTA && p.mask_pos != nullptr && qidx == __ldg(p.mask_pos + b);
     const __half* brow = (DELTA && p.base_o != nullptr) ? p.base_o + static_cast<long long>(qidx) * p.d + h * 64 : nullptr;
@@ -213,21 +208,21 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
       float x0 = o[4 * n + 2 * r] * rl, x1 = o[4 * n + 2 * r + 1] * rl;
       if (DELTA && crow) {  // rare (one row per sequence and head): fp16 hi / lo pair of the full value
         __half* cr = p.cout + static_cast<long long>(b) * p.ldc + h * 64 + col;
-        const uint32_t ch = cvt2h(x0, x1);
-        const float2 cf = h2f(ch);
+        const uint32_t ch = cvt_f16x2_rn_inf(x0, x1);
+        const float2 cf = unpack_h2(ch);
         *reinterpret_cast<uint32_t*>(cr) = ch;
-        *reinterpret_cast<uint32_t*>(cr + p.c_lo_off) = cvt2h(x0 - cf.x, x1 - cf.y);
+        *reinterpret_cast<uint32_t*>(cr + p.c_lo_off) = cvt_f16x2_rn_inf(x0 - cf.x, x1 - cf.y);
       }
       if (DELTA && brow != nullptr) {
         const float2 bq = __half22float2(__ldg(reinterpret_cast<const __half2*>(brow + col)));
         x0 -= bq.x;
         x1 -= bq.y;
       }
-      const uint32_t hi = cvt2h(x0, x1);
-      const float2 hf = h2f(hi);
+      const uint32_t hi = cvt_f16x2_rn_inf(x0, x1);
+      const float2 hf = unpack_h2(hi);
       *reinterpret_cast<uint32_t*>(orow + col) = hi;
       if (p.out_fmt == 1) {
-        *reinterpret_cast<uint32_t*>(orow + p.out_lo_off + col) = cvt2h(x0 - hf.x, x1 - hf.y);
+        *reinterpret_cast<uint32_t*>(orow + p.out_lo_off + col) = cvt_f16x2_rn_inf(x0 - hf.x, x1 - hf.y);
       } else if (p.out_fmt == 2) {
         *reinterpret_cast<uint16_t*>(f8 + col) = static_cast<uint16_t>(cvt_e4m3x2((x0 - hf.x) * sl, (x1 - hf.y) * sl));
         *reinterpret_cast<uint16_t*>(f8 + p.d + col) = static_cast<uint16_t>(cvt_e4m3x2(hf.x * sh, hf.y * sh));
@@ -253,15 +248,14 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
   p.nqt = (a.T + QT - 1) / QT; p.nkb = (p.T + KT - 1) / KT;
   p.lo_off = a.lo_off; p.out = a.out; p.ldo = a.ldo; p.out_lo_off = a.out_lo_off;
   p.causal = a.causal; p.alibi_slopes = a.alibi_slopes;
-  p.out_fmt = a.out_fmt < 0 ? (a.out_lo_off > 0 ? 1 : 0) : a.out_fmt;
+  p.out_fmt = a.out_fmt;
+  if (int rc = resolve_out_fmt(p.out_fmt, a.out_lo_off, a.out_scale, "attention_wgmma")) return rc;
   p.out_scale = a.out_scale;
   p.perm_C = a.perm_C;
   p.base_o = a.base_o; p.mask_pos = a.mask_pos; p.cout = a.cout; p.ldc = a.ldc; p.c_lo_off = a.c_lo_off;
   if ((a.base_o || a.mask_pos) && (a.prefix || a.perm_C || (a.mask_pos && (!a.cout || a.ldc % 2 || a.c_lo_off % 2 || a.c_lo_off <= 0))))
     return set_error(PG_ERR_ARG, "attention_wgmma: delta-operand mode needs plain sequences and, with mask_pos, a compact hi/lo output");
   if (a.perm_C < 0 || (a.perm_C > 0 && (a.prefix || a.B % a.perm_C))) return set_error(PG_ERR_ARG, "attention_wgmma: bad column-attention arguments");
-  if (p.out_fmt > 2 || (p.out_fmt >= 1 && a.out_lo_off <= 0) || (p.out_fmt == 2 && !(a.out_scale > 0.f)))
-    return set_error(PG_ERR_ARG, "attention_wgmma: bad output format");
   const int np = a.nseg == 3 ? 2 : 1;
   const uint64_t width = static_cast<uint64_t>(3) * p.d * np;
   if (np == 2 && a.lo_off != 3ll * p.d) return set_error(PG_ERR_ARG, "attention_wgmma: lo planes must follow the hi planes (lo_off == 3*d)");

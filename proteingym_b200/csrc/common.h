@@ -39,6 +39,14 @@ struct ProfScope {  // records an event pair around the launches issued in its l
 //   fmt 2  [hi fp16 (n) | lo8 (n bytes) | hi8 (n bytes)]   e4m3 planes start at element offset lo_off (= byte 2*lo_off);
 //          lo8 = e4m3(lo * 2^11 * s), hi8 = e4m3(hi * s) with the power-of-two scale s of the consuming GEMM (gemm_tc.cu).
 //          Weights use [hi fp16 | hi8 | lo8] with a per-row scale instead (api.cu pack_weight_f8_kernel).
+// operand.cuh holds the device code that writes and reads these rows.
+// Output format of a launcher: -1 = fmt 1 when there is a lo plane (lo_off > 0), else fmt 0. Resolves that default in place and
+// rejects a format without its planes or its scale (`who` prefixes the error text).
+inline int resolve_out_fmt(int& fmt, int64_t lo_off, float scale, const char* who) {
+  if (fmt < 0) fmt = lo_off > 0 ? 1 : 0;
+  if (fmt > 2 || (fmt >= 1 && lo_off <= 0) || (fmt == 2 && !(scale > 0.f))) return set_error(PG_ERR_ARG, std::string(who) + ": bad output format");
+  return PG_OK;
+}
 struct GemmLaunch {
   const void* a; int64_t lda;
   const void* w; int64_t ldw;

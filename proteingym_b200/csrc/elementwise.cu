@@ -1,38 +1,12 @@
 // K1 (embedding), K2 (LayerNorm -> fp16 hi/lo), K5 (masked-row LM head + log-softmax), K6 (mutant scoring gather).
 // These are the HBM-bound helpers of the path (SURVEY.md §2.3); all arithmetic is fp32.
 #include "common.h"
-#include "ptx.cuh"
+#include "operand.cuh"
+#include "reduce.cuh"
 
 namespace pg {
 
 namespace {
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// Block-wide sum for blockDim.x <= 1024 (result broadcast to all threads).
-__device__ __forceinline__ float block_sum(float v, float* sh) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-  v = warp_sum(v);
-  __syncthreads();
-  if (lane == 0) sh[w] = v;
-  __syncthreads();
-  float t = (threadIdx.x < nw) ? sh[threadIdx.x] : 0.f;
-  if (w == 0) {
-    t = warp_sum(t);
-    if (lane == 0) sh[32] = t;
-  }
-  __syncthreads();
-  return sh[32];
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // K2: one warp per row. Two-pass (mean, then centred variance) like torch.nn.LayerNorm; eps = 1e-5
@@ -99,34 +73,11 @@ __global__ void layernorm_f16_kernel(const float* __restrict__ x, long long ldx,
         const float2 q01 = __half22float2(*reinterpret_cast<const __half2*>(&q.x)), q23 = __half22float2(*reinterpret_cast<const __half2*>(&q.y));
         y[0] -= q01.x; y[1] -= q01.y; y[2] -= q23.x; y[3] -= q23.y;
       }
-      __half h[4], l[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) split_hi_lo(y[j], h[j], l[j]);
-      *reinterpret_cast<uint2*>(orow + idx * 4) = make_uint2(pack_h2(h[0], h[1]), pack_h2(h[2], h[3]));
-      if (fmt == 1) {
-        *reinterpret_cast<uint2*>(orow + lo_off + idx * 4) = make_uint2(pack_h2(l[0], l[1]), pack_h2(l[2], l[3]));
-      } else if (fmt == 2) {  // e4m3 planes [lo8 (d bytes) | hi8 (d bytes)] for the fp8 cross terms of the next GEMM
-        uint8_t* f8 = reinterpret_cast<uint8_t*>(orow + lo_off);
-        const float sl = scale * 2048.f;
-        *reinterpret_cast<uint32_t*>(f8 + idx * 4) =
-            pack4_e4m3((y[0] - __half2float(h[0])) * sl, (y[1] - __half2float(h[1])) * sl, (y[2] - __half2float(h[2])) * sl,
-                       (y[3] - __half2float(h[3])) * sl);
-        *reinterpret_cast<uint32_t*>(f8 + dp + idx * 4) =
-            pack4_e4m3(__half2float(h[0]) * scale, __half2float(h[1]) * scale, __half2float(h[2]) * scale, __half2float(h[3]) * scale);
-      }
+      store_operand_quad(orow, lo_off, dp, fmt, scale, idx * 4, y);
     }
   }
   if (!PAD) return;
-  for (int c = d + lane * 4; c < dp; c += 128) {  // padding columns, 4 per lane (d and dp are multiples of 4)
-    *reinterpret_cast<uint2*>(orow + c) = make_uint2(0u, 0u);
-    if (fmt == 1) {
-      *reinterpret_cast<uint2*>(orow + lo_off + c) = make_uint2(0u, 0u);
-    } else if (fmt == 2) {
-      uint8_t* f8 = reinterpret_cast<uint8_t*>(orow + lo_off);
-      *reinterpret_cast<uint32_t*>(f8 + c) = 0u;
-      *reinterpret_cast<uint32_t*>(f8 + dp + c) = 0u;
-    }
-  }
+  for (int c = d + lane * 4; c < dp; c += 128) zero_operand_quad(orow, lo_off, dp, fmt, c);  // 4 per lane (d and dp are multiples of 4)
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -152,22 +103,15 @@ __global__ void embed_kernel(EmbedLaunch e) {
   const float* er = e.embed + static_cast<long long>(tok) * e.d;
   const float* pr = e.pos_table ? e.pos_table + static_cast<long long>(t + 2) * e.d : nullptr;
   float* xr = e.x + r * e.d;
-  float s = 0.f;
   for (int j = threadIdx.x; j < e.d; j += blockDim.x) {
     float v = er[j];
     if (e.token_dropout) v = (masked ? 0.f : v) * scale;
     if (pr) v += pr[j];
     xr[j] = v;
-    s += v;
   }
-  if (e.lnb_gamma) {
-    const float mean = block_sum(s, sh) / e.d;
-    float ss = 0.f;
-    for (int j = threadIdx.x; j < e.d; j += blockDim.x) {
-      const float c = xr[j] - mean;
-      ss += c * c;
-    }
-    const float rstd = rsqrtf(block_sum(ss, sh) / e.d + 1e-5f);
+  if (e.lnb_gamma) {  // every thread reads back the columns it wrote itself
+    float mean, rstd;
+    block_ln_stats(xr, e.d, sh, mean, rstd);
     for (int j = threadIdx.x; j < e.d; j += blockDim.x) xr[j] = (xr[j] - mean) * rstd * e.lnb_gamma[j] + e.lnb_beta[j];
   }
 }
@@ -179,15 +123,8 @@ __global__ void head_gather_ln_kernel(HeadLaunch h) {
   const int p = blockIdx.x;
   const long long src = h.all_rows ? p : static_cast<long long>(p) * h.T + h.row_in_seq[p];
   const float* xr = h.x + src * h.d;
-  float s = 0.f;
-  for (int j = threadIdx.x; j < h.d; j += blockDim.x) s += xr[j];
-  const float mean = block_sum(s, sh) / h.d;
-  float ss = 0.f;
-  for (int j = threadIdx.x; j < h.d; j += blockDim.x) {
-    const float c = xr[j] - mean;
-    ss += c * c;
-  }
-  const float rstd = rsqrtf(block_sum(ss, sh) / h.d + 1e-5f);
+  float mean, rstd;
+  block_ln_stats(xr, h.d, sh, mean, rstd);
   float* o = h.scratch_a + static_cast<long long>(p) * h.d;
   for (int j = threadIdx.x; j < h.d; j += blockDim.x) o[j] = (xr[j] - mean) * rstd * h.lna_g[j] + h.lna_b[j];
 }
@@ -241,36 +178,13 @@ __global__ void head_logits_kernel(HeadLaunch h) {
   float* logits = dyn + h.d;
   const int p = blockIdx.x;
   const float* xr = h.scratch_b + static_cast<long long>(p) * h.d;
-  float s = 0.f;
-  for (int j = threadIdx.x; j < h.d; j += blockDim.x) s += xr[j];
-  const float mean = block_sum(s, sh) / h.d;
-  float ss = 0.f;
-  for (int j = threadIdx.x; j < h.d; j += blockDim.x) {
-    const float c = xr[j] - mean;
-    ss += c * c;
-  }
-  const float rstd = rsqrtf(block_sum(ss, sh) / h.d + 1e-5f);
+  float mean, rstd;
+  block_ln_stats(xr, h.d, sh, mean, rstd);
   for (int j = threadIdx.x; j < h.d; j += blockDim.x) y[j] = (xr[j] - mean) * rstd * h.ln_g[j] + h.ln_b[j];
   __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int v = warp; v < h.vocab; v += nw) {
-    const float* wr = h.out_w + static_cast<long long>(v) * h.d;
-    float acc = 0.f;
-    for (int j = lane; j < h.d; j += 32) acc = fmaf(y[j], wr[j], acc);
-    acc = warp_sum(acc);
-    if (lane == 0) logits[v] = acc + h.out_b[v];
-  }
-  __syncthreads();
-  if (warp == 0) {
-    float m = -INFINITY;
-    for (int v = lane; v < h.vocab; v += 32) m = fmaxf(m, logits[v]);
-    m = warp_max(m);
-    float se = 0.f;
-    for (int v = lane; v < h.vocab; v += 32) se += expf(logits[v] - m);
-    se = warp_sum(se);
-    const float lse = m + logf(se);
-    for (int v = lane; v < h.vocab; v += 32) h.out[static_cast<long long>(p) * h.vocab + v] = logits[v] - lse;
-  }
+  const float lse = block_logits_lse(y, h.d, h.out_w, h.out_b, h.vocab, logits);
+  if (threadIdx.x < 32)
+    for (int v = threadIdx.x; v < h.vocab; v += 32) h.out[static_cast<long long>(p) * h.vocab + v] = logits[v] - lse;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -304,24 +218,7 @@ __global__ void __launch_bounds__(128) attn_single_query_kernel(const __half* __
   const __half* base = qkv + static_cast<long long>(b) * T * ld;
   auto load64 = [&](const __half* p, float (&v)[64]) {
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const uint4 hv = *reinterpret_cast<const uint4*>(p + c * 8);
-      const __half2* h2 = reinterpret_cast<const __half2*>(&hv);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(h2[i]);
-        v[c * 8 + 2 * i] = f.x; v[c * 8 + 2 * i + 1] = f.y;
-      }
-      if (lo_off > 0) {
-        const uint4 lv = *reinterpret_cast<const uint4*>(p + lo_off + c * 8);
-        const __half2* l2 = reinterpret_cast<const __half2*>(&lv);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float2 f = __half22float2(l2[i]);
-          v[c * 8 + 2 * i] += f.x; v[c * 8 + 2 * i + 1] += f.y;
-        }
-      }
-    }
+    for (int c = 0; c < 8; ++c) load_operand<8>(p + c * 8, lo_off, v + c * 8);
   };
   float q[64];
   load64(base + static_cast<long long>(row_sel[b]) * ld + h * 64, q);
@@ -346,23 +243,11 @@ __global__ void __launch_bounds__(128) attn_single_query_kernel(const __half* __
   const float sc = (m == -INFINITY) ? 0.f : __expf(m - mw);  // lanes that saw no key (T < 32) contribute nothing
   l = warp_sum(l * sc);
   const float rl = 1.f / l;
-  __half* orow = out + static_cast<long long>(b) * ldo + h * 64;
+  __half* orow = out + static_cast<long long>(b) * ldo;
 #pragma unroll
   for (int i = 0; i < 64; ++i) {
     const float v = warp_sum(acc[i] * sc) * rl;
-    if (lane == (i & 31)) {
-      __half hi, lo;
-      split_hi_lo(v, hi, lo);
-      orow[i] = hi;
-      if (out_fmt == 1) {
-        orow[out_lo_off + i] = lo;
-      } else if (out_fmt == 2) {  // e4m3 planes [lo8 (d) | hi8 (d)] of the row, head h at byte h*64 of each plane
-        uint8_t* f8 = reinterpret_cast<uint8_t*>(out + static_cast<long long>(b) * ldo + out_lo_off);
-        const float hf = __half2float(hi);
-        f8[h * 64 + i] = static_cast<uint8_t>(cvt_e4m3x2((v - hf) * out_scale * 2048.f, 0.f) & 0xff);
-        f8[d + h * 64 + i] = static_cast<uint8_t>(cvt_e4m3x2(hf * out_scale, 0.f) & 0xff);
-      }
-    }
+    if (lane == (i & 31)) store_operand_one(orow, out_lo_off, d, out_fmt, out_scale, h * 64 + i, v);
   }
 }
 
@@ -379,7 +264,7 @@ __global__ void gather_rows_kernel(const float* __restrict__ x, const int32_t* _
 int launch_attn_single_query(const __half* qkv, int64_t ld, int64_t lo_off, const int32_t* row_sel, int B, int T, int heads,
                              __half* out, int64_t ldo, int64_t out_lo_off, cudaStream_t s, int out_fmt, float out_scale) {
   if (B <= 0) return PG_OK;
-  if (out_fmt < 0) out_fmt = out_lo_off > 0 ? 1 : 0;
+  if (int rc = resolve_out_fmt(out_fmt, out_lo_off, out_scale, "attn_single_query")) return rc;
   attn_single_query_kernel<<<(B * heads + 3) / 4, 128, 0, s>>>(qkv, ld, lo_off, row_sel, B, T, heads, out, ldo, out_lo_off, out_fmt,
                                                               out_scale);
   PG_CUDA_OK(cudaGetLastError());
@@ -422,8 +307,7 @@ int launch_layernorm_f16(const float* x, int64_t ldx, const float* gamma, const 
   if (dp <= 0) dp = d;
   if (d % 4 || dp % 4 || dp < d || ldx % 4 || ldo % 4 || lo_off % 4) return set_error(PG_ERR_ARG, "layernorm: d, the plane width and pitches must be multiples of 4");
   if (base && dp != d) return set_error(PG_ERR_ARG, "layernorm: a base needs unpadded rows");
-  if (fmt < 0) fmt = lo_off > 0 ? 1 : 0;
-  if (fmt > 2 || (fmt >= 1 && lo_off <= 0) || (fmt == 2 && !(scale > 0.f))) return set_error(PG_ERR_ARG, "layernorm: bad output format");
+  if (int rc = resolve_out_fmt(fmt, lo_off, scale, "layernorm")) return rc;
   const int wpb = 8;
   const int grid = (rows + wpb - 1) / wpb;
 #define PG_LN(MAXV)                                                                                                               \

@@ -9,29 +9,17 @@
 // copies, ~5 % of a layer). The column attention needs nothing here: LayerNorm writes its rows in (b, c, r) order and the
 // attention kernel writes its output back in (b, r, c) order (attention_tc4.cu perm_C).
 #include "common.h"
-#include "ptx.cuh"
+#include "operand.cuh"
+#include "reduce.cuh"
 
 namespace pg {
 namespace {
-
-__device__ __forceinline__ float block_sum(float v, float* sh) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (l == 0) sh[w] = v;
-  __syncthreads();
-  float t = (l < nw) ? sh[l] : 0.f;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-  return t;
-}
 
 // One block per token row (b, r, c): x = LayerNorm_before(E[tok] + Pos[c + 2] + RowPos[r]); the token at (row 0, column positions[p])
 // is <mask>. msa_transformer.py:157-172; LearnedPositionalEmbedding positions = column + 2 (modules.py:254-271), no padding here.
 constexpr int EMB_MAXV = 8;  // d <= 256 * 8
 __global__ void msa_embed_kernel(MsaEmbedLaunch e) {
-  __shared__ float sh[32];
+  __shared__ float sh[33];
   const long long row = blockIdx.x;
   const int c = static_cast<int>(row % e.Cw);
   const int r = static_cast<int>((row / e.Cw) % e.R);
@@ -135,19 +123,14 @@ __global__ void tied_softmax_kernel(const float* __restrict__ S, long long lds, 
   const float* s = S + row * lds;
   float m = -INFINITY;
   for (int j = lane; j < C; j += 32) m = fmaxf(m, s[j] * scale);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  m = warp_max(m);
   float l = 0.f;
   for (int j = lane; j < C; j += 32) l += expf(s[j] * scale - m);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+  l = warp_sum(l);
   __half* p = P + row * ldp;
   for (int j = lane; j < Kp; j += 32) {
     const float v = (j < C) ? expf(s[j] * scale - m) / l : 0.f;
-    __half hi, lo;
-    split_hi_lo(v, hi, lo);
-    p[j] = hi;
-    if (np == 2) p[Kp + j] = lo;
+    store_operand_one(p, Kp, 0, np == 2 ? 1 : 0, 0.f, j, v);
   }
 }
 
@@ -181,17 +164,6 @@ __global__ void tied_scatter_out_kernel(const uint8_t* __restrict__ src, long lo
 // Its column attention needs the row-attention output at column sel[b] for every alignment row, and that needs ONE row of each head's
 // tied attention map: S1[b,h,j] = scale * sum_r q[b,r,sel_b,h,:] . k[b,r,j,h,:]. fp32 SIMT arithmetic on the fp16 hi(+lo) planes; K and
 // V are read once (HBM-bound), everything downstream runs on B*R (then B) rows.
-__device__ __forceinline__ float4 load4_hilo(const __half* p, long long lo_off) {
-  const uint2 hv = *reinterpret_cast<const uint2*>(p);
-  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&hv.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&hv.y));
-  float4 v = make_float4(a.x, a.y, b.x, b.y);
-  if (lo_off > 0) {
-    const uint2 lv = *reinterpret_cast<const uint2*>(p + lo_off);
-    const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&lv.x)), e = __half22float2(*reinterpret_cast<const __half2*>(&lv.y));
-    v.x += c.x; v.y += c.y; v.z += e.x; v.w += e.y;
-  }
-  return v;
-}
 // grid (C, B), block H * 16: thread = (head, 4 of the 64 head dims)
 __global__ void tied_col_scores_kernel(const __half* __restrict__ qkv, long long ldq, long long lo_off, const int32_t* __restrict__ sel,
                                        int R, int C, int H, float scale, float* __restrict__ S1) {
@@ -205,8 +177,10 @@ __global__ void tied_col_scores_kernel(const __half* __restrict__ qkv, long long
   const long long step = static_cast<long long>(C) * ldq;
   float acc = 0.f;
   for (int r = 0; r < (live ? R : 0); ++r) {
-    const float4 a = load4_hilo(q + r * step, lo_off), c = load4_hilo(k + r * step, lo_off);
-    acc = fmaf(a.x, c.x, fmaf(a.y, c.y, fmaf(a.z, c.z, fmaf(a.w, c.w, acc))));
+    float a[4], c[4];
+    load_operand<4>(q + r * step, lo_off, a);
+    load_operand<4>(k + r * step, lo_off, c);
+    acc = fmaf(a[0], c[0], fmaf(a[1], c[1], fmaf(a[2], c[2], fmaf(a[3], c[3], acc))));
   }
 #pragma unroll
   for (int o = 8; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o, 16);
@@ -219,12 +193,10 @@ __global__ void tied_col_softmax_kernel(float* __restrict__ S1, int G, int C) {
   float* s = S1 + static_cast<long long>(w) * C;
   float m = -INFINITY;
   for (int j = lane; j < C; j += 32) m = fmaxf(m, s[j]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  m = warp_max(m);
   float l = 0.f;
   for (int j = lane; j < C; j += 32) l += expf(s[j] - m);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+  l = warp_sum(l);
   for (int j = lane; j < C; j += 32) s[j] = expf(s[j] - m) / l;
 }
 // grid (R, B), block H * 16: ctx[(b, r)][h, :] = sum_j P1[b,h,j] v[b,r,j,h,:], written as an operand row (common.h formats)
@@ -237,29 +209,15 @@ __global__ void tied_col_context_kernel(const __half* __restrict__ qkv, long lon
   const int d = H * 64;
   const __half* v = qkv + (static_cast<long long>(b) * R + r) * C * ldq + 2 * d + h * 64 + l * 4;
   const float* p = P1 + (static_cast<long long>(b) * H + h) * C;
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};
   for (int j = 0; j < C; ++j) {
     const float pj = __ldg(p + j);
-    const float4 x = load4_hilo(v + j * ldq, lo_off);
-    acc.x = fmaf(pj, x.x, acc.x); acc.y = fmaf(pj, x.y, acc.y); acc.z = fmaf(pj, x.z, acc.z); acc.w = fmaf(pj, x.w, acc.w);
-  }
-  const long long row = static_cast<long long>(b) * R + r;
-  __half* o = out + row * ldo + h * 64 + l * 4;
-  const float y[4] = {acc.x, acc.y, acc.z, acc.w};
-  __half hi[4], lo[4];
+    float x[4];
+    load_operand<4>(v + j * ldq, lo_off, x);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) split_hi_lo(y[i], hi[i], lo[i]);
-  *reinterpret_cast<uint2*>(o) = make_uint2(pack_h2(hi[0], hi[1]), pack_h2(hi[2], hi[3]));
-  if (out_fmt == 1) {
-    *reinterpret_cast<uint2*>(o + out_lo_off) = make_uint2(pack_h2(lo[0], lo[1]), pack_h2(lo[2], lo[3]));
-  } else if (out_fmt == 2) {
-    uint8_t* f8 = reinterpret_cast<uint8_t*>(out + row * ldo + out_lo_off) + h * 64 + l * 4;
-    const float sl = out_scale * 2048.f;
-    *reinterpret_cast<uint32_t*>(f8) = pack4_e4m3((y[0] - __half2float(hi[0])) * sl, (y[1] - __half2float(hi[1])) * sl,
-                                                  (y[2] - __half2float(hi[2])) * sl, (y[3] - __half2float(hi[3])) * sl);
-    *reinterpret_cast<uint32_t*>(f8 + d) = pack4_e4m3(__half2float(hi[0]) * out_scale, __half2float(hi[1]) * out_scale,
-                                                      __half2float(hi[2]) * out_scale, __half2float(hi[3]) * out_scale);
+    for (int i = 0; i < 4; ++i) acc[i] = fmaf(pj, x[i], acc[i]);
   }
+  store_operand_quad(out + (static_cast<long long>(b) * R + r) * ldo, out_lo_off, d, out_fmt, out_scale, h * 64 + l * 4, acc);
 }
 // xr[(b, r)] = x[(b, r, sel[b])]: the residual rows of column sel[b]. grid (R, B)
 __global__ void msa_gather_col_kernel(const float* __restrict__ x, const int32_t* __restrict__ sel, int R, int C, int d, float* __restrict__ xr) {
@@ -331,6 +289,7 @@ int launch_tied_scatter_out(const __half* ot, int64_t ldo_t, __half* out, int64_
 int launch_tied_col_attention(const __half* qkv, int64_t ldq, int64_t lo_off, const int32_t* sel, int B, int R, int C, int H, float scale,
                               float* S1, __half* out, int64_t ldo, int64_t out_lo_off, int out_fmt, float out_scale, cudaStream_t s) {
   if (H * 16 > 1024 || B > 65535 || R > 2147483647 / 2) return set_error(PG_ERR_UNSUPPORTED, "tied attention: more than 64 heads or 65535 alignments per pass");
+  if (int rc = resolve_out_fmt(out_fmt, out_lo_off, out_scale, "tied attention")) return rc;
   tied_col_scores_kernel<<<dim3(C, B), (H * 16 + 31) / 32 * 32, 0, s>>>(qkv, ldq, lo_off, sel, R, C, H, scale, S1);
   tied_col_softmax_kernel<<<(B * H + 7) / 8, 256, 0, s>>>(S1, B * H, C);
   tied_col_context_kernel<<<dim3(R, B), (H * 16 + 31) / 32 * 32, 0, s>>>(qkv, ldq, lo_off, S1, R, C, H, out, ldo, out_lo_off, out_fmt, out_scale);

@@ -93,6 +93,13 @@ __device__ __forceinline__ uint32_t cvt_f16x2_rn(float lo_elem, float hi_elem) {
   return d;
 }
 
+// Same without saturation: a value beyond the fp16 range becomes inf.
+__device__ __forceinline__ uint32_t cvt_f16x2_rn_inf(float lo_elem, float hi_elem) {
+  uint32_t d;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi_elem), "f"(lo_elem));
+  return d;
+}
+
 // two fp32 -> packed e4m3 pair (round to nearest even, saturating at +-448): byte 0 = e0, byte 1 = e1
 __device__ __forceinline__ uint32_t cvt_e4m3x2(float e0, float e1) {
   uint16_t d;
@@ -216,20 +223,6 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// fp32 -> fp16 hi (+ residual lo), saturating so an outlier cannot become inf
-__device__ __forceinline__ __half f2h_sat(float v) {
-  unsigned short u;
-  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(u) : "f"(v));
-  return __ushort_as_half(u);
-}
-__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
-  return static_cast<uint32_t>(__half_as_ushort(a)) | (static_cast<uint32_t>(__half_as_ushort(b)) << 16);
-}
-__device__ __forceinline__ void split_hi_lo(float v, __half& hi, __half& lo) {
-  hi = f2h_sat(v);
-  lo = __float2half_rn(v - __half2float(hi));
 }
 
 }  // namespace pg

@@ -5,39 +5,13 @@
 //   ar_head_kernel        ln_f -> tied lm_head (no bias) -> log_softmax -> optional retrieval-prior fusion -> log p(next token)
 //                         (model_pytorch.py:612, :783, :806-830; utils/scoring_utils.py:121-128)
 //   seq_sum_kernel        per-sequence sum over the real (non-pad) predicted tokens, fixed order
-#include <cstdlib>
-
 #include "common.h"
-#include "ptx.cuh"
+#include "operand.cuh"
+#include "reduce.cuh"
 
 namespace pg {
 
 namespace {
-
-__device__ __forceinline__ float warp_sum_t(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max_t(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-__device__ __forceinline__ float block_sum_t(float v, float* sh) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-  v = warp_sum_t(v);
-  __syncthreads();
-  if (lane == 0) sh[w] = v;
-  __syncthreads();
-  float t = (threadIdx.x < nw) ? sh[threadIdx.x] : 0.f;
-  if (w == 0) {
-    t = warp_sum_t(t);
-    if (lane == 0) sh[32] = t;
-  }
-  __syncthreads();
-  return sh[32];
-}
 
 __global__ void gather_embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ wte, int d, int vocab,
                                     float* __restrict__ x) {
@@ -49,129 +23,26 @@ __global__ void gather_embed_kernel(const int32_t* __restrict__ ids, const float
   for (int j = threadIdx.x; j < d / 4; j += blockDim.x) dst[j] = src[j];
 }
 
-// One thread per (sequence, 8-channel chunk, block of CONV_TB time steps): the 8x(7 taps + bias) coefficients and a 7-row
-// sliding window live in registers, so every input row is read once per block instead of once per tap.
+// Depthwise conv: the block stages a [CV_T + 6 rows] x [CV_C channels] tile (hi and lo planes) in shared memory with cp.async —
+// every byte of the tile is in flight at once, independent of the arithmetic — then each thread walks down time for ONE channel pair
+// with a 7-deep register window (16 tap registers, so several blocks fit per SM). One warp = the 64 channels of one head, hence
+// uniform in its conv group.
 // taps: [3 (q,k,v)][4 groups][64 channels][8] = 7 look-back taps + bias.
 // in/out: [B*T, ld] fp16 with columns [q | k | v] (+ lo plane at lo_off). out[t] = bias + sum_o tap[o] * in[t - o].
-constexpr int CONV_TB = 16;
-__global__ void qkv_conv_kernel(const __half* __restrict__ in, __half* __restrict__ out, long long ld, long long lo_off, int B, int T,
-                                int heads, const float* __restrict__ taps, float qscale) {
-  const int d = heads * 64;
-  const int chunks = 3 * d / 8;
-  const int tblocks = (T + CONV_TB - 1) / CONV_TB;
-  const long long gid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (gid >= static_cast<long long>(B) * tblocks * chunks) return;
-  const int ck = static_cast<int>(gid % chunks);  // fastest: neighbouring threads read neighbouring 16-byte chunks of a row
-  const int tb = static_cast<int>((gid / chunks) % tblocks);
-  const int b = static_cast<int>(gid / (static_cast<long long>(chunks) * tblocks));
-  const int c0 = ck * 8;
-  const int which = c0 / d, head = (c0 % d) / 64, ch0 = c0 % 64;
-  const int group = head / (heads / 4);
-  const int klen = group == 0 ? 1 : 2 * group + 1;
-  const float4* tp4 = reinterpret_cast<const float4*>(taps + ((static_cast<long long>(which) * 4 + group) * 64 + ch0) * 8);
-  float tap[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4 lo4 = __ldg(tp4 + 2 * i), hi4 = __ldg(tp4 + 2 * i + 1);
-    tap[i][0] = lo4.x; tap[i][1] = lo4.y; tap[i][2] = lo4.z; tap[i][3] = lo4.w;
-    tap[i][4] = hi4.x; tap[i][5] = hi4.y; tap[i][6] = hi4.z; tap[i][7] = hi4.w;
-  }
-  const float sc = which == 0 ? qscale : 1.f;
-  const long long row0 = static_cast<long long>(b) * T;
-  const int t0 = tb * CONV_TB;
-  float win[7][8];  // win[o] = input row t - o
-#pragma unroll
-  for (int o = 0; o < 7; ++o)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) win[o][i] = 0.f;
-  auto decode = [&](const uint4& hv, const uint4& lv, float (&v)[8]) {
-    const __half2* h2 = reinterpret_cast<const __half2*>(&hv);
-    const __half2* l2 = reinterpret_cast<const __half2*>(&lv);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float2 f = __half22float2(h2[i]);
-      v[2 * i] = f.x; v[2 * i + 1] = f.y;
-      if (lo_off > 0) {
-        const float2 e = __half22float2(l2[i]);
-        v[2 * i] += e.x; v[2 * i + 1] += e.y;
-      }
-    }
-  };
-  auto fetch = [&](int t, uint4& hv, uint4& lv) {
-    const __half* src = in + (row0 + t) * ld + c0;
-    hv = *reinterpret_cast<const uint4*>(src);
-    if (lo_off > 0) lv = *reinterpret_cast<const uint4*>(src + lo_off);
-  };
-  // prime the window with the klen-1 rows before the block (zeros before the start of the sequence): all loads first
-  {
-    uint4 hv[6], lv[6];
-#pragma unroll
-    for (int o = 1; o < 7; ++o)
-      if (o < klen && t0 - o >= 0) fetch(t0 - o, hv[o - 1], lv[o - 1]);
-#pragma unroll
-    for (int o = 1; o < 7; ++o)
-      if (o < klen && t0 - o >= 0) decode(hv[o - 1], lv[o - 1], win[o]);
-  }
-  // CONV_LD rows are requested before any of them is consumed: the kernel is HBM-bound and a thread that waits for one 16-byte
-  // load per step leaves the memory system idle (measured 3.5x off the copy roofline before this batching)
-  constexpr int CONV_LD = 4;
-#pragma unroll 1
-  for (int tt0 = 0; tt0 < CONV_TB; tt0 += CONV_LD) {
-    if (t0 + tt0 >= T) break;
-    uint4 hv[CONV_LD], lv[CONV_LD];
-#pragma unroll
-    for (int u = 0; u < CONV_LD; ++u)
-      if (t0 + tt0 + u < T) fetch(t0 + tt0 + u, hv[u], lv[u]);
-#pragma unroll
-    for (int u = 0; u < CONV_LD; ++u) {
-      const int t = t0 + tt0 + u;
-      if (t < T) {
-        decode(hv[u], lv[u], win[0]);
-        float acc[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float a = tap[i][7];
-#pragma unroll
-          for (int o = 0; o < 7; ++o) a = fmaf(tap[i][o], win[o][i], a);  // taps beyond klen are zero
-          acc[i] = a * sc;
-        }
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          __half h0, l0, h1, l1;
-          split_hi_lo(acc[2 * i], h0, l0);
-          split_hi_lo(acc[2 * i + 1], h1, l1);
-          hi[i] = pack_h2(h0, h1);
-          lo[i] = pack_h2(l0, l1);
-        }
-        __half* dst = out + (row0 + t) * ld + c0;
-        *reinterpret_cast<uint4*>(dst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        if (lo_off > 0) *reinterpret_cast<uint4*>(dst + lo_off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-#pragma unroll
-        for (int o = 6; o > 0; --o)
-#pragma unroll
-          for (int i = 0; i < 8; ++i) win[o][i] = win[o - 1][i];
-      }
-    }
-  }
-}
-
-// v2 of the depthwise conv (default; PG_CONV_V2=0 falls back to qkv_conv_kernel): the block stages a [CV_T + 6 rows] x [CV_C channels] tile (hi and lo planes) in shared
-// memory with cp.async — every byte of the tile is in flight at once, independent of the arithmetic — then each thread walks down
-// time for ONE channel pair with a 7-deep register window (16 tap registers instead of 64, so several blocks fit per SM). One warp =
-// the 64 channels of one head, hence uniform in its conv group. Same FMA order as qkv_conv_kernel: bit-identical results.
+// Blocks are numbered channel tile fastest, then time tile, then sequence.
 constexpr int CV_T = 64;
 constexpr int CV_C = 256;
 // `prefix` (optional): the 6 raw q/k/v rows that precede row 0 of every sequence (same pitch and planes) — the look-back of a
 // suffix whose earlier rows were computed elsewhere (exact wild-type-prefix reuse); null = start of sequence (zeros).
 template <int NP>
-__global__ void __launch_bounds__(128) qkv_conv2_kernel(const __half* __restrict__ in, __half* __restrict__ out, long long ld,
-                                                        long long lo_off, int T, int heads, const float* __restrict__ taps, float qscale,
-                                                        const __half* __restrict__ prefix) {
+__global__ void __launch_bounds__(128) qkv_conv_kernel(const __half* __restrict__ in, __half* __restrict__ out, long long ld,
+                                                       long long lo_off, int T, int heads, const float* __restrict__ taps, float qscale,
+                                                       const __half* __restrict__ prefix) {
   extern __shared__ __align__(16) uint8_t cv_smem[];
   constexpr int ROWS = CV_T + 6;
   constexpr int ROWB = CV_C * 2;                      // bytes per staged row and plane
-  const int c0 = blockIdx.x * CV_C, t0 = blockIdx.y * CV_T, b = blockIdx.z;
+  const int ctiles = 3 * heads * 64 / CV_C, ttiles = (T + CV_T - 1) / CV_T;
+  const int c0 = (blockIdx.x % ctiles) * CV_C, t0 = (blockIdx.x / ctiles % ttiles) * CV_T, b = blockIdx.x / (ctiles * ttiles);
   const long long row0 = static_cast<long long>(b) * T;
   const uint32_t sbase = smem_u32(cv_smem);
   // ---- stage: rows t0-6 .. t0+CV_T-1 (zero-filled outside [0, T)), 32 16-byte chunks per row and plane ----
@@ -207,15 +78,8 @@ __global__ void __launch_bounds__(128) qkv_conv2_kernel(const __half* __restrict
   const float sc = which == 0 ? qscale : 1.f;
   cp_async_wait<0>();
   __syncthreads();
-  auto rd = [&](int r, float (&v)[2]) {
-    const __half2 hv = *reinterpret_cast<const __half2*>(cv_smem + r * ROWB + threadIdx.x * 4);
-    const float2 f = __half22float2(hv);
-    v[0] = f.x; v[1] = f.y;
-    if (NP == 2) {
-      const __half2 lv = *reinterpret_cast<const __half2*>(cv_smem + (ROWS + r) * ROWB + threadIdx.x * 4);
-      const float2 e = __half22float2(lv);
-      v[0] += e.x; v[1] += e.y;
-    }
+  auto rd = [&](int r, float (&v)[2]) {  // staged row r of this thread's channel pair; the lo plane lies ROWS staged rows further
+    load_operand<2>(reinterpret_cast<const __half*>(cv_smem + r * ROWB) + 2 * threadIdx.x, NP == 2 ? ROWS * CV_C : 0, v);
   };
   float win[7][2];  // win[o] = input row t - o
 #pragma unroll
@@ -232,12 +96,7 @@ __global__ void __launch_bounds__(128) qkv_conv2_kernel(const __half* __restrict
       for (int o = 0; o < 7; ++o) a = fmaf(tap[i][o], win[o][i], a);  // taps beyond the group's kernel length are zero
       acc[i] = a * sc;
     }
-    __half h0, l0, h1, l1;
-    split_hi_lo(acc[0], h0, l0);
-    split_hi_lo(acc[1], h1, l1);
-    __half* dst = out + (row0 + t0 + tt) * ld + c;
-    *reinterpret_cast<uint32_t*>(dst) = pack_h2(h0, h1);
-    if (NP == 2) *reinterpret_cast<uint32_t*>(dst + lo_off) = pack_h2(l0, l1);
+    store_operand_pair(out + (row0 + t0 + tt) * ld, lo_off, 0, NP == 2 ? 1 : 0, 0.f, c, acc[0], acc[1]);
 #pragma unroll
     for (int o = 6; o > 0; --o) {
       win[o][0] = win[o - 1][0];
@@ -285,34 +144,13 @@ __global__ void ar_head_kernel(ArHeadParams p) {
     return;
   }
   const float* xr = p.x + r * p.d;
-  float s = 0.f;
-  for (int j = threadIdx.x; j < p.d; j += blockDim.x) s += xr[j];
-  const float mean = block_sum_t(s, sh) / p.d;
-  float ss = 0.f;
-  for (int j = threadIdx.x; j < p.d; j += blockDim.x) {
-    const float c = xr[j] - mean;
-    ss += c * c;
-  }
-  const float rstd = rsqrtf(block_sum_t(ss, sh) / p.d + 1e-5f);
+  float mean, rstd;
+  block_ln_stats(xr, p.d, sh, mean, rstd);
   for (int j = threadIdx.x; j < p.d; j += blockDim.x) y[j] = (xr[j] - mean) * rstd * p.lnf_g[j] + p.lnf_b[j];
   __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int v = warp; v < p.vocab; v += nw) {
-    const float* wr = p.wte + static_cast<long long>(v) * p.d;
-    float acc = 0.f;
-    for (int j = lane; j < p.d; j += 32) acc = fmaf(y[j], wr[j], acc);
-    acc = warp_sum_t(acc);
-    if (lane == 0) logits[v] = acc;
-  }
-  __syncthreads();
-  if (warp == 0) {
-    float m = -INFINITY;
-    for (int v = lane; v < p.vocab; v += 32) m = fmaxf(m, logits[v]);
-    m = warp_max_t(m);
-    float se = 0.f;
-    for (int v = lane; v < p.vocab; v += 32) se += expf(logits[v] - m);
-    se = warp_sum_t(se);
-    const float lse = m + logf(se);
+  const float lse = block_logits_lse(y, p.d, p.wte, nullptr, p.vocab, logits);
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
     if (p.f.out_logprobs)
       for (int v = lane; v < p.vocab; v += 32) p.f.out_logprobs[r * p.vocab + v] = fuse_logp(p.f, p.vocab, r, v, logits[v] - lse);
     if (lane == 0) {
@@ -331,7 +169,7 @@ __global__ void seq_sum_kernel(const float* __restrict__ tok_logp, const int32_t
   const int n = lens[b] - 1;
   float s = 0.f;
   for (int t = lane; t < n; t += 32) s += tok_logp[static_cast<long long>(b) * T + t];
-  s = warp_sum_t(s);
+  s = warp_sum(s);
   if (lane == 0) out[b] = s;
 }
 
@@ -346,29 +184,23 @@ int launch_gather_embed(const int32_t* ids, const float* wte, long long rows, in
 
 int launch_qkv_conv(const __half* in, __half* out, int64_t ld, int64_t lo_off, int B, int T, int heads, const float* taps,
                     float qscale, cudaStream_t s, const __half* prefix) {
-  const long long n = static_cast<long long>(B) * ((T + CONV_TB - 1) / CONV_TB) * (3 * heads * 64 / 8);
+  const long long ctiles = 3 * heads * 64 / CV_C, ttiles = (T + CV_T - 1) / CV_T;
+  const long long n = B * ttiles * ctiles;
   if (n <= 0) return PG_OK;
   if (heads % 4) return set_error(PG_ERR_ARG, "qkv_conv: heads must be a multiple of 4");
-  // default: the shared-memory-tiled kernel (2.3-2.5x faster: 116 vs 294 ms per 300-mutant L=1500 assay in f16); PG_CONV_V2=0 selects v1
-  static const bool v2 = !(getenv("PG_CONV_V2") && getenv("PG_CONV_V2")[0] == '0');
-  if (v2 && B <= 65535) {
-    const dim3 grid(3 * heads * 64 / CV_C, (T + CV_T - 1) / CV_T, B);
-    const int np = lo_off > 0 ? 2 : 1;
-    const int smem = np * (CV_T + 6) * CV_C * 2;
-    int dev = 0;
-    PG_CUDA_OK(cudaGetDevice(&dev));
-    static bool attr[64] = {};  // the attribute is per device
-    if (dev < 64 && !attr[dev]) {
-      PG_CUDA_OK(cudaFuncSetAttribute(qkv_conv2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * (CV_T + 6) * CV_C * 2));
-      attr[dev] = true;
-    }
-    if (np == 2) qkv_conv2_kernel<2><<<grid, 128, smem, s>>>(in, out, ld, lo_off, T, heads, taps, qscale, prefix);
-    else qkv_conv2_kernel<1><<<grid, 128, smem, s>>>(in, out, ld, lo_off, T, heads, taps, qscale, prefix);
-    PG_CUDA_OK(cudaGetLastError());
-    return PG_OK;
+  if (n > 0x7FFFFFFFll) return set_error(PG_ERR_ARG, "qkv_conv: grid too large");
+  const unsigned grid = static_cast<unsigned>(n);
+  const int np = lo_off > 0 ? 2 : 1;
+  const int smem = np * (CV_T + 6) * CV_C * 2;
+  int dev = 0;
+  PG_CUDA_OK(cudaGetDevice(&dev));
+  static bool attr[64] = {};  // the attribute is per device
+  if (dev < 64 && !attr[dev]) {
+    PG_CUDA_OK(cudaFuncSetAttribute(qkv_conv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * (CV_T + 6) * CV_C * 2));
+    attr[dev] = true;
   }
-  if (prefix) return set_error(PG_ERR_UNSUPPORTED, "qkv_conv: prefix look-back is only implemented in the tiled kernel");
-  qkv_conv_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(in, out, ld, lo_off, B, T, heads, taps, qscale);
+  if (np == 2) qkv_conv_kernel<2><<<grid, 128, smem, s>>>(in, out, ld, lo_off, T, heads, taps, qscale, prefix);
+  else qkv_conv_kernel<1><<<grid, 128, smem, s>>>(in, out, ld, lo_off, T, heads, taps, qscale, prefix);
   PG_CUDA_OK(cudaGetLastError());
   return PG_OK;
 }

@@ -1,0 +1,81 @@
+"""Outputs of every model family on seeded synthetic models, in one .npz: run it on two builds of the library and compare the files
+with --compare. A change that only moves device code between files must leave every array np.array_equal.
+
+    python scripts/check_refactor_bits.py out.npz
+    python scripts/check_refactor_bits.py --compare a.npz b.npz
+
+ESM-1v scores in f16x3 / f16f8 / f16d / f16, an ESM2 of the 35M release's shape (480 wide, 24-wide heads: the padded LayerNorm) in
+f16f8, Tranception mutant scores with and without prefix reuse and rows with a three-way retrieval fusion in f16x3 / f16f8, and a
+two-layer MSA Transformer table (a full and a pruned last layer) in f16x3 / f16f8."""
+import sys
+
+import numpy as np
+
+
+def collect():
+    import pandas as pd
+    from proteingym_b200 import checkpoint, msa_engine, synth
+    from proteingym_b200.esm_engine import EsmScorer
+    from proteingym_b200.tranception_engine import TranceptionScorer
+    out = {}
+    seq = synth.random_protein(200, 3)
+    muts = synth.sample_mutants(seq, 400, 4, multi_frac=0.2)
+    for name, arch, modes in (("esm1v", synth.EsmArch("esm1v", 3, 256, 4, 1024), ("f16x3", "f16f8", "f16d", "f16")),
+                              ("esm2_35m", synth.EsmArch("esm2", 2, 480, 20, 1920), ("f16f8",))):
+        st = checkpoint.normalise_synth_state(arch, synth.make_esm_state(arch, seed=1))
+        for mode in modes:
+            sc = EsmScorer(checkpoint.config_from_synth(arch), st, precision=mode)
+            out[f"{name}.{mode}"] = np.asarray(sc.score_assay(seq, muts))
+            sc.close()
+    arch = synth.TranceptionArch(2, 768, 12, 3072)
+    cfg = {"n_embd": 768, "n_head": 12, "n_layer": 2, "n_ctx": 1024, "n_inner": 3072, "vocab_size": 25, "layer_norm_epsilon": 1e-5,
+           "activation_function": "squared_relu"}
+    st = {k[len("transformer."):]: v for k, v in synth.make_tranception_state(arch, 5).items() if k.startswith("transformer.")}
+    wt = synth.random_protein(400, 6)
+    m = synth.sample_mutants(wt, 120, 7)
+    dms = pd.DataFrame({"mutant": m, "mutated_sequence": [synth.apply_mutant(wt, x) for x in m]})
+    L = 300
+    rng = np.random.RandomState(8)
+    prior = np.log(rng.dirichlet(np.ones(25), size=L)).astype(np.float32)
+    prior2 = np.log(rng.dirichlet(np.ones(25), size=L)).astype(np.float32)
+    for mode in ("f16x3", "f16f8"):
+        for reuse in (True, False):
+            sc = TranceptionScorer(cfg, st, precision=mode)
+            sc.prefix_reuse = reuse
+            df = sc.score_mutants(dms, wt)
+            out[f"tranception.{mode}.reuse{int(reuse)}"] = df.select_dtypes("number").to_numpy()
+            sc.close()
+        sc = TranceptionScorer(cfg, st, precision=mode)
+        sums, rows = sc.sequence_logprobs([wt[:L]], prior=prior, windows=[(0, L)], alpha=0.6, msa_start=40, msa_end=L - 30, prior2=prior2,
+                                          beta=0.3, first_col=5, return_rows=True)
+        out[f"tranception.{mode}.fusion3"] = rows[0]
+        out[f"tranception.{mode}.fusion3.sum"] = sums
+        sc.close()
+    arch = synth.MsaArch(2, 256, 4, 1024)
+    cfg = checkpoint.config_from_msa_synth(arch)
+    st = checkpoint.normalise_msa_synth_state(arch, synth.make_msa_state(arch, 9))
+    toks = msa_engine.tokenize_alignment(synth.random_alignment(synth.random_protein(90, 10), 24, seed=11))
+    R, Cc = toks.shape
+    pos = np.arange(1, Cc, 7).astype(np.int32)
+    for mode in ("f16x3", "f16f8"):
+        sc = msa_engine.MsaScorer(cfg, st, precision=mode, max_rows=msa_engine.default_max_rows(cfg, R, Cc, want=4))
+        out[f"msa.{mode}"] = sc.masked_marginal_rows(toks, pos).cpu().numpy()
+        sc.close()
+    return out
+
+
+def main():
+    if sys.argv[1] == "--compare":
+        a, b = np.load(sys.argv[2]), np.load(sys.argv[3])
+        bad = [k for k in a.files if k not in b.files or not np.array_equal(a[k], b[k], equal_nan=True)] + [k for k in b.files if k not in a.files]
+        for k in a.files:
+            print(f"{k:40s} {a[k].shape} {'DIFFERENT' if k in bad else 'equal'}")
+        sys.exit(1 if bad else 0)
+    arrays = collect()
+    assert all(np.isfinite(v).any() for v in arrays.values())
+    np.savez(sys.argv[1], **arrays)
+    print(f"wrote {len(arrays)} arrays to {sys.argv[1]}")
+
+
+if __name__ == "__main__":
+    main()

@@ -3,13 +3,10 @@ every predicted row and vocabulary column, at 4, 12, 16 and 20 heads (one ALiBi 
 head groups otherwise), at the 64-row attention / conv tile edges, the conv halo rows, the 128-row prefix tile and n_ctx, in ragged
 batches, at Tranception-L depth and with the retrieval fusions. Then the exact wild-type-prefix reuse (pg_ar_prefix_begin /
 pg_ar_loglik_prefix): its rows are bit-identical to the plain path's; and the plain rows do not depend on how the sequences are
-split into passes or on which depthwise-conv kernel runs. Cases and bounds: tests/tranception_fp64_cases.py;
+split into passes, also when one pass holds more than 65 535 sequences. Cases and bounds: tests/tranception_fp64_cases.py;
 tests/test_tranception_fp64_bounds_cpu.py shows the bounds would catch an emulated kernel fault."""
 import ctypes as C
 import functools
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -198,26 +195,21 @@ def test_pass_split_is_bit_identical(precision):
     assert all(np.array_equal(x, y) for x, y in zip(a, b))
 
 
-def test_conv_v1_rows_equal_v2_rows(tmp_path):
-    """The per-thread depthwise conv (PG_CONV_V2=0, also the kernel of passes over more than 65535 sequences) gives the tiled
-    kernel's bits. The kernel is chosen once per process, so the v1 rows come from a child process."""
-    ids = ["h12-ragged", "h20-t1024"]
-    tests_dir = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(tests_dir)
-    env = dict(os.environ, PG_CONV_V2="0", PYTHONPATH=os.pathsep.join(p for p in (root, tests_dir, os.environ.get("PYTHONPATH")) if p))
-    path = tmp_path / "v1.npz"
-    code = f"import tranception_fp64_cases as c; c.dump_plain_rows({str(path)!r}, {ids!r})"
-    flags = ["-s"] if sys.flags.no_user_site else []
-    r = subprocess.run([sys.executable, *flags, "-c", code], env=env, cwd=root, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    v1 = np.load(path)
-    for cid in ids:
-        case = BY_ID[cid]
-        for mode in MODES:
-            sc = case.scorer(mode)
-            try:
-                _, rows = case.run(sc)
-            finally:
-                sc.close()
-            for i, row in enumerate(rows):
-                assert np.array_equal(v1[f"{cid}.{mode}.{i}"], row), (cid, mode, i)
+@pytest.mark.parametrize("precision", ["f16x3", "f16"])  # the two-plane and the one-plane instance of the depthwise conv
+def test_one_pass_over_65535_sequences(precision):
+    """65 600 sequences of two and three tokens on the 4-head model as ONE pass (no kernel of the pass may depend on a 16-bit
+    grid dimension for the sequence index), against the same sequences in three passes of under 30 000."""
+    aa = "ACDEFGHIKLMNPQRSTVWY"
+    seqs = [aa[i % 20] if i % 3 else "" for i in range(65600)]
+    case = BY_ID["h4-t3"]
+    one = case.scorer(precision, max_rows=1 << 18)
+    split = case.scorer(precision, max_rows=90000)  # 30 000 sequences of T = 3 rows
+    try:
+        a_sums, a = one.sequence_logprobs(seqs, chunk_rows=1 << 18, return_rows=True)
+        b_sums, b = split.sequence_logprobs(seqs, chunk_rows=1 << 18, return_rows=True)
+    finally:
+        one.close()
+        split.close()
+    assert np.isfinite(a_sums).all() and len(set(a_sums.tolist())) > 1
+    assert np.array_equal(a_sums, b_sums)
+    assert all(np.array_equal(x, y) for x, y in zip(a, b))

@@ -146,19 +146,3 @@ BY_ID = {c.id: c for c in CASES}
 def max_err(got, ref):
     return max(float(np.abs(np.asarray(g, dtype=np.float64) - r).max()) for g, r in zip(got, ref))
 
-
-def dump_plain_rows(path, ids):
-    """Writes the plain rows of the cases ``ids`` in every mode to ``path`` (npz): run in a child process to compare conv kernels,
-    which are chosen once per process."""
-    arrays = {}
-    for cid in ids:
-        case = BY_ID[cid]
-        for mode in MODES:
-            sc = case.scorer(mode)
-            try:
-                _, rows = case.run(sc)
-            finally:
-                sc.close()
-            for i, r in enumerate(rows):
-                arrays[f"{cid}.{mode}.{i}"] = r
-    np.savez(path, **arrays)

@@ -27,9 +27,16 @@ enum pg_arch {
   PG_ARCH_ESM2 = 1,  /* ESM2: rotary (esm/model/esm2.py:40-74) */
   PG_ARCH_TRANCEPTION = 2, /* Tranception decoder: grouped ALiBi, depthwise-conv q/k/v, relu^2 MLP
                               (tranception/model_pytorch.py:90-632); max_positions = n_ctx, vocab = 25 */
-  PG_ARCH_MSA = 3          /* MSA Transformer: tied row attention + column attention + FFN per layer, learned column positions and
+  PG_ARCH_MSA = 3,         /* MSA Transformer: tied row attention + column attention + FFN per layer, learned column positions and
                               (when the state holds "msa_position_embedding") row positions (esm/model/msa_transformer.py:100-222,
                               esm/axial_attention.py) */
+  PG_ARCH_ESMC = 4         /* ESM C (evoscale esm/models/esmc.py:117-173): pre-LN blocks without linear biases, q/k LayerNorm over the
+                              full width + rotary, SwiGLU MLP (ffn_dim = the SwiGLU hidden width f; fc1 is [2f, d]), residual branches
+                              divided by sqrt(layers / 36), untied 64-way output head; vocab 64, heads = embed_dim / 64, token_dropout
+                              = emb_ln_before = 0, max_positions unused. Weights: the reference state-dict keys verbatim plus
+                              "rotary.cos" / "rotary.sin" [T, 32]. Windows (compute_fitness.py:346-409 re-tokenises each one as
+                              <cls> slice <eos>) are the caller's: pass one token row per distinct window, concatenated, with
+                              win_start[p] = that row's offset and positions[p] = offset + index within the row. */
 };
 
 /* Tensor-core operand precision. The reference is strict fp32 (SURVEY.md §0.4). Every operand is an fp16 pair hi + lo.
@@ -185,7 +192,10 @@ int pg_score_mutants(const float* table, int32_t n_rows, int32_t vocab, const in
  *   epi 2: resid[M, ldr] (fp32) += acc + bias
  *   epi 3: as 0, with rotary applied to the first 2*rot_dim columns ([q | k], heads of 64; esm/rotary_embedding.py:11-20),
  *          token index = row % rot_T, cos/sin tables [rot_T, 32] fp32 in rot_cos/rot_sin.
- *   epi 4: as 0 with squared ReLU relu(x)^2 (tranception/activations.py:79-84). bias may be NULL (no bias). */
+ *   epi 4: as 0 with squared ReLU relu(x)^2 (tranception/activations.py:79-84). bias may be NULL (no bias).
+ *   epi 5: SwiGLU silu(g) * v (esm/layers/blocks.py:21-43): w rows interleaved in blocks of 8 (rows 16i..16i+7 = gate rows 8i..8i+7,
+ *          rows 16i+8..16i+15 = up rows 8i..8i+7; N % 16 == 0); the output is N/2 columns wide (planes of N/2 columns at out_lo_off,
+ *          out_fmt 2 needs N/2 % 64 == 0), column 8i + c = silu(acc[16i + c]) * acc[16i + 8 + c]. */
 typedef struct {
   const void* a; int64_t lda;
   const void* w; int64_t ldw;

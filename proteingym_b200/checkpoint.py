@@ -20,7 +20,7 @@ MASK_IDX = 32
 
 @dataclass
 class EsmConfig:
-    arch: str            # "esm1b" (ESM-1b / ESM-1v, learned positions) | "esm2" (rotary) | "msa" (MSA Transformer)
+    arch: str            # "esm1b" (ESM-1b / ESM-1v, learned positions) | "esm2" (rotary) | "msa" (MSA Transformer) | "esmc" (ESM C)
     layers: int
     embed_dim: int
     heads: int
@@ -154,4 +154,79 @@ def rotary_tables(inv_freq: torch.Tensor, T: int):
     arange(T) with the checkpoint's ``inv_freq`` buffer, then cos / sin. Both halves of the 64-wide table are equal."""
     t = torch.arange(T).type_as(inv_freq)
     freqs = torch.einsum("i,j->ij", t, inv_freq.float())
+    return freqs.cos().contiguous(), freqs.sin().contiguous()
+
+
+# ESM C releases (evoscale esm/pretrained.py:65-98; f = swiglu_correction_fn(8/3, d), esm/layers/blocks.py:15-17):
+# name -> (layers, d_model, SwiGLU hidden width f, weight file under the snapshot root)
+ESMC_RELEASES = {"esmc_300M": (30, 960, 2560, "data/weights/esmc_300m_2024_12_v0.pth"),
+                 "esmc_600M": (36, 1152, 3072, "data/weights/esmc_600m_2024_12_v0.pth")}
+ESMC_HF_REPOS = {"esmc_300M": "EvolutionaryScale/esmc-300m-2024-12", "esmc_600M": "EvolutionaryScale/esmc-600m-2024-12"}
+
+
+def esmc_config_from_state(state: dict) -> EsmConfig:
+    """Dims of an ESM C state dict from its shapes: d from ``embed.weight`` [64, d], layers from the block keys, f from
+    ``ffn.1.weight`` [2f, d]; checks every key the scorer reads and its shape."""
+    d = int(state["embed.weight"].shape[1])
+    if state["embed.weight"].shape[0] != 64 or d % 64:
+        raise ValueError("ESM C: embed.weight must be [64, d] with d a multiple of 64 (head_dim 64)")
+    layers = 1 + max(int(k.split(".")[2]) for k in state if k.startswith("transformer.blocks."))
+    f = int(state["transformer.blocks.0.ffn.1.weight"].shape[0]) // 2
+    want = {"embed.weight": (64, d), "transformer.norm.weight": (d,), "sequence_head.0.weight": (d, d), "sequence_head.0.bias": (d,),
+            "sequence_head.2.weight": (d,), "sequence_head.2.bias": (d,), "sequence_head.3.weight": (64, d), "sequence_head.3.bias": (64,)}
+    for i in range(layers):
+        p = f"transformer.blocks.{i}."
+        want.update({p + "attn.layernorm_qkv.0.weight": (d,), p + "attn.layernorm_qkv.0.bias": (d,),
+                     p + "attn.layernorm_qkv.1.weight": (3 * d, d), p + "attn.q_ln.weight": (d,), p + "attn.k_ln.weight": (d,),
+                     p + "attn.out_proj.weight": (d, d), p + "ffn.0.weight": (d,), p + "ffn.0.bias": (d,),
+                     p + "ffn.1.weight": (2 * f, d), p + "ffn.3.weight": (d, f)})
+    for k, shape in want.items():
+        if k not in state:
+            raise ValueError(f"ESM C state dict: missing {k}")
+        if tuple(state[k].shape) != shape:
+            raise ValueError(f"ESM C state dict: {k} has shape {tuple(state[k].shape)}, expected {shape}")
+    return EsmConfig("esmc", layers, d, d // 64, f, False, False, 1024, 64)
+
+
+def resolve_esmc_weights(model_type: str, model_path: str | None = None) -> str:
+    """``--model_path`` as the .pth file itself or a snapshot directory holding ``data/weights/esmc_*_2024_12_v0.pth``; without it, the
+    local Hugging Face cache (HF_HUB_CACHE / HF_HOME / ~/.cache/huggingface). Never downloads."""
+    rel = ESMC_RELEASES[model_type][3]
+    if model_path:
+        p = Path(model_path)
+        if p.is_file():
+            return str(p)
+        if (p / rel).is_file():
+            return str(p / rel)
+        raise FileNotFoundError(f"{model_path}: neither an ESM C .pth file nor a directory holding {rel}")
+    hub = os.environ.get("HF_HUB_CACHE") or os.path.join(os.environ.get("HF_HOME") or os.path.expanduser("~/.cache/huggingface"), "hub")
+    snaps = Path(hub) / ("models--" + ESMC_HF_REPOS[model_type].replace("/", "--")) / "snapshots"
+    found = sorted(snaps.glob("*/" + rel)) if snaps.is_dir() else []
+    if not found:
+        raise FileNotFoundError(f"{model_type} weights not found in the local Hugging Face cache ({snaps}); pass --model_path "
+                                f"(a {os.path.basename(rel)} file or a snapshot directory). Weights are never downloaded.")
+    return str(found[-1])
+
+
+def load_esmc_checkpoint(model_type: str, model_path: str | None = None):
+    """-> (EsmConfig with arch "esmc", state: dict[str, fp32 CPU tensor] with the reference key names, score column name
+    ``{model_type}_score``). Reads the .pth state dict (weights_only) and checks its dims against the release table."""
+    if model_type not in ESMC_RELEASES:
+        raise ValueError(f"unknown ESM C release {model_type!r} (esmc_300M, esmc_600M)")
+    path = resolve_esmc_weights(model_type, model_path)
+    raw = torch.load(path, map_location="cpu", weights_only=True)
+    state = {k: v.detach().to(torch.float32).contiguous() for k, v in raw.items()}
+    conf = esmc_config_from_state(state)
+    layers, d, f, _ = ESMC_RELEASES[model_type]
+    if (conf.layers, conf.embed_dim, conf.ffn_dim) != (layers, d, f):
+        raise ValueError(f"{path}: dims (layers {conf.layers}, d {conf.embed_dim}, f {conf.ffn_dim}) are not {model_type}'s "
+                         f"({layers}, {d}, {f})")
+    return conf, state, f"{model_type}_score"
+
+
+def esmc_rotary_tables(T: int = 1024):
+    """cos/sin [T, 32] of ESM C's rotary (esm/layers/rotary.py:136-165): inv_freq = 1 / 10000^(arange(0, 64, 2) / 64) in fp32,
+    torch.outer with arange(T) in fp32, then cos / sin."""
+    inv_freq = 1.0 / (10000 ** (torch.arange(0, 64, 2, dtype=torch.float32) / 64))
+    freqs = torch.outer(torch.arange(T, dtype=torch.float32), inv_freq)
     return freqs.cos().contiguous(), freqs.sin().contiguous()

@@ -158,6 +158,7 @@ struct Layer {
   float *ln1g = nullptr, *ln1b = nullptr, *ln2g = nullptr, *ln2b = nullptr;
   float *iqkv = nullptr, *io = nullptr, *i1 = nullptr, *i2 = nullptr;  // PG_PREC_F16F8: 1 / t_n per weight row
   float* conv_taps = nullptr;  // Tranception: [3][4][64][8]
+  float *qlng = nullptr, *klng = nullptr;  // ESM C: q_ln / k_ln weights [d]
 };
 
 // Power-of-two scales the producers of A operands apply to their e4m3 planes (PG_PREC_F16F8; gemm_tc.cu header). e4m3 keeps
@@ -168,6 +169,7 @@ constexpr float S_LN = 4.f;     // LayerNorm output            -> QKV / fc1 GEMM
 constexpr float S_ATT = 4.f;    // attention output            -> out_proj GEMM
 constexpr float S_GELU = 2.f;   // GELU(fc1) (ESM)             -> fc2 GEMM           (up to 224)
 constexpr float S_RELU2 = 1.f;  // relu(fc1)^2 (Tranception)   -> fc2 GEMM           (up to 448)
+constexpr float S_SWIGLU = 2.f; // silu(g) * v (ESM C)         -> fc2 GEMM           (up to 224)
 
 // Operand formats of a precision mode (common.h fmt 0 / 1 / 2), fixed at pg_create. Pitches and offsets in fp16 elements.
 // Widths (DESIGN.md §3): residual rows d; GEMM-input rows of width d (LayerNorm outputs) dk = d rounded up to 64, zero-padded; q/k/v
@@ -223,6 +225,18 @@ __global__ void expand_slots_kernel(const float* __restrict__ src, int n_src, in
   dst[i] = (r >= 0 && c >= 0) ? src[static_cast<long long>(r) * k_src + c] : 0.f;
 }
 
+// ESM C fc1 [2f, K] = [gate (f rows) ; up (f rows)] -> rows interleaved in blocks of 8 (rows 16i..16i+7 = gate rows 8i..8i+7, rows
+// 16i+8..16i+15 = up rows 8i..8i+7): the SwiGLU epilogue (gemm_tc.cu, epi 5) then finds each gate column and its up column in one
+// thread's fragment. A row permutation, so one e4m3 scale per matrix still covers it.
+__global__ void interleave_gate_up_kernel(const float* __restrict__ src, int f, int K, float* __restrict__ dst) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= 2LL * f * K) return;
+  const int r = static_cast<int>(i / K), k = static_cast<int>(i % K);
+  const int blk = r >> 4, c = r & 15;
+  const int sr = c < 8 ? 8 * blk + c : f + 8 * blk + (c - 8);
+  dst[i] = src[static_cast<long long>(sr) * K + k];
+}
+
 }  // namespace
 }  // namespace pg
 
@@ -235,6 +249,7 @@ struct pg_handle_s {
   std::vector<pg::Layer> layers;
   float *embed = nullptr, *pos = nullptr, *lnbg = nullptr, *lnbb = nullptr, *lnag = nullptr, *lnab = nullptr;
   float *hdw = nullptr, *hdb = nullptr, *hlng = nullptr, *hlnb = nullptr, *hbias = nullptr;
+  float* outw = nullptr;  // untied output matrix [vocab, d] (ESM C sequence_head.3); null = the tied embedding
   float *rot_cos = nullptr, *rot_sin = nullptr;
   int rot_rows = 0;
   // workspace
@@ -329,7 +344,7 @@ GemmLaunch proj_gemm(pg_handle h, const Layer& L, Proj p, const __half* a, float
   switch (p) {
     case QKV: g.w = L.wqkv; g.w_inv = L.iqkv; g.bias = L.bqkv; g.N = 3 * da; g.K = dk; break;
     case OUT: g.w = L.wo; g.w_inv = L.io; g.bias = L.bo; g.N = d; g.K = da; break;
-    case FC1: g.w = L.w1; g.w_inv = L.i1; g.bias = L.b1; g.N = f; g.K = dk; break;
+    case FC1: g.w = L.w1; g.w_inv = L.i1; g.bias = L.b1; g.N = h->desc.arch == PG_ARCH_ESMC ? 2 * f : f; g.K = dk; break;  // ESM C: gate|up
     case FC2: g.w = L.w2; g.w_inv = L.i2; g.bias = L.b2; g.N = d; g.K = f; break;
   }
   g.a = a; g.lda = static_cast<int64_t>(g.K) * h->op.np; g.ldw = g.lda; g.M = M; g.nseg = h->op.nseg;
@@ -337,13 +352,15 @@ GemmLaunch proj_gemm(pg_handle h, const Layer& L, Proj p, const __half* a, float
   return g;
 }
 // ... written as operand rows to `out` through epilogue `epi`: q/k/v in the q/k/v format (epi 0, or 3: rotary embedding over windows of
-// rot_T rows), fc1 in the GEMM-input format (epi: the MLP's activation, out_scale: the e4m3 scale of its output).
+// rot_T rows), fc1 in the GEMM-input format (epi: the MLP's activation, out_scale: the e4m3 scale of its output; SwiGLU, epi 5, writes
+// half as many columns as the GEMM has).
 int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int M, __half* out, cudaStream_t s, int epi = 0,
         float out_scale = 0.f, int rot_T = 0) {
   GemmLaunch g = proj_gemm(h, L, p, a, a_scale, M);
+  const int n_out = epi == 5 ? g.N / 2 : g.N;
   g.epi = epi;
-  g.out = out; g.ldo = static_cast<int64_t>(g.N) * h->op.np; g.out_fmt = p == QKV ? h->op.qfmt : h->op.afmt;
-  g.out_lo_off = g.out_fmt ? g.N : 0; g.out_scale = out_scale;
+  g.out = out; g.ldo = static_cast<int64_t>(n_out) * h->op.np; g.out_fmt = p == QKV ? h->op.qfmt : h->op.afmt;
+  g.out_lo_off = g.out_fmt ? n_out : 0; g.out_scale = out_scale;
   if (epi == 3) { g.rot_cos = h->rot_cos; g.rot_sin = h->rot_sin; g.rot_T = rot_T; g.rot_dim = h->op.da; }  // q and k slots
   ProfScope ps(p, s);
   return launch_gemm(g, s);
@@ -357,12 +374,23 @@ int lin_add(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale,
 }
 
 // MLP block on M fp32 residual rows x: x += fc2(act(fc1(LN2(x)))), through operand rows `ab` (LayerNorm output) and `fb` (hidden
-// layer). act: fc1's activation epilogue (1 GELU, 4 relu^2); act_scale: the e4m3 scale of its output (S_GELU, S_RELU2).
+// layer). act: fc1's activation epilogue (1 GELU, 4 relu^2, 5 SwiGLU); act_scale: the e4m3 scale of its output (S_GELU, S_RELU2,
+// S_SWIGLU).
 int mlp(pg_handle h, const Layer& L, float* x, int M, __half* ab, __half* fb, int act, float act_scale, cudaStream_t s) {
   int rc = ln(h, x, L.ln2g, L.ln2b, M, ab, s);
   if (!rc) rc = lin(h, L, FC1, ab, S_LN, M, fb, s, act, act_scale);
   if (!rc) rc = lin_add(h, L, FC2, fb, act_scale, M, x, s);
   return rc;
+}
+
+// The activation of the ESM-family MLPs (fc1 epilogue) and the e4m3 scale of its output: erf-GELU, or SwiGLU for ESM C.
+struct Act { int epi; float scale; };
+Act esm_act(pg_handle h) { return h->desc.arch == PG_ARCH_ESMC ? Act{5, S_SWIGLU} : Act{1, S_GELU}; }
+
+// ESM C after the QKV projection of M rows in h->qkv (windows of T rows): q/k LayerNorm + rotary + q scaling, in place.
+int qk_norm(pg_handle h, const Layer& L, int M, int T, cudaStream_t s) {
+  ProfScope ps(CAT_LN, s);
+  return launch_qk_ln_rotary(h->qkv, h->op.ldq, h->op.lo_q, M, h->desc.heads, L.qlng, L.klng, h->rot_cos, h->rot_sin, T, s);
 }
 
 // Attention over B sequences of T rows, q/k/v rows `qkv` -> operand rows `out` in the GEMM-input format; bidirectional and without
@@ -386,7 +414,7 @@ int last_layer(pg_handle h, const Layer& L, const int32_t* emit_rows, int Bc, in
     rc = launch_attn_single_query(h->qkv, o.ldq, o.lo_q, emit_rows, Bc, T, h->desc.heads, h->cabuf, o.ldat, o.lo_at, s, o.afmt, S_ATT);
     if (!rc && gather) rc = launch_gather_rows(h->x, emit_rows, Bc, T, h->desc.embed_dim, h->xc, s); }
   if (!rc) rc = lin_add(h, L, OUT, h->cabuf, S_ATT, Bc, h->xc, s);
-  if (!rc) rc = mlp(h, L, h->xc, Bc, h->cabuf, h->cfbuf, 1, S_GELU, s);
+  if (!rc) rc = mlp(h, L, h->xc, Bc, h->cabuf, h->cfbuf, esm_act(h).epi, esm_act(h).scale, s);
   return rc;
 }
 
@@ -403,12 +431,13 @@ int forward_rows(pg_handle h, const int32_t* tokens, int n_tokens, const int32_t
     const Layer& L = h->layers[l];
     if ((rc = ln(h, h->x, L.ln1g, L.ln1b, rows, h->abuf, s))) return rc;
     if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s, rotary ? 3 : 0, 0.f, T))) return rc;
+    if (D.arch == PG_ARCH_ESMC && (rc = qk_norm(h, L, rows, T, s))) return rc;  // every row: the pruned layer reads all keys
     if (emit_rows && l == D.layers - 1) return last_layer(h, L, emit_rows, Bc, T, true, s);
     const AttnLaunch a = attn_args(h, h->qkv, h->abuf, Bc, T);
     { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
     if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
-    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, 1, S_GELU, s))) return rc;
+    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, esm_act(h).epi, esm_act(h).scale, s))) return rc;
   }
   return PG_OK;
 }
@@ -714,7 +743,7 @@ HeadLaunch head_args(pg_handle h, int T) {
   HeadLaunch hl{};
   hl.x = h->x; hl.d = h->desc.embed_dim; hl.T = T;
   hl.lna_g = h->lnag; hl.lna_b = h->lnab; hl.dense_w = h->hdw; hl.dense_b = h->hdb;
-  hl.ln_g = h->hlng; hl.ln_b = h->hlnb; hl.out_w = h->embed; hl.out_b = h->hbias; hl.vocab = h->desc.vocab;
+  hl.ln_g = h->hlng; hl.ln_b = h->hlnb; hl.out_w = h->outw ? h->outw : h->embed; hl.out_b = h->hbias; hl.vocab = h->desc.vocab;
   hl.scratch_a = h->hs_a; hl.scratch_b = h->hs_b;
   return hl;
 }
@@ -819,8 +848,9 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     if (D.embed_dim != D.heads * 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: head_dim must be 64");
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
   }
-  if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA)
+  if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC)
     return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
+  if (D.arch == PG_ARCH_ESMC && D.heads > 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: the ESM C q/k LayerNorm kernel holds at most 24 heads");
   if (D.arch == PG_ARCH_TRANCEPTION && D.heads % 4) return set_error(PG_ERR_UNSUPPORTED, "pg_create: Tranception needs heads % 4 == 0 (model_pytorch.py:129-131)");
   if (D.precision != PG_PREC_F16 && D.precision != PG_PREC_F16X3 && D.precision != PG_PREC_F16F8 && D.precision != PG_PREC_F16D)
     return set_error(PG_ERR_ARG, "pg_create: unknown precision");
@@ -844,14 +874,18 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   int rc = PG_OK;
   auto A = [&](auto** p, size_t n) { if (!rc) rc = dev_alloc(h, p, n); };
   h->layers.resize(D.layers);
+  const bool esmc = D.arch == PG_ARCH_ESMC;
+  const int f1 = esmc ? 2 * f : f;  // rows of fc1: ESM C holds the SwiGLU gate and up halves
   for (auto& L : h->layers) {
     A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
-    A(&L.w1, static_cast<size_t>(f) * dk * np); A(&L.w2, static_cast<size_t>(d) * f * np);
-    A(&L.bqkv, 3 * da); A(&L.bo, d); A(&L.b1, f); A(&L.b2, d);
+    A(&L.w1, static_cast<size_t>(f1) * dk * np); A(&L.w2, static_cast<size_t>(d) * f * np);
+    if (!esmc) { A(&L.bqkv, 3 * da); A(&L.bo, d); A(&L.b1, f); A(&L.b2, d); }  // ESM C linear layers have no bias (null = none)
     A(&L.ln1g, d); A(&L.ln1b, d); A(&L.ln2g, d); A(&L.ln2b, d);
-    if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); A(&L.i1, f); A(&L.i2, d); }
+    if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); A(&L.i1, f1); A(&L.i2, d); }
     if (D.arch == PG_ARCH_TRANCEPTION) A(&L.conv_taps, 3 * 4 * 64 * 8);
+    if (esmc) { A(&L.qlng, d); A(&L.klng, d); }
   }
+  if (esmc) A(&h->outw, static_cast<size_t>(D.vocab) * d);
   if (D.arch == PG_ARCH_MSA) {
     h->col_layers.resize(D.layers);
     for (auto& L : h->col_layers) {
@@ -956,6 +990,58 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     copy(h->lnag, get("ln_f.weight", d, 1), d);
     copy(h->lnab, get("ln_f.bias", d, 1), d);
     copy(h->slopes, get("alibi_slopes", D.heads, 1), D.heads);
+  } else if (D.arch == PG_ARCH_ESMC) {
+    // evoscale key names (esm/models/esmc.py:63-76, layers/blocks.py:35-43,95-110, layers/attention.py:28-39). Residual branches are
+    // divided by s = sqrt(layers / 36) (transformer_stack.py:48-50, blocks.py:150-160): 1/s is folded into out_proj and fc2 here.
+    const float rs = static_cast<float>(1.0 / std::sqrt(static_cast<double>(D.layers) / 36.0));
+    for (int l = 0; l < D.layers; ++l) {
+      Layer& L = h->layers[l];
+      const std::string p = "transformer.blocks." + std::to_string(l) + ".";
+      copy(L.ln1g, get(p + "attn.layernorm_qkv.0.weight", d, 1), d);
+      copy(L.ln1b, get(p + "attn.layernorm_qkv.0.bias", d, 1), d);
+      pack(L.wqkv, L.iqkv, {get(p + "attn.layernorm_qkv.1.weight", 3 * d, d)}, 3 * d, d);
+      copy(L.qlng, get(p + "attn.q_ln.weight", d, 1), d);
+      copy(L.klng, get(p + "attn.k_ln.weight", d, 1), d);
+      pack(L.wo, L.io, {{get(p + "attn.out_proj.weight", d, d), rs}}, d, d);
+      copy(L.ln2g, get(p + "ffn.0.weight", d, 1), d);
+      copy(L.ln2b, get(p + "ffn.0.bias", d, 1), d);
+      const float* w1 = get(p + "ffn.1.weight", 2 * f, d);
+      if (w1) {  // gate / up rows interleaved in blocks of 8 for the SwiGLU epilogue
+        float* t = nullptr;
+        const cudaError_t e = cudaMalloc(&t, static_cast<size_t>(2) * f * d * sizeof(float));
+        if (e != cudaSuccess) {
+          if (!exp_err) exp_err = e;
+        } else {
+          expanded.p.push_back(t);
+          const long long tot = 2LL * f * d;
+          interleave_gate_up_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(w1, f, d, t);
+          pack(L.w1, L.i1, {t}, 2 * f, d);
+        }
+      }
+      pack(L.w2, L.i2, {{get(p + "ffn.3.weight", d, f), rs}}, d, f);
+    }
+    copy(h->embed, get("embed.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    copy(h->lnag, get("transformer.norm.weight", d, 1), d);
+    PG_CUDA_OK(cudaMemset(h->lnab, 0, static_cast<size_t>(d) * sizeof(float)));  // the final norm has no bias
+    copy(h->hdw, get("sequence_head.0.weight", d, d), static_cast<size_t>(d) * d);
+    copy(h->hdb, get("sequence_head.0.bias", d, 1), d);
+    copy(h->hlng, get("sequence_head.2.weight", d, 1), d);
+    copy(h->hlnb, get("sequence_head.2.bias", d, 1), d);
+    copy(h->outw, get("sequence_head.3.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    copy(h->hbias, get("sequence_head.3.bias", D.vocab, 1), D.vocab);
+    auto it = by_name.find("rotary.cos");
+    auto is = by_name.find("rotary.sin");
+    if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != 32 || is->second->shape[1] != 32 ||
+        is->second->shape[0] != it->second->shape[0]) {
+      missing += "rotary.cos/rotary.sin[T,32] ";
+    } else {
+      h->rot_rows = static_cast<int>(it->second->shape[0]);
+      int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
+      if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
+      if (rc) return rc;
+      copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * 32);
+      copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * 32);
+    }
   } else {
     const int hd = d / D.heads, dk = h->op.dk, da = h->op.da;
     // head_dim^-1/2 (multihead_attention.py:103,261), folded into the fp32 q weights and bias: 0.125 (exact) for head_dim 64
@@ -1069,7 +1155,8 @@ int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, co
   if (P < 0 || T <= 0 || T > n_tokens) return fail(h, PG_ERR_ARG, "pg_masked_marginals: bad P/T");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions)
     return fail(h, PG_ERR_ARG, "pg_masked_marginals: window longer than the learned position table (modules.py:256-260)");
-  if (h->desc.arch == PG_ARCH_ESM2 && T > h->rot_rows) return fail(h, PG_ERR_ARG, "pg_masked_marginals: window longer than rotary tables");
+  if ((h->desc.arch == PG_ARCH_ESM2 || h->desc.arch == PG_ARCH_ESMC) && T > h->rot_rows)
+    return fail(h, PG_ERR_ARG, "pg_masked_marginals: window longer than rotary tables");
   if (T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_masked_marginals: window longer than workspace (raise max_rows)");
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1130,7 +1217,8 @@ int pg_forward_logprobs(pg_handle h, const int32_t* tokens, int32_t n_tokens, in
   if (h->desc.arch == PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an MSA Transformer (use pg_msa_masked_marginals)");
   if (!tokens || !out_logprobs || T <= 0 || win_start < 0 || win_start + T > n_tokens) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: bad arguments");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than the learned position table");
-  if (h->desc.arch == PG_ARCH_ESM2 && T > h->rot_rows) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than rotary tables");
+  if ((h->desc.arch == PG_ARCH_ESM2 || h->desc.arch == PG_ARCH_ESMC) && T > h->rot_rows)
+    return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than rotary tables");
   if (T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than workspace");
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);

@@ -158,6 +158,10 @@ namespace pg {
 int launch_attn_single_query(const __half* qkv, int64_t ld, int64_t lo_off, const int32_t* row_sel, int B, int T, int heads,
                              __half* out, int64_t ldo, int64_t out_lo_off, cudaStream_t s, int out_fmt = -1, float out_scale = 0.f);
 int launch_gather_rows(const float* x, const int32_t* row_sel, int B, int T, int d, float* xc, cudaStream_t s);
+// ESM C: in place on q/k rows (q at column 0, k at heads*64, fp16 hi [+ lo at lo_off]): weight-only LayerNorm over the full width, then
+// rotary per 64-wide head (t = row % T, cos/sin [T, 32]) and q *= 1/8 (elementwise.cu).
+int launch_qk_ln_rotary(__half* qkv, int64_t ld, int64_t lo_off, int rows, int heads, const float* q_gamma, const float* k_gamma,
+                        const float* rot_cos, const float* rot_sin, int T, cudaStream_t s);
 int launch_gather_embed(const int32_t* ids, const float* wte, long long rows, int d, int vocab, float* x, cudaStream_t s);
 int launch_qkv_conv(const __half* in, __half* out, int64_t ld, int64_t lo_off, int B, int T, int heads, const float* taps,
                     float qscale, cudaStream_t s, const __half* prefix = nullptr);

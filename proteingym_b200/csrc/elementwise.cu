@@ -251,6 +251,59 @@ __global__ void __launch_bounds__(128) attn_single_query_kernel(const __half* __
   }
 }
 
+// ESM C attention (esm/layers/attention.py:50-60, rotary.py:36-65): q = q_ln(q) and k = k_ln(k) — LayerNorm over the full width d,
+// weight only, eps 1e-5 — then rotate-half rotary on every 64-wide head (token index t = row % T, tables [T, 32]) and q *= 64^-1/2
+// (exact). In place on the fp16 hi [+ lo] q/k rows (fmt 0 / 1) the QKV GEMM wrote: the statistics span the whole row, 7.5-9 of the
+// GEMM's 128-column tiles, so they cannot live in its epilogue. One warp per (row, q or k); lane l holds columns 64h + l and
+// 64h + 32 + l of every head h, which is exactly a rotary pair.
+template <int MAXH>
+__global__ void __launch_bounds__(256) qk_ln_rotary_kernel(__half* __restrict__ qkv, long long ld, long long lo_off, int rows, int heads,
+                                                           const float* __restrict__ q_gamma, const float* __restrict__ k_gamma,
+                                                           const float* __restrict__ rot_cos, const float* __restrict__ rot_sin, int T) {
+  const long long w = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w >= 2LL * rows) return;
+  const long long row = w >> 1;
+  const int is_k = static_cast<int>(w & 1), lane = threadIdx.x & 31, d = heads * 64;
+  __half* p = qkv + row * ld + is_k * d;
+  const float* g = is_k ? k_gamma : q_gamma;
+  float a[MAXH], b[MAXH];
+  float s = 0.f;
+#pragma unroll
+  for (int h = 0; h < MAXH; ++h) {
+    if (h < heads) {
+      a[h] = __half2float(p[64 * h + lane]);
+      b[h] = __half2float(p[64 * h + 32 + lane]);
+      if (lo_off > 0) {
+        a[h] += __half2float(p[lo_off + 64 * h + lane]);
+        b[h] += __half2float(p[lo_off + 64 * h + 32 + lane]);
+      }
+      s += a[h] + b[h];
+    }
+  }
+  const float mean = warp_sum(s) / d;
+  float ss = 0.f;
+#pragma unroll
+  for (int h = 0; h < MAXH; ++h) {
+    if (h < heads) {
+      const float x = a[h] - mean, y = b[h] - mean;
+      ss += x * x + y * y;
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(ss) / d + 1e-5f);
+  const int t = static_cast<int>(row % T);
+  const float co = __ldg(rot_cos + t * 32 + lane), si = __ldg(rot_sin + t * 32 + lane);
+  const float sc = is_k ? 1.f : 0.125f;
+  const int fmt = lo_off > 0 ? 1 : 0;
+#pragma unroll
+  for (int h = 0; h < MAXH; ++h) {
+    if (h < heads) {
+      const float x = (a[h] - mean) * rstd * __ldg(g + 64 * h + lane), y = (b[h] - mean) * rstd * __ldg(g + 64 * h + 32 + lane);
+      store_operand_one(p, lo_off, d, fmt, 0.f, 64 * h + lane, (x * co - y * si) * sc);
+      store_operand_one(p, lo_off, d, fmt, 0.f, 64 * h + 32 + lane, (y * co + x * si) * sc);
+    }
+  }
+}
+
 __global__ void gather_rows_kernel(const float* __restrict__ x, const int32_t* __restrict__ row_sel, int T, int d,
                                    float* __restrict__ xc) {
   const int b = blockIdx.x;
@@ -267,6 +320,18 @@ int launch_attn_single_query(const __half* qkv, int64_t ld, int64_t lo_off, cons
   if (int rc = resolve_out_fmt(out_fmt, out_lo_off, out_scale, "attn_single_query")) return rc;
   attn_single_query_kernel<<<(B * heads + 3) / 4, 128, 0, s>>>(qkv, ld, lo_off, row_sel, B, T, heads, out, ldo, out_lo_off, out_fmt,
                                                               out_scale);
+  PG_CUDA_OK(cudaGetLastError());
+  return PG_OK;
+}
+
+int launch_qk_ln_rotary(__half* qkv, int64_t ld, int64_t lo_off, int rows, int heads, const float* q_gamma, const float* k_gamma,
+                        const float* rot_cos, const float* rot_sin, int T, cudaStream_t s) {
+  if (rows <= 0) return PG_OK;
+  if (heads <= 0 || heads > 24 || T <= 0 || !q_gamma || !k_gamma || !rot_cos || !rot_sin)
+    return set_error(PG_ERR_ARG, "qk_ln_rotary: needs 1..24 heads of 64, T > 0, q/k weights and rotary tables");
+  const long long warps = 2LL * rows;
+  qk_ln_rotary_kernel<24><<<static_cast<unsigned>((warps + 7) / 8), 256, 0, s>>>(qkv, ld, lo_off, rows, heads, q_gamma, k_gamma, rot_cos,
+                                                                               rot_sin, T);
   PG_CUDA_OK(cudaGetLastError());
   return PG_OK;
 }

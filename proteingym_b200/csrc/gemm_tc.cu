@@ -23,7 +23,7 @@
 //   warpgroup 0   TMA producer (one elected thread of warp 0): cp.async.bulk.tensor 2D tiles (128 rows x 128 B of A, 128 rows
 //                 x 128 B of W, 128B swizzle; a row of 128 B is 64 fp16 or 128 e4m3 along K) into a 6-stage ring; 40 registers
 //   warpgroups 1-2 consumers, rows [0, 64) and [64, 128) of the tile: wgmma m64n128 (K = 16 fp16 / 32 e4m3: 32 B of each row) x4
-//                 per stage, then bias / erf-GELU / relu^2 / rotary and fp16 hi [+ fp16 lo | + e4m3 planes for the next GEMM]
+//                 per stage, then bias / erf-GELU / relu^2 / rotary / SwiGLU and fp16 hi [+ fp16 lo | + e4m3 planes for the next GEMM]
 //                 stored straight from the accumulator fragments, or added into the fp32 residual stream (one owner per element)
 // Roofline: tensor bound. Algorithmic FLOPs = 2*M*N*K; issued tensor-pipe work = x1 / x2 / x3 by mode.
 #include <cstdlib>
@@ -89,6 +89,15 @@ __device__ __forceinline__ float gelu_erf(float x) {
   npoly = npoly * t;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"((x * x) * -0.72134752044448170368f));
   return fmaf(ax * 0.5f, fmaf(npoly, e, 1.0f), x * 0.5f);
+}
+
+// SiLU (ESM C SwiGLU, esm/layers/blocks.py:21-33): g / (1 + e^-g) with e^-g from MUFU.EX2 (ex2.approx.ftz, <= 2 ulp) and the quotient
+// from MUFU.RCP (rcp.approx.ftz, <= 1 ulp): relative error <= ~4 ulp (5e-7) over the range; for g < -88 e^-g is inf and the result 0.
+__device__ __forceinline__ float silu(float g) {
+  float e, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(g * -1.4426950408889634074f));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+  return g * r;
 }
 
 // Bias, activation and store of one consumer thread's fragment: rows row0 and row0 + 8, columns col0 + 8j (+1), j < 16.
@@ -165,6 +174,30 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
         } else {
           r[col] += acc[4 * j + 2 * h];
           if (col + 1 < p.N) r[col + 1] += acc[4 * j + 2 * h + 1];
+        }
+      }
+    } else if (EPI == 5) {
+      // SwiGLU: W rows come interleaved in blocks of 8 (api.cu), so block j (even) of the fragment holds gate columns and block j + 1
+      // the matching up columns. silu(gate) * up goes to output column (col / 16) * 8 + col % 8 of an N/2-wide operand row
+      // (planes of N/2 columns at out_lo_off; N % 16 == 0).
+      __half* o = p.out + row * p.ldo;
+      const int nh = p.N >> 1;
+      uint8_t* f8 = reinterpret_cast<uint8_t*>(o + p.out_lo_off);
+      const float sh = p.out_scale, sl = p.out_scale * LO8_GAIN;
+#pragma unroll
+      for (int j = 0; j < 16; j += 2) {
+        const int col = col0 + 8 * j;
+        if (col >= p.N) continue;
+        const int oc = ((col >> 4) << 3) + (col & 7);
+        const float x0 = silu(acc[4 * j + 2 * h]) * acc[4 * (j + 1) + 2 * h];
+        const float x1 = silu(acc[4 * j + 2 * h + 1]) * acc[4 * (j + 1) + 2 * h + 1];
+        const uint32_t hi = cvt_f16x2_rn(x0, x1);
+        const float2 hf = unpack_h2(hi);
+        *reinterpret_cast<uint32_t*>(o + oc) = hi;
+        if (p.out_fmt == 1) *reinterpret_cast<uint32_t*>(o + p.out_lo_off + oc) = cvt_f16x2_rn(x0 - hf.x, x1 - hf.y);
+        else if (p.out_fmt == 2) {
+          *reinterpret_cast<uint16_t*>(f8 + oc) = static_cast<uint16_t>(cvt_e4m3x2((x0 - hf.x) * sl, (x1 - hf.y) * sl));
+          *reinterpret_cast<uint16_t*>(f8 + nh + oc) = static_cast<uint16_t>(cvt_e4m3x2(hf.x * sh, hf.y * sh));
         }
       }
     } else {
@@ -469,7 +502,9 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return set_error(PG_ERR_ARG, "gemm: empty problem");
   if (g.K % BK) return set_error(PG_ERR_ARG, "gemm: K must be a multiple of 64");
   if (g.nseg < 1 || g.nseg > 3) return set_error(PG_ERR_ARG, "gemm: nseg must be 1, 2 (fp16 + e4m3 cross terms) or 3");
-  if (g.epi < 0 || g.epi > 4) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
+  if (g.epi < 0 || g.epi > 5) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
+  if (g.epi == 5 && (g.N % 16 || (g.out_fmt == 2 && (g.N / 2) % 64) || g.grp_rows_a || (g.out_fmt >= 1 && g.out_lo_off < g.N / 2)))
+    return set_error(PG_ERR_ARG, "gemm: the SwiGLU epilogue needs N % 16 == 0 (N/2 % 64 == 0 for out_fmt 2), no groups, planes >= N/2 apart");
   if (g.epi == 2 ? !g.resid : !g.out) return set_error(PG_ERR_ARG, "gemm: missing output");
   if (g.epi == 3 && (!g.rot_cos || !g.rot_sin || g.rot_T <= 0 || g.rot_dim % 64)) return set_error(PG_ERR_ARG, "gemm: bad rotary args");
   if (g.nseg == 2 && (!g.w_inv || !(g.a_scale > 0.f))) return set_error(PG_ERR_ARG, "gemm: nseg 2 needs w_inv[N] and a_scale > 0");
@@ -491,7 +526,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
 #define PG_SET_SMEM(E)                                                                                           \
   PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM)); \
   PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM))
-    PG_SET_SMEM(0); PG_SET_SMEM(1); PG_SET_SMEM(2); PG_SET_SMEM(3); PG_SET_SMEM(4);
+    PG_SET_SMEM(0); PG_SET_SMEM(1); PG_SET_SMEM(2); PG_SET_SMEM(3); PG_SET_SMEM(4); PG_SET_SMEM(5);
 #undef PG_SET_SMEM
     attr_set[dev] = true;
   }
@@ -579,7 +614,8 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
     case 1: e = PG_LAUNCH(1); break;
     case 2: e = PG_LAUNCH(2); break;
     case 3: e = PG_LAUNCH(3); break;
-    default: e = PG_LAUNCH(4); break;
+    case 4: e = PG_LAUNCH(4); break;
+    default: e = PG_LAUNCH(5); break;
   }
 #undef PG_LAUNCH
   PG_CUDA_OK(e);

@@ -15,11 +15,12 @@ import torch
 
 from . import _lib
 from .alphabet import ALPHABET
-from .checkpoint import EsmConfig, rotary_tables
-from .mutants import parse_mutants
-from .windows import optimal_window_starts
+from .checkpoint import EsmConfig, esmc_rotary_tables, rotary_tables
+from .mutants import parse_esmc_mutants, parse_mutants
+from .windows import esmc_window_rows, optimal_window_starts
 
 PRECISIONS = {"f16": _lib.PG_PREC_F16, "f16x3": _lib.PG_PREC_F16X3, "f16f8": _lib.PG_PREC_F16F8, "f16d": _lib.PG_PREC_F16D}
+ARCHS = {"esm1b": _lib.PG_ARCH_ESM1B, "esm2": _lib.PG_ARCH_ESM2, "esmc": _lib.PG_ARCH_ESMC}
 
 
 def choose_precision(config: EsmConfig, mutants=None, strategy: str = "masked-marginals", seq_len: int = None) -> str:
@@ -32,7 +33,10 @@ def choose_precision(config: EsmConfig, mutants=None, strategy: str = "masked-ma
     for the ESM-1b / ESM-1v masked-marginal pass over ONE shared window) measures 6.8e-5 mean / 3.9e-4 max on the same BLAT golden
     (286 residues). Its error scales with the size of the perturbation one mask causes, i.e. ~1/L: on a 96-residue protein it is
     7.6e-4 / 8.8e-4 / 1.5e-3 for 1 / 2 / 3 sites (f16f8: 3.4e-4 / 5.6e-4 / 6.0e-4; test_multi_site_error_growth_650m_vs_oracle), so
-    short proteins stay on f16f8. ESM2 8M / 35M / 150M stay within 6.1e-4 in f16f8 (tests/test_gpu_esm2_small.py).
+    short proteins stay on f16f8. ESM2 8M / 35M / 150M stay within 6.1e-4 in f16f8 (tests/test_gpu_esm2_small.py). ESM C (H100 80GB
+    HBM3, goldens of the unmodified evoscale script at true size, tests/test_gpu_esmc.py) in f16f8: max score error 1.2e-4 (300M, 1- and
+    2-site mutants), 1.4e-4 (600M), 9.9e-5 (300M, windowed L = 1150); f16x3 3.3e-5 / 4.9e-5 / 4.6e-5 — so ESM C follows the same rule
+    (f16d is refused for it).
     Rule: for models up to 1280 wide when no mutant has more than two sites — f16d if the architecture and the strategy allow it and
     192 <= ``seq_len`` (residues; + 2 tokens must fit the 1024-token window), else f16f8; f16x3 otherwise."""
     if config.embed_dim > 1280:
@@ -61,7 +65,7 @@ class EsmScorer:
         self.device = torch.device("cuda", device)
         self.precision = precision
         desc = _lib.PgModelDesc(
-            arch=_lib.PG_ARCH_ESM2 if config.arch == "esm2" else _lib.PG_ARCH_ESM1B, layers=config.layers,
+            arch=ARCHS[config.arch], layers=config.layers,
             embed_dim=config.embed_dim, heads=config.heads, ffn_dim=config.ffn_dim, vocab=config.vocab,
             max_positions=config.max_positions, token_dropout=int(config.token_dropout),
             emb_ln_before=int(config.emb_layer_norm_before), precision=PRECISIONS[precision], device=device,
@@ -81,6 +85,8 @@ class EsmScorer:
             inv = state["layers.0.self_attn.rot_emb.inv_freq"]
             cos, sin = rotary_tables(inv, 16384)  # rotary has no length limit in the reference; 16384 tokens covers every ProteinGym target (max 3423)
             tensors["rotary.cos"], tensors["rotary.sin"] = cos, sin
+        elif cfg.arch == "esmc":
+            tensors["rotary.cos"], tensors["rotary.sin"] = esmc_rotary_tables(1024)  # every ESM C window is <= 1024 tokens
         # fp32 staging copy on the device (ESM-1v 2.6 GB, ESM2-3B 11 GB); the library repacks and we free it
         gpu = [(n, t.to(self.device, torch.float32).contiguous()) for n, t in tensors.items()]
         arr = (_lib.PgTensor * len(gpu))()
@@ -134,10 +140,32 @@ class EsmScorer:
         if positions is None:
             positions = np.arange(1, len(sequence) + 1, dtype=np.int32)
         positions = np.asarray(positions, dtype=np.int32)
-        rows = self.masked_marginal_rows(tokens, positions, model_window)
+        if self.config.arch == "esmc" and len(sequence) > model_window - 2:  # compute_fitness.py:346-409: re-tokenised windows
+            if len(positions) and (positions.min() < 1 or positions.max() > len(sequence)):
+                raise IndexError("ESM C windows hold residue positions 1..L only")
+            rows = self.esmc_rows(sequence, positions - 1, model_window)
+        else:
+            rows = self.masked_marginal_rows(tokens, positions, model_window)
         table = torch.full((len(tok_np), self.config.vocab), float("nan"), dtype=torch.float32, device=self.device)
         table[torch.from_numpy(positions.astype(np.int64)).to(self.device)] = rows
         return table
+
+    def esmc_rows(self, sequence: str, seq_positions, window_size: int = 1024) -> torch.Tensor:
+        """ESM C: log_softmax rows [P, 64] with residue ``seq_positions[p]`` (0-based) masked in its window (one token row per distinct
+        ``<cls> slice <eos>`` window, windows.esmc_window_rows)."""
+        res = ALPHABET.tokenize_sequence(sequence)[1:-1]
+        tok, pos, starts, T = esmc_window_rows(res, seq_positions, ALPHABET.cls_idx, ALPHABET.eos_idx, window_size)
+        P = len(pos)
+        out = torch.empty((P, self.config.vocab), dtype=torch.float32, device=self.device)
+        if P == 0:
+            return out
+        stage = torch.from_numpy(np.concatenate([tok, pos, starts])).to(self.device)
+        n = len(tok)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.pg_masked_marginals(self.handle, stage.data_ptr(), n, stage[n:].data_ptr(), stage[n + P:].data_ptr(), None,
+                                                P, T, out.data_ptr(), stream), self.handle)
+        self._keepalive = stage
+        return out
 
     def wt_marginal_table(self, sequence: str) -> torch.Tensor:
         """One unmasked forward, log_softmax of every token (compute_fitness.py:475)."""
@@ -205,7 +233,10 @@ class EsmScorer:
     # ------------------------------------------------------------------------------------------------------------
     def prepare_assay(self, sequence: str, mutants, offset_idx: int = 1, model_window: int = 1024, pinned: bool = True):
         """Host half of one assay: tokenise, parse mutants, find which token rows ``label_row`` will read and their
-        windows. Returns pinned host arrays + sizes; nothing touches the device."""
+        windows. Returns pinned host arrays + sizes; nothing touches the device. ESM C follows its own script's rules instead
+        (evoscale compute_fitness.py:69-136, 346-409): no offset, invalid mutants skipped (NaN), re-tokenised windows."""
+        if self.config.arch == "esmc":
+            return self._prepare_assay_esmc(sequence, mutants, model_window, pinned)
         tok = ALPHABET.tokenize_sequence(sequence)
         site_row, site_wt, site_mt, offs = parse_mutants(mutants, sequence, offset_idx)
         if len(site_row) and (site_row.min() < 1 or site_row.max() > len(sequence)):
@@ -221,6 +252,21 @@ class EsmScorer:
             host = host.pin_memory()
         sizes = dict(n_tokens=len(tok), P=len(positions), T=T, S=len(site_row), M=len(offs) - 1,
                      windowed=len(tok) > model_window)
+        return host, sizes
+
+    def _prepare_assay_esmc(self, sequence: str, mutants, window_size: int, pinned: bool):
+        site_pos, site_wt, site_mt, offs, valid = parse_esmc_mutants(mutants, sequence)
+        seq_pos = np.unique(site_pos).astype(np.int32)
+        res = ALPHABET.tokenize_sequence(sequence)[1:-1]
+        tok, positions, starts, T = esmc_window_rows(res, seq_pos, ALPHABET.cls_idx, ALPHABET.eos_idx, window_size)
+        row_of = np.full(len(sequence) + 1, -1, dtype=np.int32)
+        row_of[seq_pos] = np.arange(len(seq_pos), dtype=np.int32)
+        packed = np.concatenate([tok, positions, starts, row_of[site_pos], site_wt, site_mt, offs]).astype(np.int32)
+        host = torch.from_numpy(packed)
+        if pinned:
+            host = host.pin_memory()
+        sizes = dict(n_tokens=len(tok), P=len(seq_pos), T=T, S=len(site_pos), M=len(offs) - 1, windowed=True,
+                     invalid=np.flatnonzero(~valid))
         return host, sizes
 
     def run_assay(self, host: torch.Tensor, sizes: dict, dev: torch.Tensor | None = None, shard=None) -> torch.Tensor:
@@ -250,6 +296,9 @@ class EsmScorer:
         if M:
             _lib.check(self.lib.pg_score_mutants(table.data_ptr(), P, self.config.vocab, trow.data_ptr(), wt.data_ptr(),
                                                  mt.data_ptr(), offs.data_ptr(), M, scores.data_ptr(), stream))
+        invalid = sizes.get("invalid")
+        if invalid is not None and len(invalid):  # mutants the reference skips get NaN (evoscale compute_fitness.py:592)
+            scores[torch.from_numpy(invalid).to(self.device)] = float("nan")
         self._keepalive3 = (dev, table)
         return scores
 

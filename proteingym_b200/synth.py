@@ -461,3 +461,62 @@ def random_alignment(target_seq: str, n_rows: int, seed: int, sub_rate=(0.05, 0.
                 s[j] = AA20[rng.randint(0, 20)]
         rows.append((">seq%d/1-%d" % (i, len(target_seq)), "".join(s)))
     return rows
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# ESM C (reference: proteingym/baselines/evoscale/esm/models/esmc.py, esm/pretrained.py:65-98)
+@dataclass
+class EsmcArch:
+    layers: int
+    embed_dim: int
+    ffn_dim: int  # SwiGLU hidden width f (fc1 is [2f, d])
+
+    @property
+    def heads(self) -> int:
+        return self.embed_dim // 64
+
+
+ESMC_300M = EsmcArch(30, 960, 2560)
+ESMC_600M = EsmcArch(36, 1152, 3072)
+
+
+def make_esmc_state(arch: EsmcArch, seed: int = 0) -> dict:
+    """ESM C state dict with the reference key names, drawn on the CPU from ``seed`` (deterministic: tests regenerate it).
+
+    Linear weights follow nn.Linear's U(+-1/sqrt(fan_in)); every LayerNorm weight is 1 + 0.1 N(0,1) and every LayerNorm bias 0.1 N(0,1)
+    (q_ln / k_ln included) so that a dropped affine term shows up; all 64 output rows are random, so the 64-way normaliser matters.
+    The embedding is N(0,1) like nn.Embedding (every block starts with a LayerNorm), the output matrix is scaled by 3 so log-prob
+    differences are in the single digits."""
+    g = torch.Generator().manual_seed(seed)
+    d, f = arch.embed_dim, arch.ffn_dim
+    ln_w = lambda: 1 + 0.1 * torch.randn(d, generator=g)
+    ln_b = lambda: 0.1 * torch.randn(d, generator=g)
+    st = {"embed.weight": torch.randn((64, d), generator=g)}
+    for i in range(arch.layers):
+        p = f"transformer.blocks.{i}."
+        st[p + "attn.layernorm_qkv.0.weight"] = ln_w()
+        st[p + "attn.layernorm_qkv.0.bias"] = ln_b()
+        st[p + "attn.layernorm_qkv.1.weight"] = _uniform(g, (3 * d, d), 1 / math.sqrt(d))
+        st[p + "attn.q_ln.weight"] = ln_w()
+        st[p + "attn.k_ln.weight"] = ln_w()
+        st[p + "attn.out_proj.weight"] = _uniform(g, (d, d), 1 / math.sqrt(d))
+        st[p + "ffn.0.weight"] = ln_w()
+        st[p + "ffn.0.bias"] = ln_b()
+        st[p + "ffn.1.weight"] = _uniform(g, (2 * f, d), 1 / math.sqrt(d))
+        st[p + "ffn.3.weight"] = _uniform(g, (d, f), 1 / math.sqrt(f))
+    st["transformer.norm.weight"] = ln_w()
+    st["sequence_head.0.weight"] = _uniform(g, (d, d), 1 / math.sqrt(d))
+    st["sequence_head.0.bias"] = _uniform(g, (d,), 1 / math.sqrt(d))
+    st["sequence_head.2.weight"] = ln_w()
+    st["sequence_head.2.bias"] = ln_b()
+    st["sequence_head.3.weight"] = 3 * _uniform(g, (64, d), 1 / math.sqrt(d))
+    st["sequence_head.3.bias"] = 0.1 * torch.randn(64, generator=g)
+    return st
+
+
+def write_esmc_checkpoint(path: str, arch: EsmcArch, seed: int = 0, state: dict | None = None) -> dict:
+    """Write the state dict as the .pth file the reference's loader reads (``torch.load`` + ``load_state_dict``, pretrained.py:65-98)."""
+    st = state if state is not None else make_esmc_state(arch, seed)
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    torch.save(st, path)
+    return st

@@ -30,13 +30,22 @@ enum pg_arch {
   PG_ARCH_MSA = 3,         /* MSA Transformer: tied row attention + column attention + FFN per layer, learned column positions and
                               (when the state holds "msa_position_embedding") row positions (esm/model/msa_transformer.py:100-222,
                               esm/axial_attention.py) */
-  PG_ARCH_ESMC = 4         /* ESM C (evoscale esm/models/esmc.py:117-173): pre-LN blocks without linear biases, q/k LayerNorm over the
+  PG_ARCH_ESMC = 4,        /* ESM C (evoscale esm/models/esmc.py:117-173): pre-LN blocks without linear biases, q/k LayerNorm over the
                               full width + rotary, SwiGLU MLP (ffn_dim = the SwiGLU hidden width f; fc1 is [2f, d]), residual branches
                               divided by sqrt(layers / 36), untied 64-way output head; vocab 64, heads = embed_dim / 64, token_dropout
                               = emb_ln_before = 0, max_positions unused. Weights: the reference state-dict keys verbatim plus
                               "rotary.cos" / "rotary.sin" [T, 32]. Windows (compute_fitness.py:346-409 re-tokenises each one as
                               <cls> slice <eos>) are the caller's: pass one token row per distinct window, concatenated, with
                               win_start[p] = that row's offset and positions[p] = offset + index within the row. */
+  PG_ARCH_RITA = 5         /* RITA S / M / L causal decoder (proteingym/baselines/rita/rita_modeling.py:129-252): pre-LN blocks, separate
+                              q/k/v Linear with bias, rotate-half rotary over 64-wide heads, no attention bias, tanh-GELU MLP (ffn_dim =
+                              ff_ratio * d), final LayerNorm, head without bias; heads = embed_dim / 64 (RITA XL's 128-wide heads are
+                              refused), max_positions = rows of the rotary tables = the longest token row a call may pass. Scored through
+                              the pg_ar_* entry points without retrieval fusion. Weights: the HF state-dict keys without "transformer."
+                              ("layers.{i}.self_attention.{query,key,value,proj}.{weight,bias}", "layers.{i}.{attn_norm,mlp_norm}.*",
+                              "layers.{i}.mlp.{0,2}.*", "embedding.weight", "final_norm.*"), "lm_head.weight" [vocab, d] only for an
+                              untied head (absent = the embedding), plus "rotary.cos" / "rotary.sin" [T, 32] = cos / sin(t * inv_freq[c])
+                              from the checkpoint's rotary_embedding.inv_freq. */
 };
 
 /* Tensor-core operand precision. The reference is strict fp32 (SURVEY.md §0.4). Every operand is an fp16 pair hi + lo.
@@ -122,6 +131,8 @@ int pg_forward_logprobs(pg_handle h, const int32_t* tokens, int32_t n_tokens, in
  *   out_sum_logp [B] fp32: sum_{t < len-1} log p(ids[b, t+1] | ids[b, <= t])
  * Weights for a PG_ARCH_TRANCEPTION handle use the HF names without the "transformer." prefix (Conv1D weights [in, out]),
  * plus "h.{i}.attn.conv_taps" [768, 8] (look-back taps + bias per q/k/v, head group, channel) and "alibi_slopes" [heads, 1]. */
+/* A PG_ARCH_RITA handle runs the same entry points on its own token ids (any vocabulary, no [CLS] / [SEP] assumed): out_sum_logp[b] =
+ * sum_{t < lens[b]-1} log p(ids[b, t+1] | ids[b, <= t]); a retrieval prior is refused with PG_ERR_ARG (f->out_logprobs is allowed). */
 int pg_ar_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, const float* log_prior,
                  const int32_t* prior_row, float alpha, float* out_sum_logp, pg_stream stream);
 

@@ -230,3 +230,83 @@ def esmc_rotary_tables(T: int = 1024):
     inv_freq = 1.0 / (10000 ** (torch.arange(0, 64, 2, dtype=torch.float32) / 64))
     freqs = torch.outer(torch.arange(T, dtype=torch.float32), inv_freq)
     return freqs.cos().contiguous(), freqs.sin().contiguous()
+
+
+# ---- RITA (proteingym/baselines/rita: rita_configuration.py, rita_modeling.py) ----------------------------------------------------
+@dataclass
+class RitaConfig:
+    layers: int
+    embed_dim: int
+    heads: int
+    ffn_dim: int
+    vocab: int
+    tied: bool               # the output head is the embedding matrix
+
+
+def load_rita_checkpoint(folder: str):
+    """RITA model directory -> (RitaConfig, state, inv_freq). ``state`` has the key names of include/pgscore.h's PG_ARCH_RITA (the
+    ``transformer.`` prefix stripped, no rotary buffers) as fp32 CPU tensors; ``inv_freq`` is the checkpoint's rotary buffer.
+
+    config.json: ``d_model``, ``num_layers``, ``num_heads``, ``ff_ratio`` (the FFN width is d_model * ff_ratio, rita_configuration.py:
+    25-26), ``vocab_size`` and ``tie_word_embeddings``, with RITAConfig's defaults for absent keys. Weights: pytorch_model.bin or
+    *.safetensors.
+
+    Head tying follows the rule of PretrainedConfig in the transformers release the reference pins (4.32.1): ``tie_word_embeddings``
+    defaults to true, and ``from_pretrained`` then ties ``lm_head.weight`` to the embedding. That release could not be inspected here
+    (DESIGN.md §2 records this assumption and what would change it); an ``lm_head.weight`` that tying discards and that differs from
+    the embedding is reported with a warning. With ``"tie_word_embeddings": false`` the checkpoint's ``lm_head.weight`` is the head."""
+    import json
+    import warnings
+    cfg = json.load(open(os.path.join(folder, "config.json")))
+    pbin = os.path.join(folder, "pytorch_model.bin")
+    if os.path.exists(pbin):
+        raw = torch.load(pbin, map_location="cpu", weights_only=True)
+    else:
+        st_files = sorted(Path(folder).glob("*.safetensors"))
+        if not st_files:
+            raise FileNotFoundError(f"{folder}: neither pytorch_model.bin nor *.safetensors")
+        from safetensors.torch import load_file
+        raw = {}
+        for f in st_files:
+            raw.update(load_file(str(f)))
+    d, layers, heads = int(cfg.get("d_model", 768)), int(cfg.get("num_layers", 12)), int(cfg.get("num_heads", 12))
+    ffn, vocab = d * int(cfg.get("ff_ratio", 4)), int(cfg.get("vocab_size", 26))
+    tied = bool(cfg.get("tie_word_embeddings", True))
+    state, inv = {}, []
+    for k, v in raw.items():
+        name = k[len("transformer."):] if k.startswith("transformer.") else k
+        if name.endswith("rotary_embedding.inv_freq"):
+            inv.append((name, v.float()))
+            continue
+        state[name] = v.detach().float().contiguous()
+    if len(inv) != layers:
+        raise ValueError(f"{folder}: {len(inv)} rotary_embedding.inv_freq buffers for {layers} layers")
+    inv_freq = inv[0][1]
+    for name, t in inv[1:]:
+        if t.shape != inv_freq.shape or not torch.equal(t, inv_freq):
+            raise ValueError(f"{folder}: {name} differs from {inv[0][0]}: the layers disagree on the rotary frequencies")
+    if tied:
+        head = state.pop("lm_head.weight", None)
+        if head is not None and not torch.equal(head, state.get("embedding.weight", head)):
+            warnings.warn(f"{folder}: lm_head.weight differs from the embedding and is discarded: config.json does not set "
+                          "tie_word_embeddings to false, so the head is tied to the embedding")
+    elif "lm_head.weight" not in state:
+        raise ValueError(f"{folder}: tie_word_embeddings is false but the checkpoint has no lm_head.weight")
+    want = {"embedding.weight": (vocab, d), "final_norm.weight": (d,), "final_norm.bias": (d,)}
+    if not tied:
+        want["lm_head.weight"] = (vocab, d)
+    for i in range(layers):
+        p = f"layers.{i}."
+        for nm in ("query", "key", "value", "proj"):
+            want[p + f"self_attention.{nm}.weight"] = (d, d)
+            want[p + f"self_attention.{nm}.bias"] = (d,)
+        want.update({p + "attn_norm.weight": (d,), p + "attn_norm.bias": (d,), p + "mlp_norm.weight": (d,), p + "mlp_norm.bias": (d,),
+                     p + "mlp.0.weight": (ffn, d), p + "mlp.0.bias": (ffn,), p + "mlp.2.weight": (d, ffn), p + "mlp.2.bias": (d,)})
+    for k, shape in want.items():
+        if k not in state:
+            raise ValueError(f"RITA state dict: missing {k}")
+        if tuple(state[k].shape) != shape:
+            raise ValueError(f"RITA state dict: {k} has shape {tuple(state[k].shape)}, expected {shape}")
+    if d % heads or inv_freq.numel() != (d // heads) // 2:
+        raise ValueError(f"RITA: d_model {d} / num_heads {heads} does not match inv_freq of {inv_freq.numel()} frequencies")
+    return RitaConfig(layers, d, heads, ffn, vocab, tied), state, inv_freq

@@ -352,16 +352,19 @@ GemmLaunch proj_gemm(pg_handle h, const Layer& L, Proj p, const __half* a, float
   return g;
 }
 // ... written as operand rows to `out` through epilogue `epi`: q/k/v in the q/k/v format (epi 0, or 3: rotary embedding over windows of
-// rot_T rows), fc1 in the GEMM-input format (epi: the MLP's activation, out_scale: the e4m3 scale of its output; SwiGLU, epi 5, writes
-// half as many columns as the GEMM has).
+// rot_T rows, row t of a window at position rot_start + t), fc1 in the GEMM-input format (epi: the MLP's activation, out_scale: the e4m3
+// scale of its output; SwiGLU, epi 5, writes half as many columns as the GEMM has).
 int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int M, __half* out, cudaStream_t s, int epi = 0,
-        float out_scale = 0.f, int rot_T = 0) {
+        float out_scale = 0.f, int rot_T = 0, int rot_start = 0) {
   GemmLaunch g = proj_gemm(h, L, p, a, a_scale, M);
   const int n_out = epi == 5 ? g.N / 2 : g.N;
   g.epi = epi;
   g.out = out; g.ldo = static_cast<int64_t>(n_out) * h->op.np; g.out_fmt = p == QKV ? h->op.qfmt : h->op.afmt;
   g.out_lo_off = g.out_fmt ? n_out : 0; g.out_scale = out_scale;
-  if (epi == 3) { g.rot_cos = h->rot_cos; g.rot_sin = h->rot_sin; g.rot_T = rot_T; g.rot_dim = h->op.da; }  // q and k slots
+  if (epi == 3) {  // q and k slots
+    g.rot_cos = h->rot_cos + static_cast<int64_t>(rot_start) * 32; g.rot_sin = h->rot_sin + static_cast<int64_t>(rot_start) * 32;
+    g.rot_T = rot_T; g.rot_dim = h->op.da;
+  }
   ProfScope ps(p, s);
   return launch_gemm(g, s);
 }
@@ -374,8 +377,8 @@ int lin_add(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale,
 }
 
 // MLP block on M fp32 residual rows x: x += fc2(act(fc1(LN2(x)))), through operand rows `ab` (LayerNorm output) and `fb` (hidden
-// layer). act: fc1's activation epilogue (1 GELU, 4 relu^2, 5 SwiGLU); act_scale: the e4m3 scale of its output (S_GELU, S_RELU2,
-// S_SWIGLU).
+// layer). act: fc1's activation epilogue (1 GELU, 4 relu^2, 5 SwiGLU, 6 tanh-GELU); act_scale: the e4m3 scale of its output (S_GELU,
+// S_RELU2, S_SWIGLU).
 int mlp(pg_handle h, const Layer& L, float* x, int M, __half* ab, __half* fb, int act, float act_scale, cudaStream_t s) {
   int rc = ln(h, x, L.ln2g, L.ln2b, M, ab, s);
   if (!rc) rc = lin(h, L, FC1, ab, S_LN, M, fb, s, act, act_scale);
@@ -592,13 +595,19 @@ int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const i
   return PG_OK;
 }
 
-// Tranception decoder stack over B right-padded sequences of T tokens (model_pytorch.py:526-612): no padding mask is needed
-// because pads sit to the right of every real token and attention is causal.
-// mode 0: plain forward. mode 1 (B == 1): also record every layer's raw and conv'd q/k/v rows into the prefix caches.
+// Causal decoder stack over B right-padded sequences of T tokens: no padding mask is needed because pads sit to the right of every real
+// token and attention is causal.
+//   Tranception (model_pytorch.py:526-612): grouped ALiBi, depthwise-conv q/k/v, relu^2 MLP.
+//   RITA (rita_modeling.py:129-210, 244-252): rotary q/k (GEMM epilogue 3, q pre-scaled by 1/8 at load), no attention bias, tanh-GELU
+//   MLP (epilogue 6).
+// mode 0: plain forward. mode 1 (B == 1): also record every layer's keys / values (Tranception: the raw q/k/v rows for the conv
+// look-back and the conv'd rows; RITA: the rotated rows) into the prefix caches.
 // mode 2: the B sequences are rows [start, start + T) of sequences whose first `start` rows (multiple of 128) equal the recorded
-// wild type's: depthwise-conv look-back and the keys / values of the prefix come from the caches.
-int forward_tranception(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, int mode = 0, int start = 0) {
+// wild type's: the keys / values of the prefix (and Tranception's conv look-back) come from the caches, and RITA's rotary runs at the
+// absolute positions start + t.
+int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, int mode = 0, int start = 0) {
   const pg_model_desc& D = h->desc;
+  const bool rita = D.arch == PG_ARCH_RITA;
   const int64_t ldq = h->op.ldq;
   const int rows = B * T;
   int rc;
@@ -607,23 +616,27 @@ int forward_tranception(pg_handle h, const int32_t* ids, int B, int T, cudaStrea
   for (int l = 0; l < D.layers; ++l) {
     const Layer& L = h->layers[l];
     if ((rc = ln(h, h->x, L.ln1g, L.ln1b, rows, h->abuf, s))) return rc;
-    if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s, rita ? 3 : 0, 0.f, T, mode == 2 ? start : 0))) return rc;
     const size_t layer_off = static_cast<size_t>(l) * h->prefix_cap * ldq;
+    const __half* kv = h->qkv;  // the q/k/v rows attention reads
+    if (!rita) {
+      if (mode == 1)
+        PG_CUDA_OK(cudaMemcpyAsync(h->raw_cache + layer_off, h->qkv, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+      { ProfScope ps(CAT_OTHER, s);
+        rc = launch_qkv_conv(h->qkv, h->qkv2, ldq, h->op.lo_q, B, T, D.heads, L.conv_taps, 0.125f, s,
+                             mode == 2 ? h->raw_cache + layer_off + static_cast<size_t>(start - 6) * ldq : nullptr); }
+      if (rc) return rc;
+      kv = h->qkv2;
+    }
     if (mode == 1)
-      PG_CUDA_OK(cudaMemcpyAsync(h->raw_cache + layer_off, h->qkv, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
-    { ProfScope ps(CAT_OTHER, s);
-      rc = launch_qkv_conv(h->qkv, h->qkv2, ldq, h->op.lo_q, B, T, D.heads, L.conv_taps, 0.125f, s,
-                           mode == 2 ? h->raw_cache + layer_off + static_cast<size_t>(start - 6) * ldq : nullptr); }
-    if (rc) return rc;
-    if (mode == 1)
-      PG_CUDA_OK(cudaMemcpyAsync(h->kv_cache + layer_off, h->qkv2, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
-    AttnLaunch a = attn_args(h, h->qkv2, h->abuf, B, T);
-    a.causal = 1; a.alibi_slopes = h->slopes;
+      PG_CUDA_OK(cudaMemcpyAsync(h->kv_cache + layer_off, kv, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    AttnLaunch a = attn_args(h, kv, h->abuf, B, T);
+    a.causal = 1; a.alibi_slopes = rita ? nullptr : h->slopes;
     if (mode == 2) { a.prefix = h->kv_cache + layer_off; a.prefix_len = start; }
     { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
     if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
-    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, 4, S_RELU2, s))) return rc;
+    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, rita ? 6 : 4, rita ? S_GELU : S_RELU2, s))) return rc;
   }
   return PG_OK;
 }
@@ -768,23 +781,23 @@ int compact_head(pg_handle h, int T, int Bc, float* out, int launches, cudaStrea
   return launch_head(hl, s);
 }
 
-// The Tranception passes over B sequences of T rows (forward_tranception mode 0, or mode 2 after the recorded prefix at `start`), as
-// many sequences per pass as the workspace holds, each followed by the head on its rows.
+// The decoder passes over B sequences of T rows (forward_ar mode 0, or mode 2 after the recorded prefix at `start`), as many sequences
+// per pass as the workspace holds, each followed by the head on its rows (the tied embedding, or RITA's untied lm_head).
 int ar_passes(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, int mode, int start, const ArFusion& fusion,
               float* out_sum_logp, cudaStream_t s) {
   const long long per = balanced_per(B, h->max_rows / T);
   for (int b0 = 0; b0 < B; b0 += static_cast<int>(per)) {
     const int Bc = (B - b0) < per ? (B - b0) : static_cast<int>(per);
     const long long off = static_cast<long long>(b0) * T;
-    int rc = forward_tranception(h, ids + off, Bc, T, s, mode, start);
+    int rc = forward_ar(h, ids + off, Bc, T, s, mode, start);
     if (rc) return fail(h, rc, tls_error());
     ProfScope ps(CAT_HEAD, s, 2);
     ArFusion fc = fusion;
     if (fc.prior_row) fc.prior_row += off;
     if (fc.prior_row2) fc.prior_row2 += off;
     if (fc.out_logprobs) fc.out_logprobs += off * h->desc.vocab;
-    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->lnag, h->lnab, h->embed, fc, h->tok_logp,
-                        out_sum_logp + b0, s);
+    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->lnag, h->lnab, h->outw ? h->outw : h->embed,
+                        fc, h->tok_logp, out_sum_logp + b0, s);
     if (rc) return fail(h, rc, tls_error());
   }
   return PG_OK;
@@ -845,10 +858,13 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
       return set_error(PG_ERR_UNSUPPORTED, "pg_create: ESM2 head_dim must be even and at most 64");
     if (D.embed_dim % 4 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ESM2 needs embed_dim % 4 == 0 and ffn_dim % 64 == 0");
   } else {
+    if (D.arch == PG_ARCH_RITA && D.embed_dim != D.heads * 64)  // RITA XL (2048 / 16) has 128-wide heads
+      return set_error(PG_ERR_UNSUPPORTED, "pg_create: RITA needs head_dim 64 (RITA S / M / L); 128-wide heads (RITA XL) have no attention tile");
     if (D.embed_dim != D.heads * 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: head_dim must be 64");
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
   }
-  if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC)
+  if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC &&
+      D.arch != PG_ARCH_RITA)
     return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
   if (D.arch == PG_ARCH_ESMC && D.heads > 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: the ESM C q/k LayerNorm kernel holds at most 24 heads");
   if (D.arch == PG_ARCH_TRANCEPTION && D.heads % 4) return set_error(PG_ERR_UNSUPPORTED, "pg_create: Tranception needs heads % 4 == 0 (model_pytorch.py:129-131)");
@@ -885,7 +901,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     if (D.arch == PG_ARCH_TRANCEPTION) A(&L.conv_taps, 3 * 4 * 64 * 8);
     if (esmc) { A(&L.qlng, d); A(&L.klng, d); }
   }
-  if (esmc) A(&h->outw, static_cast<size_t>(D.vocab) * d);
+  if (esmc || D.arch == PG_ARCH_RITA) A(&h->outw, static_cast<size_t>(D.vocab) * d);
   if (D.arch == PG_ARCH_MSA) {
     h->col_layers.resize(D.layers);
     for (auto& L : h->col_layers) {
@@ -897,9 +913,9 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   }
   if (D.arch == PG_ARCH_TRANCEPTION) {
     A(&h->qkv2, static_cast<size_t>(h->max_rows) * 3 * d * np);
-    A(&h->tok_logp, static_cast<size_t>(h->max_rows));
     A(&h->slopes, D.heads);
   }
+  if (D.arch == PG_ARCH_TRANCEPTION || D.arch == PG_ARCH_RITA) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
   if (h->op.nseg == 2) A(&h->pack_scratch, static_cast<size_t>(D.layers) * 6);
   A(&h->embed, static_cast<size_t>(D.vocab) * d);
   if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA) A(&h->pos, static_cast<size_t>(D.max_positions + 2) * d);
@@ -967,6 +983,23 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     unsigned int* f8_scratch = h->op.nseg == 2 ? h->pack_scratch + (h->pack_used++ % (D.layers * 6)) : nullptr;
     pack_weights(group, N, K, conv1d ? 1 : K, conv1d ? N : 1, np, f8_scratch, dst, inv, 0);
   };
+  // "rotary.cos" / "rotary.sin" [T, 32] (ESM C, RITA: heads of 64) -> the device tables of the rotary GEMM epilogue
+  auto rotary32 = [&]() -> int {
+    auto it = by_name.find("rotary.cos");
+    auto is = by_name.find("rotary.sin");
+    if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != 32 || is->second->shape[1] != 32 ||
+        is->second->shape[0] != it->second->shape[0]) {
+      missing += "rotary.cos/rotary.sin[T,32] ";
+      return PG_OK;
+    }
+    h->rot_rows = static_cast<int>(it->second->shape[0]);
+    int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
+    if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
+    if (rc) return rc;
+    copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * 32);
+    copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * 32);
+    return PG_OK;
+  };
   if (D.arch == PG_ARCH_TRANCEPTION) {
     // HF GPT2-style names with the "transformer." prefix stripped by the host
     for (int l = 0; l < D.layers; ++l) {
@@ -1029,19 +1062,37 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     copy(h->hlnb, get("sequence_head.2.bias", d, 1), d);
     copy(h->outw, get("sequence_head.3.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
     copy(h->hbias, get("sequence_head.3.bias", D.vocab, 1), D.vocab);
-    auto it = by_name.find("rotary.cos");
-    auto is = by_name.find("rotary.sin");
-    if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != 32 || is->second->shape[1] != 32 ||
-        is->second->shape[0] != it->second->shape[0]) {
-      missing += "rotary.cos/rotary.sin[T,32] ";
-    } else {
-      h->rot_rows = static_cast<int>(it->second->shape[0]);
-      int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
-      if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
-      if (rc) return rc;
-      copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * 32);
-      copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * 32);
+    if (int rc = rotary32()) return rc;
+  } else if (D.arch == PG_ARCH_RITA) {
+    // HF names without the "transformer." prefix (rita_modeling.py:113-121, 185-194, 222-224). q, k and v form one GEMM operand with
+    // 1/sqrt(64) = 0.125 folded into the q rows and bias: exact (a power of two), and it commutes with the (linear) rotary.
+    for (int l = 0; l < D.layers; ++l) {
+      Layer& L = h->layers[l];
+      const std::string p = "layers." + std::to_string(l) + ".";
+      const std::string a = p + "self_attention.";
+      pack(L.wqkv, L.iqkv, {{get(a + "query.weight", d, d), 0.125f}, get(a + "key.weight", d, d), get(a + "value.weight", d, d)}, d, d);
+      copy(L.bqkv, get(a + "query.bias", d, 1), d, 0.125f);
+      copy(L.bqkv + d, get(a + "key.bias", d, 1), d);
+      copy(L.bqkv + 2 * d, get(a + "value.bias", d, 1), d);
+      pack(L.wo, L.io, {get(a + "proj.weight", d, d)}, d, d);
+      copy(L.bo, get(a + "proj.bias", d, 1), d);
+      copy(L.ln1g, get(p + "attn_norm.weight", d, 1), d);
+      copy(L.ln1b, get(p + "attn_norm.bias", d, 1), d);
+      pack(L.w1, L.i1, {get(p + "mlp.0.weight", f, d)}, f, d);
+      copy(L.b1, get(p + "mlp.0.bias", f, 1), f);
+      pack(L.w2, L.i2, {get(p + "mlp.2.weight", d, f)}, d, f);
+      copy(L.b2, get(p + "mlp.2.bias", d, 1), d);
+      copy(L.ln2g, get(p + "mlp_norm.weight", d, 1), d);
+      copy(L.ln2b, get(p + "mlp_norm.bias", d, 1), d);
     }
+    copy(h->embed, get("embedding.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    copy(h->lnag, get("final_norm.weight", d, 1), d);
+    copy(h->lnab, get("final_norm.bias", d, 1), d);
+    // the output head: "lm_head.weight" when the caller passes it (an untied checkpoint), else the embedding matrix
+    if (by_name.count("lm_head.weight")) copy(h->outw, get("lm_head.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    else copy(h->outw, get("embedding.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    if (int rc = rotary32()) return rc;
+    if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
   } else {
     const int hd = d / D.heads, dk = h->op.dk, da = h->op.da;
     // head_dim^-1/2 (multihead_attention.py:103,261), folded into the fp32 q weights and bias: 0.125 (exact) for head_dim 64
@@ -1149,7 +1200,8 @@ int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, co
                         const int32_t* out_row, int32_t P, int32_t T, float* out_logprobs, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_masked_marginals: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_masked_marginals: weights not loaded");
-  if (h->desc.arch == PG_ARCH_TRANCEPTION) return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is a Tranception model (use pg_ar_loglik)");
+  if (h->desc.arch == PG_ARCH_TRANCEPTION || h->desc.arch == PG_ARCH_RITA)
+    return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is an autoregressive model (use pg_ar_loglik)");
   if (h->desc.arch == PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is an MSA Transformer (use pg_msa_masked_marginals)");
   if (!tokens || !positions || !out_logprobs) return fail(h, PG_ERR_ARG, "pg_masked_marginals: null buffer");
   if (P < 0 || T <= 0 || T > n_tokens) return fail(h, PG_ERR_ARG, "pg_masked_marginals: bad P/T");
@@ -1213,7 +1265,8 @@ int pg_forward_logprobs(pg_handle h, const int32_t* tokens, int32_t n_tokens, in
                         float* out_logprobs, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_forward_logprobs: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: weights not loaded");
-  if (h->desc.arch == PG_ARCH_TRANCEPTION) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is a Tranception model (use pg_ar_loglik)");
+  if (h->desc.arch == PG_ARCH_TRANCEPTION || h->desc.arch == PG_ARCH_RITA)
+    return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an autoregressive model (use pg_ar_loglik)");
   if (h->desc.arch == PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an MSA Transformer (use pg_msa_masked_marginals)");
   if (!tokens || !out_logprobs || T <= 0 || win_start < 0 || win_start + T > n_tokens) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: bad arguments");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than the learned position table");
@@ -1244,6 +1297,8 @@ static int ar_fusion_args(pg_handle h, const pg_ar_fusion* f, ArFusion* base) {
   if ((f->log_prior2 == nullptr) != (f->prior_row2 == nullptr)) return fail(h, PG_ERR_ARG, "pg_ar_loglik: log_prior2 and prior_row2 go together");
   if (f->log_prior2 && !f->log_prior) return fail(h, PG_ERR_ARG, "pg_ar_loglik: the second prior needs the first (it is fused inside the MSA overlap)");
   if (f->first_col < 0 || f->first_col > h->desc.vocab) return fail(h, PG_ERR_ARG, "pg_ar_loglik: first_col outside the vocabulary");
+  if (h->desc.arch == PG_ARCH_RITA && (f->log_prior || f->log_prior2))
+    return fail(h, PG_ERR_ARG, "pg_ar_loglik: RITA has no retrieval fusion (pass no log_prior / log_prior2)");
   base->log_prior = f->log_prior; base->prior_row = f->prior_row; base->alpha = f->alpha;
   base->log_prior2 = f->log_prior2; base->prior_row2 = f->prior_row2; base->beta = f->beta;
   base->first_col = f->first_col; base->out_logprobs = f->out_logprobs;
@@ -1254,7 +1309,8 @@ int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int
                        float* out_sum_logp, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_ar_loglik: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_loglik: weights not loaded");
-  if (h->desc.arch != PG_ARCH_TRANCEPTION) return fail(h, PG_ERR_STATE, "pg_ar_loglik: handle is not a Tranception model");
+  if (h->desc.arch != PG_ARCH_TRANCEPTION && h->desc.arch != PG_ARCH_RITA)
+    return fail(h, PG_ERR_STATE, "pg_ar_loglik: handle is not an autoregressive model (Tranception, RITA)");
   if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_ar_loglik: bad B/T");
   if (B == 0) return PG_OK;
   if (!ids || !lens || !out_sum_logp) return fail(h, PG_ERR_ARG, "pg_ar_loglik: null buffer");
@@ -1269,7 +1325,8 @@ int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int
 int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_fusion* f, float* out_tok_logp, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_ar_prefix_begin: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: weights not loaded");
-  if (h->desc.arch != PG_ARCH_TRANCEPTION) return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: handle is not a Tranception model");
+  if (h->desc.arch != PG_ARCH_TRANCEPTION && h->desc.arch != PG_ARCH_RITA)
+    return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: handle is not an autoregressive model (Tranception, RITA)");
   if (!ids || !out_tok_logp || T < 2) return fail(h, PG_ERR_ARG, "pg_ar_prefix_begin: bad arguments");
   if (T > h->desc.max_positions || T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_ar_prefix_begin: sequence longer than n_ctx / workspace");
   ArFusion fu;
@@ -1278,21 +1335,22 @@ int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_f
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t ldq = static_cast<size_t>(h->op.ldq);
-  if (h->prefix_cap < h->desc.max_positions) {  // first use: [layers][n_ctx][3d*np] fp16, twice
+  if (h->prefix_cap < h->desc.max_positions) {  // first use: [layers][n_ctx][3d*np] fp16, twice (RITA: once, no conv look-back)
     const size_t n = static_cast<size_t>(h->desc.layers) * h->desc.max_positions * ldq;
-    rc = dev_alloc(h, &h->raw_cache, n);
+    rc = h->desc.arch == PG_ARCH_TRANCEPTION ? dev_alloc(h, &h->raw_cache, n) : PG_OK;
     if (!rc) rc = dev_alloc(h, &h->kv_cache, n);
     if (rc) return rc;
     h->prefix_cap = h->desc.max_positions;
   }
   h->prefix_T = 0;
-  rc = forward_tranception(h, ids, 1, T, s, 1, 0);
+  rc = forward_ar(h, ids, 1, T, s, 1, 0);
   if (rc) return fail(h, rc, tls_error());
   // per-token log p(ids[t+1] | ids[<=t]) of the wild type, t = 0 .. T-2 (and the fused rows in f->out_logprobs when asked for)
   int32_t* len_dev = h->row_sel;
   PG_CUDA_OK(cudaMemcpyAsync(len_dev, &T, sizeof(int32_t), cudaMemcpyHostToDevice, s));
   { ProfScope ps(CAT_HEAD, s, 2);
-    rc = launch_ar_head(h->x, h->desc.embed_dim, 1, T, h->desc.vocab, ids, len_dev, h->lnag, h->lnab, h->embed, fu, out_tok_logp, h->tok_logp, s); }
+    rc = launch_ar_head(h->x, h->desc.embed_dim, 1, T, h->desc.vocab, ids, len_dev, h->lnag, h->lnab, h->outw ? h->outw : h->embed, fu,
+                        out_tok_logp, h->tok_logp, s); }
   if (rc) return fail(h, rc, tls_error());
   h->prefix_T = T;
   return PG_OK;
@@ -1302,7 +1360,8 @@ int pg_ar_loglik_prefix(pg_handle h, const int32_t* ids, const int32_t* lens, in
                         float* out_sum_logp, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_ar_loglik_prefix: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: weights not loaded");
-  if (h->desc.arch != PG_ARCH_TRANCEPTION) return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: handle is not a Tranception model");
+  if (h->desc.arch != PG_ARCH_TRANCEPTION && h->desc.arch != PG_ARCH_RITA)
+    return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: handle is not an autoregressive model (Tranception, RITA)");
   if (h->prefix_T <= 0) return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: no wild-type prefix recorded (call pg_ar_prefix_begin first)");
   if (start <= 0 || start % 128 || start >= h->prefix_T) return fail(h, PG_ERR_ARG, "pg_ar_loglik_prefix: start must be a positive multiple of 128 below the recorded length");
   if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_ar_loglik_prefix: bad B/T");

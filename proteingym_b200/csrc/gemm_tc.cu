@@ -23,7 +23,7 @@
 //   warpgroup 0   TMA producer (one elected thread of warp 0): cp.async.bulk.tensor 2D tiles (128 rows x 128 B of A, 128 rows
 //                 x 128 B of W, 128B swizzle; a row of 128 B is 64 fp16 or 128 e4m3 along K) into a 6-stage ring; 40 registers
 //   warpgroups 1-2 consumers, rows [0, 64) and [64, 128) of the tile: wgmma m64n128 (K = 16 fp16 / 32 e4m3: 32 B of each row) x4
-//                 per stage, then bias / erf-GELU / relu^2 / rotary / SwiGLU and fp16 hi [+ fp16 lo | + e4m3 planes for the next GEMM]
+//                 per stage, then bias / erf-GELU / relu^2 / rotary / SwiGLU / tanh-GELU and fp16 hi [+ fp16 lo | + e4m3 planes for the next GEMM]
 //                 stored straight from the accumulator fragments, or added into the fp32 residual stream (one owner per element)
 // Roofline: tensor bound. Algorithmic FLOPs = 2*M*N*K; issued tensor-pipe work = x1 / x2 / x3 by mode.
 #include <cstdlib>
@@ -91,6 +91,12 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(ax * 0.5f, fmaf(npoly, e, 1.0f), x * 0.5f);
 }
 
+// tanh-approximated GELU of RITA (rita_modeling.py:24-26), with the reference's constants: x*0.5*(1+tanh(0.79788456*x*(1+0.044715*x^2))).
+// tanhf is the accurate libdevice routine (<= 2 ulp; the library is built without fast math), not MUFU.TANH's ~2^-11 relative error.
+__device__ __forceinline__ float gelu_tanh(float x) {
+  return x * 0.5f * (1.0f + tanhf(0.79788456f * x * (1.0f + 0.044715f * x * x)));
+}
+
 // SiLU (ESM C SwiGLU, esm/layers/blocks.py:21-33): g / (1 + e^-g) with e^-g from MUFU.EX2 (ex2.approx.ftz, <= 2 ulp) and the quotient
 // from MUFU.RCP (rcp.approx.ftz, <= 1 ulp): relative error <= ~4 ulp (5e-7) over the range; for g < -88 e^-g is inf and the result 0.
 __device__ __forceinline__ float silu(float g) {
@@ -135,6 +141,9 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
         const float a = fmaxf(v0, 0.f), b = fmaxf(v1, 0.f);
         v0 = a * a;
         v1 = b * b;
+      } else if (EPI == 6) {
+        v0 = gelu_tanh(v0);
+        v1 = gelu_tanh(v1);
       }
     }
     if (EPI == 3) {
@@ -502,7 +511,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return set_error(PG_ERR_ARG, "gemm: empty problem");
   if (g.K % BK) return set_error(PG_ERR_ARG, "gemm: K must be a multiple of 64");
   if (g.nseg < 1 || g.nseg > 3) return set_error(PG_ERR_ARG, "gemm: nseg must be 1, 2 (fp16 + e4m3 cross terms) or 3");
-  if (g.epi < 0 || g.epi > 5) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
+  if (g.epi < 0 || g.epi > 6) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
   if (g.epi == 5 && (g.N % 16 || (g.out_fmt == 2 && (g.N / 2) % 64) || g.grp_rows_a || (g.out_fmt >= 1 && g.out_lo_off < g.N / 2)))
     return set_error(PG_ERR_ARG, "gemm: the SwiGLU epilogue needs N % 16 == 0 (N/2 % 64 == 0 for out_fmt 2), no groups, planes >= N/2 apart");
   if (g.epi == 2 ? !g.resid : !g.out) return set_error(PG_ERR_ARG, "gemm: missing output");
@@ -526,7 +535,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
 #define PG_SET_SMEM(E)                                                                                           \
   PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM)); \
   PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM))
-    PG_SET_SMEM(0); PG_SET_SMEM(1); PG_SET_SMEM(2); PG_SET_SMEM(3); PG_SET_SMEM(4); PG_SET_SMEM(5);
+    PG_SET_SMEM(0); PG_SET_SMEM(1); PG_SET_SMEM(2); PG_SET_SMEM(3); PG_SET_SMEM(4); PG_SET_SMEM(5); PG_SET_SMEM(6);
 #undef PG_SET_SMEM
     attr_set[dev] = true;
   }
@@ -615,7 +624,8 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
     case 2: e = PG_LAUNCH(2); break;
     case 3: e = PG_LAUNCH(3); break;
     case 4: e = PG_LAUNCH(4); break;
-    default: e = PG_LAUNCH(5); break;
+    case 5: e = PG_LAUNCH(5); break;
+    default: e = PG_LAUNCH(6); break;
   }
 #undef PG_LAUNCH
   PG_CUDA_OK(e);

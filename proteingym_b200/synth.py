@@ -14,6 +14,7 @@ oracle and contains no scoring arithmetic.
 from __future__ import annotations
 
 import argparse
+import json
 import math
 import os
 from dataclasses import dataclass
@@ -520,3 +521,94 @@ def write_esmc_checkpoint(path: str, arch: EsmcArch, seed: int = 0, state: dict 
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     torch.save(st, path)
     return st
+
+
+# ---- RITA (proteingym/baselines/rita/rita_modeling.py) ----------------------------------------------------------------------------
+@dataclass(frozen=True)
+class RitaArch:
+    layers: int
+    embed_dim: int
+    heads: int
+    ff_ratio: int = 4
+    vocab: int = 26
+
+    @property
+    def ffn_dim(self) -> int:
+        return self.embed_dim * self.ff_ratio
+
+
+RITA_S = RitaArch(12, 768, 12)
+RITA_M = RitaArch(24, 1024, 16)
+RITA_L = RitaArch(24, 1536, 24)
+
+# Character-level vocabulary of the synthetic tokenizer files: specials first, then the 20 amino acids, X and U (26 ids).
+RITA_VOCAB = ["<PAD>", "<BOS>", "<EOS>", "<unk>"] + list(AA20) + ["X", "U"]
+
+
+def make_rita_state(arch: RitaArch, seed: int = 0, untied: bool = False) -> dict:
+    """RITA state dict with the HF key names of RITAModelForCausalLM (``transformer.`` prefix, per-layer rotary inv_freq buffers), drawn
+    on the CPU from ``seed``. Linear weights and biases follow nn.Linear's U(+-1/sqrt(fan_in)); LayerNorm weights 1 + 0.1 N(0,1) and
+    biases 0.1 N(0,1); the embedding N(0, 4/d), so that logits through the tied head (LayerNorm output . embedding row) have a standard
+    deviation of about 2 and log-probabilities a few nats apart. ``lm_head.weight`` equals the embedding, or (``untied``) is drawn on its
+    own at the same scale."""
+    g = torch.Generator().manual_seed(seed)
+    d, f, V = arch.embed_dim, arch.ffn_dim, arch.vocab
+    hd = d // arch.heads
+    ln_w = lambda: 1 + 0.1 * torch.randn(d, generator=g)
+    ln_b = lambda: 0.1 * torch.randn(d, generator=g)
+    emb = (2 / math.sqrt(d)) * torch.randn((V, d), generator=g)
+    st = {"transformer.embedding.weight": emb}
+    inv_freq = 1.0 / (10000 ** (torch.arange(0, hd, 2).float() / hd))
+    for i in range(arch.layers):
+        p = f"transformer.layers.{i}."
+        for nm in ("key", "query", "value", "proj"):
+            st[p + f"self_attention.{nm}.weight"] = _uniform(g, (d, d), 1 / math.sqrt(d))
+            st[p + f"self_attention.{nm}.bias"] = _uniform(g, (d,), 1 / math.sqrt(d))
+        st[p + "self_attention.rotary_embedding.inv_freq"] = inv_freq.clone()
+        st[p + "attn_norm.weight"] = ln_w()
+        st[p + "attn_norm.bias"] = ln_b()
+        st[p + "mlp.0.weight"] = _uniform(g, (f, d), 1 / math.sqrt(d))
+        st[p + "mlp.0.bias"] = _uniform(g, (f,), 1 / math.sqrt(d))
+        st[p + "mlp.2.weight"] = _uniform(g, (d, f), 1 / math.sqrt(f))
+        st[p + "mlp.2.bias"] = _uniform(g, (d,), 1 / math.sqrt(f))
+        st[p + "mlp_norm.weight"] = ln_w()
+        st[p + "mlp_norm.bias"] = ln_b()
+    st["transformer.final_norm.weight"] = ln_w()
+    st["transformer.final_norm.bias"] = ln_b()
+    st["lm_head.weight"] = (2 / math.sqrt(d)) * torch.randn((V, d), generator=g) if untied else emb.clone()
+    return st
+
+
+def write_rita_checkpoint(folder: str, arch: RitaArch, seed: int = 0, state: dict | None = None, untied: bool = False,
+                          safetensors: bool = False) -> dict:
+    """A RITA model directory: config.json (``tie_word_embeddings`` written out: false for ``untied``) and pytorch_model.bin or
+    model.safetensors."""
+    os.makedirs(folder, exist_ok=True)
+    st = make_rita_state(arch, seed, untied) if state is None else state
+    cfg = dict(model_type="rita", d_model=arch.embed_dim, num_layers=arch.layers, num_heads=arch.heads, ff_ratio=arch.ff_ratio,
+               vocab_size=arch.vocab, max_seq_len=1024, dropout=0.0, eos_token_id=2, tie_word_embeddings=not untied)
+    with open(os.path.join(folder, "config.json"), "w") as fh:
+        json.dump(cfg, fh, indent=1)
+    if safetensors:
+        from safetensors.torch import save_file
+        save_file({k: v.contiguous() for k, v in st.items()}, os.path.join(folder, "model.safetensors"))
+    else:
+        torch.save(st, os.path.join(folder, "pytorch_model.bin"))
+    return st
+
+
+def write_rita_tokenizer(folder: str, template: bool = False) -> str:
+    """A character-level tokenizer.json (BPE without merges over RITA_VOCAB, unknown characters -> <unk>) written by the ``tokenizers``
+    library, plus a tokenizer_config.json naming the fast tokenizer class. ``template``: a post-processor that wraps every sequence as
+    <BOS> seq <EOS>; otherwise encode() adds nothing."""
+    from tokenizers import Tokenizer, models, processors
+    os.makedirs(folder, exist_ok=True)
+    tok = Tokenizer(models.BPE(vocab={t: i for i, t in enumerate(RITA_VOCAB)}, merges=[], unk_token="<unk>"))
+    tok.add_special_tokens(["<PAD>", "<BOS>", "<EOS>", "<unk>"])
+    if template:
+        tok.post_processor = processors.TemplateProcessing(single="<BOS> $A <EOS>", special_tokens=[("<BOS>", 1), ("<EOS>", 2)])
+    path = os.path.join(folder, "tokenizer.json")
+    tok.save(path)
+    with open(os.path.join(folder, "tokenizer_config.json"), "w") as fh:
+        json.dump(dict(tokenizer_class="PreTrainedTokenizerFast", pad_token="<PAD>", eos_token="<EOS>", unk_token="<unk>"), fh, indent=1)
+    return path

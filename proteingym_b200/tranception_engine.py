@@ -117,6 +117,22 @@ def replace_ambiguous(seq: str) -> str:
     return seq
 
 
+def prefix_split(x, w, offset: int = 1, tile: int = 128):
+    """Exact wild-type-prefix reuse in a causal decoder: for a sequence ``x`` and the wild type ``w`` it shares a prefix with (both strings
+    or token lists, in scoring order) -> (fd, start): fd = the token index of the first difference (``offset`` tokens precede element 0,
+    e.g. 1 for [CLS]) and start = fd rounded down to the attention tile, the first row the transformer has to run for ``x``."""
+    diff = next((k for k, (c, e) in enumerate(zip(x, w)) if c != e), len(x))
+    fd = offset + diff
+    return fd, (fd // tile) * tile
+
+
+def prefix_total(wt_csum, wt_rows, start: int, label: int, suffix_sum) -> np.float32:
+    """A sequence's summed log-likelihood recombined from its suffix pass (rows >= start) and the wild type's pass: rows < start - 1
+    predict shared tokens (``wt_csum[k]`` = sum of the wild type's rows 0 .. k-1), row start - 1 has the wild type's state but predicts
+    the sequence's own token ``label`` (``wt_rows`` [T, vocab]: the wild type's log-probability rows)."""
+    return np.float32(wt_csum[start - 1] + float(wt_rows[start - 1, label]) + float(suffix_sum))
+
+
 def prior_rows(prow, prow2, ws, we, msa_start, msa_end, flip, nonfocus=None):
     """Index arithmetic of the retrieval fusion for one sequence slice [ws, we) of the full protein (Tranception
     model_pytorch.py:811-830; TranceptEVE model_pytorch.py:1085-1133): fill ``prow`` (and ``prow2`` for the EVE table) with the prior
@@ -324,8 +340,7 @@ class TranceptionScorer:
             start = 0
             if (self.prefix_reuse and w is not None and x != w and len(x) == len(w) and len(x) + 2 > tile
                     and not any(c in "XBJZ" for c in x) and not any(c in "XBJZ" for c in w)):  # those are re-drawn at random per call
-                diff = next((k for k, (c, e) in enumerate(zip(x, w)) if c != e), len(x))
-                start = ((1 + diff) // tile) * tile            # token index of the first change is 1 + diff ([CLS] is token 0)
+                start = prefix_split(x, w, 1, tile)[1]          # token index of the first change is 1 + diff ([CLS] is token 0)
             if start > 0:
                 groups.setdefault((w, windows[i], start), []).append(i)
             else:
@@ -353,7 +368,7 @@ class TranceptionScorer:
                 suffix = self._prefix_suffix([strings[i] for i in members], win, start, flip, prior_kw)
                 for i, sfx in zip(members, suffix):
                     tok_s = TOK.get(strings[i][start - 1], 0)                         # token `start` of [CLS] x [SEP] is character start-1
-                    out[i] = np.float32(csum[start - 1] + float(wt_rows[start - 1, tok_s]) + float(sfx))
+                    out[i] = prefix_total(csum, wt_rows, start, tok_s, sfx)
         if self.reuse_rows is None:
             self.reuse_rows = [0, 0]
         self.reuse_rows[0] += rows_full
@@ -535,9 +550,7 @@ def prefix_reuse_plan(slices: pd.DataFrame, target_seq: str, tile: int = 128) ->
             continue  # indels: no position-wise correspondence with a WT slice
         T = len(s) + 2
         for direction, x, y in (("L_to_R", s, wt), ("R_to_L", s[::-1], wt[::-1])):
-            diff = next((i for i, (c, d) in enumerate(zip(x, y)) if c != d), len(x))
-            fd = 1 + diff                                    # token index ([CLS] is token 0)
-            start = (fd // tile) * tile
+            fd, start = prefix_split(x, y, 1, tile)          # token index ([CLS] is token 0)
             recs.append((ms, a, b, direction, T, fd, start, T - fd, T - start))
     return pd.DataFrame(recs, columns=["mutated_sequence", "window_start", "window_end", "direction", "tokens", "first_diff_token",
                                        "aligned_start", "rows_exact", "rows_tile_aligned"])

@@ -37,7 +37,7 @@ enum pg_arch {
                               "rotary.cos" / "rotary.sin" [T, 32]. Windows (compute_fitness.py:346-409 re-tokenises each one as
                               <cls> slice <eos>) are the caller's: pass one token row per distinct window, concatenated, with
                               win_start[p] = that row's offset and positions[p] = offset + index within the row. */
-  PG_ARCH_RITA = 5         /* RITA S / M / L causal decoder (proteingym/baselines/rita/rita_modeling.py:129-252): pre-LN blocks, separate
+  PG_ARCH_RITA = 5,        /* RITA S / M / L causal decoder (proteingym/baselines/rita/rita_modeling.py:129-252): pre-LN blocks, separate
                               q/k/v Linear with bias, rotate-half rotary over 64-wide heads, no attention bias, tanh-GELU MLP (ffn_dim =
                               ff_ratio * d), final LayerNorm, head without bias; heads = embed_dim / 64 (RITA XL's 128-wide heads are
                               refused), max_positions = rows of the rotary tables = the longest token row a call may pass. Scored through
@@ -46,6 +46,21 @@ enum pg_arch {
                               "layers.{i}.mlp.{0,2}.*", "embedding.weight", "final_norm.*"), "lm_head.weight" [vocab, d] only for an
                               untied head (absent = the embedding), plus "rotary.cos" / "rotary.sin" [T, 32] = cos / sin(t * inv_freq[c])
                               from the checkpoint's rotary_embedding.inv_freq. */
+  PG_ARCH_PROGEN2 = 6      /* ProGen2 small / medium / base / large causal decoder (proteingym/baselines/progen2/models/progen/
+                              modeling_progen.py:60-282, 389-401, 541-548): parallel residual x + attn(ln_1(x)) + mlp(ln_1(x)), bias-free
+                              fused qkv_proj in 8 [q | v | k] shards (heads % 8 == 0), interleaved (rotate_every_two) rotary on the first
+                              rotary_dim dims of q and k, bias-free out_proj, tanh-GELU MLP (ffn_dim = n_inner or 4d) with biases, ln_f, and
+                              lm_head WITH bias of which only rows 5..29 are scored (compute_fitness.py:71-77: token ids 5..29, vocab =
+                              the embedding rows, >= 30). head_dim 64 runs in 64-wide head slots, 66..128 (even) in 128-wide slots; head_dim
+                              > 128 (progen2-xlarge) and PG_PREC_F16D are refused. max_positions = the longest token row a call may pass.
+                              Scored through the pg_ar_* entry points without retrieval fusion: token ids are the full vocabulary's, a
+                              next token outside 5..29 gives a NaN log-probability, and out_logprobs rows are 25 wide. Weights: the HF
+                              state-dict keys without "transformer." ("h.{i}.ln_1.*", "h.{i}.attn.qkv_proj.weight" [3d, d],
+                              "h.{i}.attn.out_proj.weight", "h.{i}.mlp.{fc_in,fc_out}.{weight,bias}", "wte.weight", "ln_f.*",
+                              "lm_head.weight" [vocab, d], "lm_head.bias" [vocab]) plus "rotary.cos" / "rotary.sin" [T, S/2] with S the
+                              slot width: column i < rotary_dim / 2 holds cos / sin(t * 10000^(-2i / rotary_dim)) in fp32 as
+                              fixed_pos_embedding computes it (rotary_dim = head_dim when the config has none), later columns cos = 1,
+                              sin = 0. ln_1 / ln_f use eps 1e-5. */
 };
 
 /* Tensor-core operand precision. The reference is strict fp32 (SURVEY.md §0.4). Every operand is an fp16 pair hi + lo.

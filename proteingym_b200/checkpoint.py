@@ -233,6 +233,21 @@ def esmc_rotary_tables(T: int = 1024):
 
 
 # ---- RITA (proteingym/baselines/rita: rita_configuration.py, rita_modeling.py) ----------------------------------------------------
+def _read_hf_weights(folder: str) -> dict:
+    """The state dict of a Hugging Face model directory: pytorch_model.bin, else every *.safetensors file."""
+    pbin = os.path.join(folder, "pytorch_model.bin")
+    if os.path.exists(pbin):
+        return torch.load(pbin, map_location="cpu", weights_only=True)
+    st_files = sorted(Path(folder).glob("*.safetensors"))
+    if not st_files:
+        raise FileNotFoundError(f"{folder}: neither pytorch_model.bin nor *.safetensors")
+    from safetensors.torch import load_file
+    raw = {}
+    for f in st_files:
+        raw.update(load_file(str(f)))
+    return raw
+
+
 @dataclass
 class RitaConfig:
     layers: int
@@ -258,17 +273,7 @@ def load_rita_checkpoint(folder: str):
     import json
     import warnings
     cfg = json.load(open(os.path.join(folder, "config.json")))
-    pbin = os.path.join(folder, "pytorch_model.bin")
-    if os.path.exists(pbin):
-        raw = torch.load(pbin, map_location="cpu", weights_only=True)
-    else:
-        st_files = sorted(Path(folder).glob("*.safetensors"))
-        if not st_files:
-            raise FileNotFoundError(f"{folder}: neither pytorch_model.bin nor *.safetensors")
-        from safetensors.torch import load_file
-        raw = {}
-        for f in st_files:
-            raw.update(load_file(str(f)))
+    raw = _read_hf_weights(folder)
     d, layers, heads = int(cfg.get("d_model", 768)), int(cfg.get("num_layers", 12)), int(cfg.get("num_heads", 12))
     ffn, vocab = d * int(cfg.get("ff_ratio", 4)), int(cfg.get("vocab_size", 26))
     tied = bool(cfg.get("tie_word_embeddings", True))
@@ -310,3 +315,86 @@ def load_rita_checkpoint(folder: str):
     if d % heads or inv_freq.numel() != (d // heads) // 2:
         raise ValueError(f"RITA: d_model {d} / num_heads {heads} does not match inv_freq of {inv_freq.numel()} frequencies")
     return RitaConfig(layers, d, heads, ffn, vocab, tied), state, inv_freq
+
+
+@dataclass
+class Progen2Config:
+    layers: int
+    embed_dim: int
+    heads: int
+    ffn_dim: int
+    vocab: int
+    rotary_dim: int          # rotary dims per head, from the front of each head (modeling_progen.py:178-186)
+    n_positions: int         # the scorer's chunk length (compute_fitness.py:163)
+
+    @property
+    def head_dim(self) -> int:
+        return self.embed_dim // self.heads
+
+
+def load_progen2_checkpoint(folder: str):
+    """ProGen2 model directory -> (Progen2Config, state). ``state`` has the key names of include/pgscore.h's PG_ARCH_PROGEN2 (the
+    ``transformer.`` prefix stripped, the causal-mask buffers ``attn.bias`` / ``attn.masked_bias`` dropped) as fp32 CPU tensors, any
+    stored dtype upcast.
+
+    config.json: ``n_embd``, ``n_layer``, ``n_head``, ``rotary_dim``, ``n_inner``, ``n_positions``, ``vocab_size``, ``layer_norm_epsilon``
+    and ``activation_function``, with ProGenConfig's defaults for absent keys (configuration_progen.py:26-46). Weights:
+    pytorch_model.bin or *.safetensors. What the kernels do not implement is refused: LayerNorm eps other than 1e-5, an activation other
+    than gelu_new, head_dim > 128 (progen2-xlarge), a vocabulary without the scored columns 5..29."""
+    import json
+    cfg = json.load(open(os.path.join(folder, "config.json")))
+    raw = _read_hf_weights(folder)
+    d, layers, heads = int(cfg.get("n_embd", 4096)), int(cfg.get("n_layer", 28)), int(cfg.get("n_head", 16))
+    vocab, npos = int(cfg.get("vocab_size", 50400)), int(cfg.get("n_positions", 2048))
+    ffn = int(cfg["n_inner"]) if cfg.get("n_inner") is not None else 4 * d
+    eps = float(cfg.get("layer_norm_epsilon", 1e-5))
+    act = cfg.get("activation_function", "gelu_new")
+    if d % heads:
+        raise ValueError(f"ProGen2: n_embd {d} is not a multiple of n_head {heads}")
+    hd = d // heads
+    rot = cfg.get("rotary_dim", 64)
+    if rot is None:  # the attention would rotate the whole head (:187-190), but ProGenModel.__init__ fails first (:325)
+        raise ValueError("ProGen2: rotary_dim null: the reference's ProGenModel cannot be built with it (modeling_progen.py:325)")
+    rot = int(rot)
+    if eps != 1e-5:
+        raise NotImplementedError(f"ProGen2: layer_norm_epsilon {eps}: the LayerNorm kernels use eps 1e-5")
+    if act != "gelu_new":
+        raise NotImplementedError(f"ProGen2: activation_function {act!r}: the MLP epilogue implements gelu_new (tanh GELU)")
+    if hd > 128:
+        raise NotImplementedError(f"ProGen2: head_dim {hd} (n_embd {d} / n_head {heads}, progen2-xlarge) has no attention tile (at most 128)")
+    if rot % 2 or not 0 < rot <= hd:
+        raise ValueError(f"ProGen2: rotary_dim {rot} must be even and within head_dim {hd}")
+    if vocab < 30:
+        raise ValueError(f"ProGen2: vocab_size {vocab} lacks the scored token ids 5..29")
+    state = {}
+    for k, v in raw.items():
+        name = k[len("transformer."):] if k.startswith("transformer.") else k
+        if name.endswith("attn.bias") or name.endswith("attn.masked_bias"):
+            continue
+        state[name] = v.detach().float().contiguous()
+    want = {"wte.weight": (vocab, d), "ln_f.weight": (d,), "ln_f.bias": (d,), "lm_head.weight": (vocab, d), "lm_head.bias": (vocab,)}
+    for i in range(layers):
+        p = f"h.{i}."
+        want.update({p + "ln_1.weight": (d,), p + "ln_1.bias": (d,), p + "attn.qkv_proj.weight": (3 * d, d),
+                     p + "attn.out_proj.weight": (d, d), p + "mlp.fc_in.weight": (ffn, d), p + "mlp.fc_in.bias": (ffn,),
+                     p + "mlp.fc_out.weight": (d, ffn), p + "mlp.fc_out.bias": (d,)})
+    for k, shape in want.items():
+        if k not in state:
+            raise ValueError(f"ProGen2 state dict: missing {k}")
+        if tuple(state[k].shape) != shape:
+            raise ValueError(f"ProGen2 state dict: {k} has shape {tuple(state[k].shape)}, expected {shape}")
+    extra = sorted(set(state) - set(want))
+    if extra:
+        raise ValueError(f"ProGen2 state dict: unexpected keys {extra[:5]}")
+    return Progen2Config(layers, d, heads, ffn, vocab, rot, npos), state
+
+
+def progen2_rotary_tables(rotary_dim: int, slot: int, T: int):
+    """cos/sin [T, slot/2] for the library's rotary epilogue: columns i < rotary_dim/2 hold sin / cos(t * inv_freq[i]) computed as
+    fixed_pos_embedding does (modeling_progen.py:38-44: inv_freq = 1 / 10000^(arange(0, dim, 2) / dim) and the outer product in fp32),
+    the others cos = 1, sin = 0 (dims that pass through unrotated)."""
+    inv_freq = 1.0 / (10000 ** (torch.arange(0, rotary_dim, 2) / rotary_dim))
+    sinusoid = torch.einsum("i , j -> i j", torch.arange(T), inv_freq).float()
+    cos, sin = torch.ones((T, slot // 2)), torch.zeros((T, slot // 2))
+    cos[:, :rotary_dim // 2], sin[:, :rotary_dim // 2] = torch.cos(sinusoid), torch.sin(sinusoid)
+    return cos.contiguous(), sin.contiguous()

@@ -173,13 +173,15 @@ constexpr float S_SWIGLU = 2.f; // silu(g) * v (ESM C)         -> fc2 GEMM      
 
 // Operand formats of a precision mode (common.h fmt 0 / 1 / 2), fixed at pg_create. Pitches and offsets in fp16 elements.
 // Widths (DESIGN.md §3): residual rows d; GEMM-input rows of width d (LayerNorm outputs) dk = d rounded up to 64, zero-padded; q/k/v
-// and attention outputs da = heads * 64, head h in the slot [64h, 64h + 64), zeros after its head_dim columns. All d for hd 64.
+// and attention outputs da = heads * S, head h in the slot [Sh, Sh + S), zeros after its head_dim columns. S = 64, except ProGen2's
+// 80- and 96-wide heads: S = 128. All d for hd 64.
 struct OpFmt {
   int np = 1;    // operand row pitch in units of the fp16 hi plane: 1 (fp16) or 2 (hi | lo, or hi | e4m3 planes)
   int nseg = 1;  // GEMM operand mode: 1 fp16, 3 fp16 hi/lo x3, 2 fp16 + e4m3 cross terms
   int afmt = 0;  // GEMM inputs (LayerNorm, attention and fc1 outputs): 2 under nseg 2, else 1 when np == 2
   int qfmt = 0;  // q/k/v rows, read by the attention kernels: fp16 hi [| lo]
   int pseg = 1;  // nseg of the operands that are fp16 hi [| lo] in every mode (attention, the MSA tied GEMMs): 3 when np == 2
+  int slot = 64;                               // head slot width S
   int dk = 0, da = 0;                          // plane widths of GEMM-input rows of width d, and of attention rows (see above)
   int64_t ldd = 0, ldf = 0, ldat = 0, ldq = 0;  // pitches of dk-, ffn-, da- and 3da-wide rows
   int64_t lo_d = 0, lo_at = 0, lo_q = 0;        // offset of the planes after the hi plane in dk-, da- and 3da-wide rows (0: none)
@@ -192,7 +194,8 @@ OpFmt op_fmt(const pg_model_desc& D) {
   o.qfmt = o.np - 1;
   o.pseg = o.np == 2 ? 3 : 1;
   o.dk = (D.embed_dim + 63) / 64 * 64;
-  o.da = D.heads * 64;
+  o.slot = D.arch == PG_ARCH_PROGEN2 && D.embed_dim / D.heads > 64 ? 128 : 64;
+  o.da = D.heads * o.slot;
   o.ldd = static_cast<int64_t>(o.dk) * o.np;
   o.ldf = static_cast<int64_t>(D.ffn_dim) * o.np;
   o.ldat = static_cast<int64_t>(o.da) * o.np;
@@ -203,25 +206,39 @@ OpFmt op_fmt(const pg_model_desc& D) {
   return o;
 }
 
-// Slot maps: index i of a padded width -> source index, or -1 (zero). SL_PAD: i < n (dk columns). SL_HEAD: dim c of head h at 64h + c
-// (v rows, out_proj columns). SL_ROT (q/k rows): dims c < hd/2 at 64h + c, the others at 64h + 32 + (c - hd/2), so ESM2's rotate-half
-// partners (c, c + hd/2) sit on the pair (c', c' + 32) the GEMM's rotary epilogue rotates; q.k is unchanged.
-enum SlotMap { SL_PAD = 0, SL_HEAD, SL_ROT };
-__device__ __forceinline__ int slot_src(int i, int map, int n, int hd) {
+// Slot maps: index i of a padded width -> source index, or -1 (zero); S = the slot width (64 or 128). SL_PAD: i < n (dk columns).
+// SL_HEAD: dim c of head h at Sh + c (v rows, out_proj columns). SL_ROT (q/k rows): dims c < hd/2 at Sh + c, the others at
+// Sh + S/2 + (c - hd/2), so ESM2's rotate-half partners (c, c + hd/2) sit on the pair (c', c' + S/2) the GEMM's rotary epilogue
+// rotates; q.k is unchanged.
+// ProGen2's fused qkv_proj [3d, d] (modeling_progen.py:157-168) is 8 shards of [q | v | k] rows, d/8 each; head h is sub-head
+// h % (heads/8) of shard h / (heads/8). SL_PGQ / SL_PGK place its q / k rows with each rotate_every_two pair (2i, 2i+1) on the slot
+// pair (Sh + i, Sh + S/2 + i), i < hd/2, which turns the interleaved rotation into the epilogue's rotate-half; SL_PGV places v dim c
+// at Sh + c. For these maps n = d.
+enum SlotMap { SL_PAD = 0, SL_HEAD, SL_ROT, SL_PGQ, SL_PGK, SL_PGV };
+__device__ __forceinline__ int slot_src(int i, int map, int n, int hd, int S) {
   if (map == SL_PAD) return i < n ? i : -1;
-  const int h = i >> 6, c = i & 63;
+  const int h = i / S, c = i % S, half = hd >> 1, hs = S >> 1;
   if (map == SL_HEAD) return c < hd ? h * hd + c : -1;
-  const int half = hd >> 1;
-  if (c < half) return h * hd + c;
-  if (c >= 32 && c < 32 + half) return h * hd + half + (c - 32);
+  if (map == SL_ROT) {
+    if (c < half) return h * hd + c;
+    if (c >= hs && c < hs + half) return h * hd + half + (c - hs);
+    return -1;
+  }
+  const int per = n / hd / 8;  // heads per shard
+  const int base = (h / per) * (3 * n / 8) + (h % per) * hd;
+  if (map == SL_PGV) return c < hd ? base + n / 8 + c : -1;
+  const int part = map == SL_PGQ ? 0 : 2 * n / 8;
+  if (c < half) return base + part + 2 * c;
+  if (c >= hs && c < hs + half) return base + part + 2 * (c - hs) + 1;
   return -1;
 }
-// dst [N, K] = src [n_src, k_src] (row-major) with its rows placed by map rmap and its columns by cmap, zeros elsewhere.
-__global__ void expand_slots_kernel(const float* __restrict__ src, int n_src, int k_src, float* __restrict__ dst, int N, int K, int rmap,
-                                    int cmap, int hd) {
+// dst [N, K] = src [*, k_src] (row-major) with its rows placed by map rmap (over rn source rows) and its columns by cmap (over kn
+// source columns), zeros elsewhere.
+__global__ void expand_slots_kernel(const float* __restrict__ src, int rn, int k_src, float* __restrict__ dst, int N, int K, int rmap,
+                                    int cmap, int hd, int S, int kn) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= static_cast<long long>(N) * K) return;
-  const int r = slot_src(static_cast<int>(i / K), rmap, n_src, hd), c = slot_src(static_cast<int>(i % K), cmap, k_src, hd);
+  const int r = slot_src(static_cast<int>(i / K), rmap, rn, hd, S), c = slot_src(static_cast<int>(i % K), cmap, kn, hd, S);
   dst[i] = (r >= 0 && c >= 0) ? src[static_cast<long long>(r) * k_src + c] : 0.f;
 }
 
@@ -250,6 +267,7 @@ struct pg_handle_s {
   float *embed = nullptr, *pos = nullptr, *lnbg = nullptr, *lnbb = nullptr, *lnag = nullptr, *lnab = nullptr;
   float *hdw = nullptr, *hdb = nullptr, *hlng = nullptr, *hlnb = nullptr, *hbias = nullptr;
   float* outw = nullptr;  // untied output matrix [vocab, d] (ESM C sequence_head.3); null = the tied embedding
+  int head_vocab = 0, label_off = 0;  // autoregressive head: columns (ProGen2: 25, vocabulary rows 5..29) and token id of column 0
   float *rot_cos = nullptr, *rot_sin = nullptr;
   int rot_rows = 0;
   // workspace
@@ -288,6 +306,8 @@ struct pg_handle_s {
 
 namespace pg {
 namespace {
+
+bool is_ar(int arch) { return arch == PG_ARCH_TRANCEPTION || arch == PG_ARCH_RITA || arch == PG_ARCH_PROGEN2; }
 
 int fail(pg_handle h, int code, const std::string& msg) {
   if (h) h->err = msg;
@@ -361,9 +381,10 @@ int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int
   g.epi = epi;
   g.out = out; g.ldo = static_cast<int64_t>(n_out) * h->op.np; g.out_fmt = p == QKV ? h->op.qfmt : h->op.afmt;
   g.out_lo_off = g.out_fmt ? n_out : 0; g.out_scale = out_scale;
-  if (epi == 3) {  // q and k slots
-    g.rot_cos = h->rot_cos + static_cast<int64_t>(rot_start) * 32; g.rot_sin = h->rot_sin + static_cast<int64_t>(rot_start) * 32;
-    g.rot_T = rot_T; g.rot_dim = h->op.da;
+  if (epi == 3) {  // q and k slots; tables [T, S/2]
+    const int hs = h->op.slot / 2;
+    g.rot_cos = h->rot_cos + static_cast<int64_t>(rot_start) * hs; g.rot_sin = h->rot_sin + static_cast<int64_t>(rot_start) * hs;
+    g.rot_T = rot_T; g.rot_dim = h->op.da; g.rot_half = hs;
   }
   ProfScope ps(p, s);
   return launch_gemm(g, s);
@@ -403,7 +424,7 @@ AttnLaunch attn_args(pg_handle h, const __half* qkv, __half* out, int B, int T) 
   AttnLaunch a{};
   a.qkv = qkv; a.ld = o.ldq; a.lo_off = o.lo_q;
   a.out = out; a.ldo = o.ldat; a.out_lo_off = o.lo_at; a.out_fmt = o.afmt; a.out_scale = S_ATT;
-  a.B = B; a.T = T; a.heads = h->desc.heads; a.nseg = o.pseg; a.causal = 0; a.alibi_slopes = nullptr;
+  a.B = B; a.T = T; a.heads = h->desc.heads; a.nseg = o.pseg; a.causal = 0; a.alibi_slopes = nullptr; a.head_dim = o.slot;
   return a;
 }
 
@@ -600,6 +621,9 @@ int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const i
 //   Tranception (model_pytorch.py:526-612): grouped ALiBi, depthwise-conv q/k/v, relu^2 MLP.
 //   RITA (rita_modeling.py:129-210, 244-252): rotary q/k (GEMM epilogue 3, q pre-scaled by 1/8 at load), no attention bias, tanh-GELU
 //   MLP (epilogue 6).
+//   ProGen2 (modeling_progen.py:244-282): RITA's rotary attention and tanh-GELU MLP as a parallel residual, x + attn(h) + mlp(h) with
+//   h = ln_1(x): fc_in runs on ln_1's output before attention overwrites it, then out_proj and fc_out add into x in that order (the
+//   reference adds (attn + mlp) + x: an fp32 reassociation).
 // mode 0: plain forward. mode 1 (B == 1): also record every layer's keys / values (Tranception: the raw q/k/v rows for the conv
 // look-back and the conv'd rows; RITA: the rotated rows) into the prefix caches.
 // mode 2: the B sequences are rows [start, start + T) of sequences whose first `start` rows (multiple of 128) equal the recorded
@@ -607,7 +631,8 @@ int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const i
 // absolute positions start + t.
 int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, int mode = 0, int start = 0) {
   const pg_model_desc& D = h->desc;
-  const bool rita = D.arch == PG_ARCH_RITA;
+  const bool progen2 = D.arch == PG_ARCH_PROGEN2;
+  const bool rita = D.arch == PG_ARCH_RITA || progen2;  // rotary, no conv, no ALiBi, tanh-GELU
   const int64_t ldq = h->op.ldq;
   const int rows = B * T;
   int rc;
@@ -617,6 +642,7 @@ int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, in
     const Layer& L = h->layers[l];
     if ((rc = ln(h, h->x, L.ln1g, L.ln1b, rows, h->abuf, s))) return rc;
     if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s, rita ? 3 : 0, 0.f, T, mode == 2 ? start : 0))) return rc;
+    if (progen2 && (rc = lin(h, L, FC1, h->abuf, S_LN, rows, h->fbuf, s, 6, S_GELU))) return rc;
     const size_t layer_off = static_cast<size_t>(l) * h->prefix_cap * ldq;
     const __half* kv = h->qkv;  // the q/k/v rows attention reads
     if (!rita) {
@@ -636,7 +662,9 @@ int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, in
     { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
     if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
-    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, rita ? 6 : 4, rita ? S_GELU : S_RELU2, s))) return rc;
+    if (progen2) rc = lin_add(h, L, FC2, h->fbuf, S_GELU, rows, h->x, s);
+    else rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, rita ? 6 : 4, rita ? S_GELU : S_RELU2, s);
+    if (rc) return rc;
   }
   return PG_OK;
 }
@@ -781,6 +809,13 @@ int compact_head(pg_handle h, int T, int Bc, float* out, int launches, cudaStrea
   return launch_head(hl, s);
 }
 
+// The autoregressive head (ln_f, the handle's head matrix and bias, log-softmax) on B sequences of T rows in h->x.
+int ar_head(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, const ArFusion& f, float* tok_logp, float* out_sum,
+            cudaStream_t s) {
+  return launch_ar_head(h->x, h->desc.embed_dim, B, T, h->head_vocab, ids, lens, h->lnag, h->lnab, h->outw ? h->outw : h->embed,
+                        h->desc.arch == PG_ARCH_PROGEN2 ? h->hbias : nullptr, h->label_off, f, tok_logp, out_sum, s);
+}
+
 // The decoder passes over B sequences of T rows (forward_ar mode 0, or mode 2 after the recorded prefix at `start`), as many sequences
 // per pass as the workspace holds, each followed by the head on its rows (the tied embedding, or RITA's untied lm_head).
 int ar_passes(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, int mode, int start, const ArFusion& fusion,
@@ -795,9 +830,8 @@ int ar_passes(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T
     ArFusion fc = fusion;
     if (fc.prior_row) fc.prior_row += off;
     if (fc.prior_row2) fc.prior_row2 += off;
-    if (fc.out_logprobs) fc.out_logprobs += off * h->desc.vocab;
-    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->lnag, h->lnab, h->outw ? h->outw : h->embed,
-                        fc, h->tok_logp, out_sum_logp + b0, s);
+    if (fc.out_logprobs) fc.out_logprobs += off * h->head_vocab;
+    rc = ar_head(h, ids + off, lens + b0, Bc, T, fc, h->tok_logp, out_sum_logp + b0, s);
     if (rc) return fail(h, rc, tls_error());
   }
   return PG_OK;
@@ -853,7 +887,16 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   const pg_model_desc& D = *desc;
   if (D.layers <= 0 || D.embed_dim <= 0 || D.heads <= 0 || D.ffn_dim <= 0 || D.vocab <= 0)
     return set_error(PG_ERR_ARG, "pg_create: non-positive model dimension");
-  if (D.arch == PG_ARCH_ESM2) {  // narrow heads in 64-wide slots, widths padded to 64 (OpFmt)
+  if (D.arch == PG_ARCH_PROGEN2) {  // head_dim 64 in 64-wide slots, 65..128 in 128-wide slots (OpFmt)
+    const int hd = D.embed_dim % D.heads ? 0 : D.embed_dim / D.heads;
+    if (hd > 128)
+      return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen2 head_dim " + std::to_string(hd) +
+                                               " > 128 (progen2-xlarge, 4096 / 16 = 256) has no attention tile");
+    if (hd < 64 || hd % 2) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen2 needs an even head_dim from 64 to 128");
+    if (D.heads % 8) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen2 needs heads % 8 == 0 (qkv_proj is 8 shards, modeling_progen.py:157-168)");
+    if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
+    if (D.vocab < 30) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen2 scores vocabulary columns 5..29 (vocab >= 30)");
+  } else if (D.arch == PG_ARCH_ESM2) {  // narrow heads in 64-wide slots, widths padded to 64 (OpFmt)
     if (D.embed_dim % D.heads || (D.embed_dim / D.heads) % 2 || D.embed_dim / D.heads > 64)
       return set_error(PG_ERR_UNSUPPORTED, "pg_create: ESM2 head_dim must be even and at most 64");
     if (D.embed_dim % 4 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ESM2 needs embed_dim % 4 == 0 and ffn_dim % 64 == 0");
@@ -864,7 +907,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
   }
   if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC &&
-      D.arch != PG_ARCH_RITA)
+      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2)
     return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
   if (D.arch == PG_ARCH_ESMC && D.heads > 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: the ESM C q/k LayerNorm kernel holds at most 24 heads");
   if (D.arch == PG_ARCH_TRANCEPTION && D.heads % 4) return set_error(PG_ERR_UNSUPPORTED, "pg_create: Tranception needs heads % 4 == 0 (model_pytorch.py:129-131)");
@@ -885,6 +928,8 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   h->delta = (D.precision == PG_PREC_F16D);
   h->max_rows = D.max_rows > 0 ? D.max_rows : 131072;
   h->head_cap = 8192;
+  h->head_vocab = D.arch == PG_ARCH_PROGEN2 ? 25 : D.vocab;
+  h->label_off = D.arch == PG_ARCH_PROGEN2 ? 5 : 0;
   const int d = D.embed_dim, f = D.ffn_dim, np = h->op.np, dk = h->op.dk, da = h->op.da;
   const int dw = dk > da ? dk : da;  // abuf / cabuf hold both LayerNorm outputs (dk) and attention outputs (da)
   int rc = PG_OK;
@@ -895,13 +940,14 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   for (auto& L : h->layers) {
     A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
     A(&L.w1, static_cast<size_t>(f1) * dk * np); A(&L.w2, static_cast<size_t>(d) * f * np);
-    if (!esmc) { A(&L.bqkv, 3 * da); A(&L.bo, d); A(&L.b1, f); A(&L.b2, d); }  // ESM C linear layers have no bias (null = none)
+    if (!esmc && D.arch != PG_ARCH_PROGEN2) { A(&L.bqkv, 3 * da); A(&L.bo, d); }  // ESM C and ProGen2 attention: no bias (null = none)
+    if (!esmc) { A(&L.b1, f); A(&L.b2, d); }  // ESM C MLP: no bias
     A(&L.ln1g, d); A(&L.ln1b, d); A(&L.ln2g, d); A(&L.ln2b, d);
     if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); A(&L.i1, f1); A(&L.i2, d); }
     if (D.arch == PG_ARCH_TRANCEPTION) A(&L.conv_taps, 3 * 4 * 64 * 8);
     if (esmc) { A(&L.qlng, d); A(&L.klng, d); }
   }
-  if (esmc || D.arch == PG_ARCH_RITA) A(&h->outw, static_cast<size_t>(D.vocab) * d);
+  if (esmc || D.arch == PG_ARCH_RITA || D.arch == PG_ARCH_PROGEN2) A(&h->outw, static_cast<size_t>(D.vocab) * d);
   if (D.arch == PG_ARCH_MSA) {
     h->col_layers.resize(D.layers);
     for (auto& L : h->col_layers) {
@@ -915,7 +961,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     A(&h->qkv2, static_cast<size_t>(h->max_rows) * 3 * d * np);
     A(&h->slopes, D.heads);
   }
-  if (D.arch == PG_ARCH_TRANCEPTION || D.arch == PG_ARCH_RITA) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
+  if (D.arch == PG_ARCH_TRANCEPTION || D.arch == PG_ARCH_RITA || D.arch == PG_ARCH_PROGEN2) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
   if (h->op.nseg == 2) A(&h->pack_scratch, static_cast<size_t>(D.layers) * 6);
   A(&h->embed, static_cast<size_t>(D.vocab) * d);
   if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA) A(&h->pos, static_cast<size_t>(D.max_positions + 2) * d);
@@ -983,22 +1029,40 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     unsigned int* f8_scratch = h->op.nseg == 2 ? h->pack_scratch + (h->pack_used++ % (D.layers * 6)) : nullptr;
     pack_weights(group, N, K, conv1d ? 1 : K, conv1d ? N : 1, np, f8_scratch, dst, inv, 0);
   };
-  // "rotary.cos" / "rotary.sin" [T, 32] (ESM C, RITA: heads of 64) -> the device tables of the rotary GEMM epilogue
+  // "rotary.cos" / "rotary.sin" [T, S/2] (ESM C, RITA: [T, 32]; ProGen2: half its slot width) -> the tables of the rotary GEMM epilogue
   auto rotary32 = [&]() -> int {
+    const int hs = h->op.slot / 2;
     auto it = by_name.find("rotary.cos");
     auto is = by_name.find("rotary.sin");
-    if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != 32 || is->second->shape[1] != 32 ||
+    if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != hs || is->second->shape[1] != hs ||
         is->second->shape[0] != it->second->shape[0]) {
-      missing += "rotary.cos/rotary.sin[T,32] ";
+      missing += "rotary.cos/rotary.sin[T," + std::to_string(hs) + "] ";
       return PG_OK;
     }
     h->rot_rows = static_cast<int>(it->second->shape[0]);
-    int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
-    if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
+    int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * hs);
+    if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * hs);
     if (rc) return rc;
-    copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * 32);
-    copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * 32);
+    copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * hs);
+    copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * hs);
     return PG_OK;
+  };
+  const int hd = d / D.heads;
+  // A [n_src, k_src] source weight placed in the padded operand layout [N, K] (OpFmt, slot maps rmap / cmap), in a scratch buffer
+  // freed on return; the source itself when the layout is unpadded. The ProGen2 maps read rows of the fused [3d, d] qkv_proj.
+  auto slots = [&](const float* w, int n_src, int k_src, int N, int K, int rmap, int cmap) -> const float* {
+    if (!w || (N == n_src && K == k_src)) return w;
+    float* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, static_cast<size_t>(N) * K * sizeof(float));
+    if (e != cudaSuccess) {
+      if (!exp_err) exp_err = e;
+      return nullptr;
+    }
+    expanded.p.push_back(p);
+    const long long tot = static_cast<long long>(N) * K;
+    const int rn = rmap >= SL_PGQ ? n_src / 3 : n_src;
+    expand_slots_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(w, rn, k_src, p, N, K, rmap, cmap, hd, h->op.slot, k_src);
+    return p;
   };
   if (D.arch == PG_ARCH_TRANCEPTION) {
     // HF GPT2-style names with the "transformer." prefix stripped by the host
@@ -1093,25 +1157,40 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     else copy(h->outw, get("embedding.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
     if (int rc = rotary32()) return rc;
     if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
+  } else if (D.arch == PG_ARCH_PROGEN2) {
+    // HF names without the "transformer." prefix (modeling_progen.py:84-95, 209-226, 389-401, 541-548). qkv_proj [3d, d] is placed
+    // into the head slots by SL_PGQ / SL_PGK / SL_PGV (one GEMM operand, no bias) with head_dim^-1/2 folded into the q rows: exact
+    // for head_dim 64, one fp32 rounding for 80 and 96. out_proj's columns take the SL_HEAD slots. The head is rows 5..29 of
+    // lm_head (weight and bias): the reference's log-softmax runs over exactly those columns (compute_fitness.py:71-77).
+    const int da = h->op.da;
+    const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(hd)));
+    for (int l = 0; l < D.layers; ++l) {
+      Layer& L = h->layers[l];
+      const std::string p = "h." + std::to_string(l) + ".";
+      const float* wqkv = get(p + "attn.qkv_proj.weight", 3 * d, d);
+      pack(L.wqkv, L.iqkv, {{slots(wqkv, 3 * d, d, da, d, SL_PGQ, SL_PAD), qscale}, slots(wqkv, 3 * d, d, da, d, SL_PGK, SL_PAD),
+                            slots(wqkv, 3 * d, d, da, d, SL_PGV, SL_PAD)}, da, d);
+      pack(L.wo, L.io, {slots(get(p + "attn.out_proj.weight", d, d), d, d, d, da, SL_PAD, SL_HEAD)}, d, da);
+      copy(L.ln1g, get(p + "ln_1.weight", d, 1), d);
+      copy(L.ln1b, get(p + "ln_1.bias", d, 1), d);
+      pack(L.w1, L.i1, {get(p + "mlp.fc_in.weight", f, d)}, f, d);
+      copy(L.b1, get(p + "mlp.fc_in.bias", f, 1), f);
+      pack(L.w2, L.i2, {get(p + "mlp.fc_out.weight", d, f)}, d, f);
+      copy(L.b2, get(p + "mlp.fc_out.bias", d, 1), d);
+    }
+    copy(h->embed, get("wte.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    copy(h->lnag, get("ln_f.weight", d, 1), d);
+    copy(h->lnab, get("ln_f.bias", d, 1), d);
+    const float* hw = get("lm_head.weight", D.vocab, d);
+    const float* hb = get("lm_head.bias", D.vocab, 1);
+    copy(h->outw, hw ? hw + static_cast<size_t>(h->label_off) * d : nullptr, static_cast<size_t>(h->head_vocab) * d);
+    copy(h->hbias, hb ? hb + h->label_off : nullptr, h->head_vocab);
+    if (int rc = rotary32()) return rc;
+    if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
   } else {
-    const int hd = d / D.heads, dk = h->op.dk, da = h->op.da;
+    const int dk = h->op.dk, da = h->op.da;
     // head_dim^-1/2 (multihead_attention.py:103,261), folded into the fp32 q weights and bias: 0.125 (exact) for head_dim 64
     const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(hd)));
-    // A [n_src, k_src] source weight placed in the padded operand layout [N, K] (OpFmt, slot maps rmap / cmap), in a scratch buffer
-    // freed on return; the source itself when the layout is unpadded.
-    auto slots = [&](const float* w, int n_src, int k_src, int N, int K, int rmap, int cmap) -> const float* {
-      if (!w || (N == n_src && K == k_src)) return w;
-      float* p = nullptr;
-      const cudaError_t e = cudaMalloc(&p, static_cast<size_t>(N) * K * sizeof(float));
-      if (e != cudaSuccess) {
-        if (!exp_err) exp_err = e;
-        return nullptr;
-      }
-      expanded.p.push_back(p);
-      const long long tot = static_cast<long long>(N) * K;
-      expand_slots_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(w, n_src, k_src, p, N, K, rmap, cmap, hd);
-      return p;
-    };
     // one attention block: q/k/v/out projections at `pa` ("...self_attn." / "...row_self_attention.layer."), its LayerNorm at `pl`
     auto load_attn = [&](Layer& L, const std::string& pa, const std::string& pl) {
       // q, k, v form ONE GEMM operand: one common e4m3 scale (matrix maximum over the three, q already scaled)
@@ -1184,7 +1263,7 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
         if (rc) return rc;
         for (auto [dst, src] : {std::make_pair(h->rot_cos, it->second->data), std::make_pair(h->rot_sin, is->second->data)})
           expand_slots_kernel<<<(h->rot_rows * 32 + 255) / 256, 256>>>(static_cast<const float*>(src), h->rot_rows, static_cast<int>(rw), dst,
-                                                                       h->rot_rows, 32, SL_PAD, SL_PAD, hd);
+                                                                       h->rot_rows, 32, SL_PAD, SL_PAD, hd, 64, static_cast<int>(rw));
       }
     }
   }
@@ -1200,8 +1279,7 @@ int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, co
                         const int32_t* out_row, int32_t P, int32_t T, float* out_logprobs, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_masked_marginals: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_masked_marginals: weights not loaded");
-  if (h->desc.arch == PG_ARCH_TRANCEPTION || h->desc.arch == PG_ARCH_RITA)
-    return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is an autoregressive model (use pg_ar_loglik)");
+  if (is_ar(h->desc.arch)) return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is an autoregressive model (use pg_ar_loglik)");
   if (h->desc.arch == PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is an MSA Transformer (use pg_msa_masked_marginals)");
   if (!tokens || !positions || !out_logprobs) return fail(h, PG_ERR_ARG, "pg_masked_marginals: null buffer");
   if (P < 0 || T <= 0 || T > n_tokens) return fail(h, PG_ERR_ARG, "pg_masked_marginals: bad P/T");
@@ -1265,8 +1343,7 @@ int pg_forward_logprobs(pg_handle h, const int32_t* tokens, int32_t n_tokens, in
                         float* out_logprobs, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_forward_logprobs: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: weights not loaded");
-  if (h->desc.arch == PG_ARCH_TRANCEPTION || h->desc.arch == PG_ARCH_RITA)
-    return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an autoregressive model (use pg_ar_loglik)");
+  if (is_ar(h->desc.arch)) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an autoregressive model (use pg_ar_loglik)");
   if (h->desc.arch == PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an MSA Transformer (use pg_msa_masked_marginals)");
   if (!tokens || !out_logprobs || T <= 0 || win_start < 0 || win_start + T > n_tokens) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: bad arguments");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than the learned position table");
@@ -1299,6 +1376,8 @@ static int ar_fusion_args(pg_handle h, const pg_ar_fusion* f, ArFusion* base) {
   if (f->first_col < 0 || f->first_col > h->desc.vocab) return fail(h, PG_ERR_ARG, "pg_ar_loglik: first_col outside the vocabulary");
   if (h->desc.arch == PG_ARCH_RITA && (f->log_prior || f->log_prior2))
     return fail(h, PG_ERR_ARG, "pg_ar_loglik: RITA has no retrieval fusion (pass no log_prior / log_prior2)");
+  if (h->desc.arch == PG_ARCH_PROGEN2 && (f->log_prior || f->log_prior2))
+    return fail(h, PG_ERR_ARG, "pg_ar_loglik: ProGen2 has no retrieval fusion (pass no log_prior / log_prior2)");
   base->log_prior = f->log_prior; base->prior_row = f->prior_row; base->alpha = f->alpha;
   base->log_prior2 = f->log_prior2; base->prior_row2 = f->prior_row2; base->beta = f->beta;
   base->first_col = f->first_col; base->out_logprobs = f->out_logprobs;
@@ -1309,8 +1388,7 @@ int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int
                        float* out_sum_logp, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_ar_loglik: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_loglik: weights not loaded");
-  if (h->desc.arch != PG_ARCH_TRANCEPTION && h->desc.arch != PG_ARCH_RITA)
-    return fail(h, PG_ERR_STATE, "pg_ar_loglik: handle is not an autoregressive model (Tranception, RITA)");
+  if (!is_ar(h->desc.arch)) return fail(h, PG_ERR_STATE, "pg_ar_loglik: handle is not an autoregressive model (Tranception, RITA, ProGen2)");
   if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_ar_loglik: bad B/T");
   if (B == 0) return PG_OK;
   if (!ids || !lens || !out_sum_logp) return fail(h, PG_ERR_ARG, "pg_ar_loglik: null buffer");
@@ -1325,8 +1403,8 @@ int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int
 int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_fusion* f, float* out_tok_logp, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_ar_prefix_begin: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: weights not loaded");
-  if (h->desc.arch != PG_ARCH_TRANCEPTION && h->desc.arch != PG_ARCH_RITA)
-    return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: handle is not an autoregressive model (Tranception, RITA)");
+  if (!is_ar(h->desc.arch))
+    return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: handle is not an autoregressive model (Tranception, RITA, ProGen2)");
   if (!ids || !out_tok_logp || T < 2) return fail(h, PG_ERR_ARG, "pg_ar_prefix_begin: bad arguments");
   if (T > h->desc.max_positions || T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_ar_prefix_begin: sequence longer than n_ctx / workspace");
   ArFusion fu;
@@ -1335,7 +1413,7 @@ int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_f
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t ldq = static_cast<size_t>(h->op.ldq);
-  if (h->prefix_cap < h->desc.max_positions) {  // first use: [layers][n_ctx][3d*np] fp16, twice (RITA: once, no conv look-back)
+  if (h->prefix_cap < h->desc.max_positions) {  // first use: [layers][n_ctx][3da*np] fp16, twice (RITA, ProGen2: once, no conv look-back)
     const size_t n = static_cast<size_t>(h->desc.layers) * h->desc.max_positions * ldq;
     rc = h->desc.arch == PG_ARCH_TRANCEPTION ? dev_alloc(h, &h->raw_cache, n) : PG_OK;
     if (!rc) rc = dev_alloc(h, &h->kv_cache, n);
@@ -1349,8 +1427,7 @@ int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_f
   int32_t* len_dev = h->row_sel;
   PG_CUDA_OK(cudaMemcpyAsync(len_dev, &T, sizeof(int32_t), cudaMemcpyHostToDevice, s));
   { ProfScope ps(CAT_HEAD, s, 2);
-    rc = launch_ar_head(h->x, h->desc.embed_dim, 1, T, h->desc.vocab, ids, len_dev, h->lnag, h->lnab, h->outw ? h->outw : h->embed, fu,
-                        out_tok_logp, h->tok_logp, s); }
+    rc = ar_head(h, ids, len_dev, 1, T, fu, out_tok_logp, h->tok_logp, s); }
   if (rc) return fail(h, rc, tls_error());
   h->prefix_T = T;
   return PG_OK;
@@ -1360,8 +1437,8 @@ int pg_ar_loglik_prefix(pg_handle h, const int32_t* ids, const int32_t* lens, in
                         float* out_sum_logp, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_ar_loglik_prefix: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: weights not loaded");
-  if (h->desc.arch != PG_ARCH_TRANCEPTION && h->desc.arch != PG_ARCH_RITA)
-    return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: handle is not an autoregressive model (Tranception, RITA)");
+  if (!is_ar(h->desc.arch))
+    return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: handle is not an autoregressive model (Tranception, RITA, ProGen2)");
   if (h->prefix_T <= 0) return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: no wild-type prefix recorded (call pg_ar_prefix_begin first)");
   if (start <= 0 || start % 128 || start >= h->prefix_T) return fail(h, PG_ERR_ARG, "pg_ar_loglik_prefix: start must be a positive multiple of 128 below the recorded length");
   if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_ar_loglik_prefix: bad B/T");

@@ -1,11 +1,14 @@
-// K4 — wgmma/TMA attention, head_dim 64: one warpgroup per CTA, 64-query tiles x 64-key blocks, flash-style online softmax.
-// Optional causal + ALiBi + shared (wild-type) key/value prefix; NP = 2 runs the hi/lo three-product scheme.
+// K4 — wgmma/TMA attention, head width HD = 64 or 128: one warpgroup per CTA, 64-query tiles x 64-key blocks, flash-style online
+// softmax. Optional causal + ALiBi + shared (wild-type) key/value prefix; NP = 2 runs the hi/lo three-product scheme.
 //
 // Per key block: S = Q K^T (wgmma, both operands from shared memory) -> online softmax on the register fragment -> O += P V (wgmma,
 // P from registers: the S accumulator fragment of 16 keys is exactly the A fragment of one k16 step, so P never touches shared
 // memory). K and V arrive by TMA into a two-slot ring (the next block loads while this one computes); several CTAs share an SM
 // (NP = 2: 81 KB of shared memory each), so one CTA's softmax overlaps another's MMAs.
 //   Work item = (sequence, head, 64-query tile); grid = items, tiles of one (sequence, head) adjacent so that K / V stay in L2.
+// HD = 128 (ProGen2's 80- and 96-wide heads in 128-wide slots, api.cu): each of q, k and v is NB = 2 boxes of 64 columns (the TMA
+// box stays at 128 B rows, SWIZZLE_128B); S = Q K^T runs 4 k16 steps per box, O += P V one n64 wgmma group per box into o[32 * NB].
+// NP = 2 then needs ~160 KB of shared memory: one CTA per SM. The delta-operand and column (perm_C) forms are HD = 64 only.
 #include <cstdlib>
 
 #include "common.h"
@@ -20,11 +23,12 @@ constexpr uint32_t TILE = 8192;  // 64 rows x 64 fp16
 constexpr int NSLOT = 2;         // K/V smem ring
 constexpr int ATT_THREADS = 128;
 
-template <int NP>
+template <int NP, int HD>
 struct SmemW {
-  static constexpr uint32_t Q = 0;                     // [NP] tiles
-  static constexpr uint32_t KV = NP * TILE;            // [NSLOT][K planes NP | V planes NP]
-  static constexpr uint32_t BAR = KV + NSLOT * 2 * NP * TILE;
+  static constexpr int NB = HD / 64;                   // 64-column boxes per head
+  static constexpr uint32_t Q = 0;                     // [NP][NB] tiles
+  static constexpr uint32_t KV = NP * NB * TILE;       // [NSLOT][K planes NP x NB | V planes NP x NB]
+  static constexpr uint32_t BAR = KV + NSLOT * 2 * NP * NB * TILE;
   static constexpr uint32_t TOTAL = BAR + 64 + 1024;   // barriers, alignment slack
 };
 
@@ -48,13 +52,15 @@ __device__ __forceinline__ float ex2a(float x) {
   return y;
 }
 
-template <int NP, int DELTA>
+template <int NP, int DELTA, int HD>
 __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tm,
                                                                  const __grid_constant__ CUtensorMap tmP, const AttnWParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (base & 1023u)) & 1023u);
-  using L = SmemW<NP>;
+  using L = SmemW<NP, HD>;
+  constexpr int NB = L::NB;
+  constexpr uint32_t PLANE = NB * TILE;  // one plane of one head: NB boxes
   uint8_t* sQ = smem + L::Q;
   uint8_t* sKV = smem + L::KV;
   uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::BAR);
@@ -67,19 +73,20 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
   const int qt = qt_l + p.s_blocks;  // tile index within the full sequence
   const int h = bh % p.heads, b = bh / p.heads;
   const int row0 = b * p.Tq;
-  const int cq = h * 64, ck = p.d + h * 64, cv = 2 * p.d + h * 64;
+  const int cq = h * HD, ck = p.d + h * HD, cv = 2 * p.d + h * HD;
   const int nkb = p.causal ? min(qt + 1, p.nkb) : p.nkb;  // causal: query tile qt needs key blocks 0 .. qt
 
   auto load_block = [&](int j) {  // K and V of key block j of the full sequence: shared prefix rows or this sequence's own rows
     const int slot = j % NSLOT;
-    mbar_arrive_expect_tx(&kv_full[slot], 2 * NP * TILE);
+    mbar_arrive_expect_tx(&kv_full[slot], 2 * NP * PLANE);
     const CUtensorMap* src = j < p.s_blocks ? &tmP : &tm;
     const int r = j < p.s_blocks ? j * KT : row0 + (j - p.s_blocks) * KT;
-    uint8_t* dst = sKV + slot * 2 * NP * TILE;
-    for (int pl = 0; pl < NP; ++pl) {
-      tma_load_2d(dst + pl * TILE, src, &kv_full[slot], ck + pl * static_cast<int>(p.lo_off), r);
-      tma_load_2d(dst + (NP + pl) * TILE, src, &kv_full[slot], cv + pl * static_cast<int>(p.lo_off), r);
-    }
+    uint8_t* dst = sKV + slot * 2 * NP * PLANE;
+    for (int pl = 0; pl < NP; ++pl)
+      for (int bx = 0; bx < NB; ++bx) {
+        tma_load_2d(dst + pl * PLANE + bx * TILE, src, &kv_full[slot], ck + 64 * bx + pl * static_cast<int>(p.lo_off), r);
+        tma_load_2d(dst + (NP + pl) * PLANE + bx * TILE, src, &kv_full[slot], cv + 64 * bx + pl * static_cast<int>(p.lo_off), r);
+      }
   };
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -87,8 +94,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
     mbar_init(q_full, 1);
     for (int i = 0; i < NSLOT; ++i) mbar_init(&kv_full[i], 1);
     fence_mbar_init();
-    mbar_arrive_expect_tx(q_full, NP * TILE);
-    for (int pl = 0; pl < NP; ++pl) tma_load_2d(sQ + pl * TILE, &tmQ, q_full, cq + pl * static_cast<int>(p.lo_off), row0 + qt_l * QT);
+    mbar_arrive_expect_tx(q_full, NP * PLANE);
+    for (int pl = 0; pl < NP; ++pl)
+      for (int bx = 0; bx < NB; ++bx)
+        tma_load_2d(sQ + pl * PLANE + bx * TILE, &tmQ, q_full, cq + 64 * bx + pl * static_cast<int>(p.lo_off), row0 + qt_l * QT);
     for (int j = 0; j < NSLOT && j < nkb; ++j) load_block(j);
   }
   __syncthreads();
@@ -97,9 +106,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
   constexpr float LOG2E = 1.4426950408889634f;
   const float slope2 = slope * LOG2E;
   const int qrow = qt * QT + warp * 16 + g;  // this thread's rows qrow and qrow + 8 (full-sequence index)
-  float o[32];
+  float o[NB][32];  // o[bx]: head-dim columns [64 bx, 64 bx + 64)
 #pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  for (int bx = 0; bx < NB; ++bx)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[bx][i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const uint32_t q_addr = smem_u32(sQ);
   mbar_wait(q_full, 0);
@@ -107,18 +118,27 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
   for (int j = 0; j < nkb; ++j) {
     const int slot = j % NSLOT;
     mbar_wait(&kv_full[slot], (j / NSLOT) & 1);
-    const uint32_t k_addr = smem_u32(sKV) + slot * 2 * NP * TILE;
-    const uint32_t v_addr = k_addr + NP * TILE;
-    // ---- S = Q K^T (64 x 64), hi*hi [+ lo*hi + hi*lo] ----
+    const uint32_t k_addr = smem_u32(sKV) + slot * 2 * NP * PLANE;
+    const uint32_t v_addr = k_addr + NP * PLANE;
+    // ---- S = Q K^T (64 x 64), hi*hi [+ lo*hi + hi*lo]; 4 k16 steps per 64-column box ----
     float s[32];
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_m64n64k16_f16_ss(s, make_desc_sw128(q_addr) + 2 * k, make_desc_sw128(k_addr) + 2 * k, k > 0 ? 1u : 0u);
+    for (int k = 0; k < 4 * NB; ++k) {
+      const uint32_t bo = (k >> 2) * TILE;
+      wgmma_m64n64k16_f16_ss(s, make_desc_sw128(q_addr + bo) + 2 * (k & 3), make_desc_sw128(k_addr + bo) + 2 * (k & 3), k > 0 ? 1u : 0u);
+    }
     if (NP == 2) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_m64n64k16_f16_ss(s, make_desc_sw128(q_addr + TILE) + 2 * k, make_desc_sw128(k_addr) + 2 * k, 1u);
+      for (int k = 0; k < 4 * NB; ++k) {
+        const uint32_t bo = (k >> 2) * TILE;
+        wgmma_m64n64k16_f16_ss(s, make_desc_sw128(q_addr + PLANE + bo) + 2 * (k & 3), make_desc_sw128(k_addr + bo) + 2 * (k & 3), 1u);
+      }
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_m64n64k16_f16_ss(s, make_desc_sw128(q_addr) + 2 * k, make_desc_sw128(k_addr + TILE) + 2 * k, 1u);
+      for (int k = 0; k < 4 * NB; ++k) {
+        const uint32_t bo = (k >> 2) * TILE;
+        wgmma_m64n64k16_f16_ss(s, make_desc_sw128(q_addr + bo) + 2 * (k & 3), make_desc_sw128(k_addr + PLANE + bo) + 2 * (k & 3), 1u);
+      }
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -149,7 +169,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
       l[r] *= alpha[r];
     }
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    for (int bx = 0; bx < NB; ++bx)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[bx][i] *= alpha[(i >> 1) & 1];
     // ---- P = 2^(s - m) as fp16 hi [+ lo] A fragments, O += P V ----
     uint32_t ph[4][4], pl[4][4];
 #pragma unroll
@@ -168,19 +190,24 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
       }
     }
     wgmma_fence();
-    wgmma_fence_regs(o);
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const uint64_t vh = make_desc_sw128(v_addr + kk * 2048);  // 16 key rows of 128 B per k-step
-      wgmma_m64n64k16_f16_rs_tb(o, ph[kk], vh, 1u);
-      if (NP == 2) {
-        wgmma_m64n64k16_f16_rs_tb(o, pl[kk], vh, 1u);
-        wgmma_m64n64k16_f16_rs_tb(o, ph[kk], make_desc_sw128(v_addr + TILE + kk * 2048), 1u);
+    for (int bx = 0; bx < NB; ++bx) wgmma_fence_regs(o[bx]);
+#pragma unroll
+    for (int bx = 0; bx < NB; ++bx) {
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t vh = make_desc_sw128(v_addr + bx * TILE + kk * 2048);  // 16 key rows of 128 B per k-step
+        wgmma_m64n64k16_f16_rs_tb(o[bx], ph[kk], vh, 1u);
+        if (NP == 2) {
+          wgmma_m64n64k16_f16_rs_tb(o[bx], pl[kk], vh, 1u);
+          wgmma_m64n64k16_f16_rs_tb(o[bx], ph[kk], make_desc_sw128(v_addr + PLANE + bx * TILE + kk * 2048), 1u);
+        }
       }
     }
     wgmma_commit();
     wgmma_wait<0>();
-    wgmma_fence_regs(o);
+#pragma unroll
+    for (int bx = 0; bx < NB; ++bx) wgmma_fence_regs(o[bx]);
     __syncthreads();  // every warp is done with this slot
     if (threadIdx.x == 0 && j + NSLOT < nkb) load_block(j + NSLOT);
   }
@@ -196,18 +223,18 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
     long long orow_idx = static_cast<long long>(b) * p.Tq + (qidx - p.s_blocks * KT);
     if (p.perm_C > 0) orow_idx = (static_cast<long long>(b / p.perm_C) * p.Tq + qidx) * p.perm_C + b % p.perm_C;
     // operand.cuh's column-pair store written out, for the same reason as in the GEMM epilogue (gemm_tc.cu)
-    __half* orow = p.out + orow_idx * p.ldo + h * 64;
-    uint8_t* f8 = reinterpret_cast<uint8_t*>(p.out + orow_idx * p.ldo + p.out_lo_off) + h * 64;
+    __half* orow = p.out + orow_idx * p.ldo + h * HD;
+    uint8_t* f8 = reinterpret_cast<uint8_t*>(p.out + orow_idx * p.ldo + p.out_lo_off) + h * HD;
     const float sh = p.out_scale, sl = p.out_scale * LO8_GAIN;
     // delta-operand mode (DELTA): this row's exact value also goes to cout[b] when it is the masked row; base row to subtract
     const bool crow = DELTA && p.mask_pos != nullptr && qidx == __ldg(p.mask_pos + b);
-    const __half* brow = (DELTA && p.base_o != nullptr) ? p.base_o + static_cast<long long>(qidx) * p.d + h * 64 : nullptr;
+    const __half* brow = (DELTA && p.base_o != nullptr) ? p.base_o + static_cast<long long>(qidx) * p.d + h * HD : nullptr;
 #pragma unroll
-    for (int n = 0; n < 8; ++n) {
+    for (int n = 0; n < 8 * NB; ++n) {
       const int col = 8 * n + 2 * t;
-      float x0 = o[4 * n + 2 * r] * rl, x1 = o[4 * n + 2 * r + 1] * rl;
+      float x0 = o[n >> 3][4 * (n & 7) + 2 * r] * rl, x1 = o[n >> 3][4 * (n & 7) + 2 * r + 1] * rl;
       if (DELTA && crow) {  // rare (one row per sequence and head): fp16 hi / lo pair of the full value
-        __half* cr = p.cout + static_cast<long long>(b) * p.ldc + h * 64 + col;
+        __half* cr = p.cout + static_cast<long long>(b) * p.ldc + h * HD + col;
         const uint32_t ch = cvt_f16x2_rn_inf(x0, x1);
         const float2 cf = unpack_h2(ch);
         *reinterpret_cast<uint32_t*>(cr) = ch;
@@ -241,8 +268,12 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
   if (a.q_begin != 0) return set_error(PG_ERR_ARG, "attention_wgmma: q_begin is only supported by the mma.sync kernel");
   if (a.prefix && (!a.causal || a.prefix_len <= 0 || a.prefix_len % 128))
     return set_error(PG_ERR_ARG, "attention_wgmma: a shared prefix needs causal attention and a length that is a multiple of 128");
+  if (a.head_dim != 64 && a.head_dim != 128) return set_error(PG_ERR_ARG, "attention_wgmma: head width must be 64 or 128");
+  const int HDw = a.head_dim;
+  if (HDw == 128 && (a.base_o || a.mask_pos || a.perm_C))
+    return set_error(PG_ERR_UNSUPPORTED, "attention_wgmma: the delta-operand and column-attention forms run on 64-wide heads only");
   AttnWParams p{};
-  p.B = a.B; p.heads = a.heads; p.d = a.heads * 64;
+  p.B = a.B; p.heads = a.heads; p.d = a.heads * HDw;
   p.Tq = a.T; p.s_blocks = a.prefix ? a.prefix_len / KT : 0;
   p.T = a.T + p.s_blocks * KT;
   p.nqt = (a.T + QT - 1) / QT; p.nkb = (p.T + KT - 1) / KT;
@@ -276,16 +307,20 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
   PG_CUDA_OK(cudaGetDevice(&dev));
   static bool attr_set[64] = {};
   if (dev < 64 && !attr_set[dev]) {
-    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<1>::TOTAL));
-    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2>::TOTAL));
-    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2>::TOTAL));
+    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<1, 0, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<1, 64>::TOTAL));
+    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 0, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2, 64>::TOTAL));
+    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2, 64>::TOTAL));
+    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<1, 0, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<1, 128>::TOTAL));
+    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 0, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2, 128>::TOTAL));
     attr_set[dev] = true;
   }
   const bool delta = a.base_o != nullptr || a.mask_pos != nullptr;
   if (delta && np != 2) return set_error(PG_ERR_UNSUPPORTED, "attention_wgmma: the delta-operand form runs on fp16 hi/lo operands (nseg 3)");
-  if (delta) attn_wgmma_kernel<2, 1><<<grid, ATT_THREADS, SmemW<2>::TOTAL, s>>>(tmQ, tm, tmP, p);
-  else if (np == 1) attn_wgmma_kernel<1, 0><<<grid, ATT_THREADS, SmemW<1>::TOTAL, s>>>(tmQ, tm, tmP, p);
-  else attn_wgmma_kernel<2, 0><<<grid, ATT_THREADS, SmemW<2>::TOTAL, s>>>(tmQ, tm, tmP, p);
+  if (delta) attn_wgmma_kernel<2, 1, 64><<<grid, ATT_THREADS, SmemW<2, 64>::TOTAL, s>>>(tmQ, tm, tmP, p);
+  else if (HDw == 128 && np == 1) attn_wgmma_kernel<1, 0, 128><<<grid, ATT_THREADS, SmemW<1, 128>::TOTAL, s>>>(tmQ, tm, tmP, p);
+  else if (HDw == 128) attn_wgmma_kernel<2, 0, 128><<<grid, ATT_THREADS, SmemW<2, 128>::TOTAL, s>>>(tmQ, tm, tmP, p);
+  else if (np == 1) attn_wgmma_kernel<1, 0, 64><<<grid, ATT_THREADS, SmemW<1, 64>::TOTAL, s>>>(tmQ, tm, tmP, p);
+  else attn_wgmma_kernel<2, 0, 64><<<grid, ATT_THREADS, SmemW<2, 64>::TOTAL, s>>>(tmQ, tm, tmP, p);
   PG_CUDA_OK(cudaGetLastError());
   return PG_OK;
 }

@@ -55,6 +55,7 @@ struct GemmLaunch {
   __half* out; int64_t ldo; int64_t out_lo_off;
   float* resid; int64_t ldr;
   const float* rot_cos; const float* rot_sin; int rot_T; int rot_dim;
+  int rot_half = 32;              // epi 3: half the head slot; 64 = 128-wide slots, tables [T, 64] (internal: pg_gemm keeps 32)
   float a_scale = 0.f;            // nseg 2: s used by the producer of a's e4m3 planes
   const float* w_inv = nullptr;   // nseg 2: [N] 1 / t_n of the weight rows
   int w_uniform = 0;              // nseg 2: all w_inv[n] are equal (one scale per matrix, as pg_load_weights / pg_pack_weight produce)
@@ -105,6 +106,8 @@ struct AttnLaunch {
   // Delta-operand mode: base_o (fp16 [T, heads*64]) is subtracted from every output row t before rounding (out = attention - base);
   // the full-precision value of row mask_pos[b] of sequence b is additionally written as an fp16 hi / lo pair to row b of `cout`.
   const __half* base_o = nullptr; const int32_t* mask_pos = nullptr; __half* cout = nullptr; int64_t ldc = 0; int64_t c_lo_off = 0;
+  // Width of a head's q / k / v / output slot (wgmma kernel): 64, or 128 for the 128-wide slots of ProGen2's 80- and 96-wide heads.
+  int head_dim = 64;
 };
 int launch_attention(const AttnLaunch& a, cudaStream_t s);
 
@@ -172,8 +175,10 @@ struct ArFusion {
   int first_col = 0;
   float* out_logprobs = nullptr;
 };
+// wte: the head [vocab, d]; bias: [vocab] or null; the label of token id v is head column v - label_off.
 int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t* ids, const int32_t* lens, const float* lnf_g,
-                   const float* lnf_b, const float* wte, const ArFusion& fusion, float* tok_logp, float* out_sum, cudaStream_t s);
+                   const float* lnf_b, const float* wte, const float* bias, int label_off, const ArFusion& fusion, float* tok_logp,
+                   float* out_sum, cudaStream_t s);
 }  // namespace pg
 
 namespace pg {

@@ -67,6 +67,7 @@ struct GemmKParams {
   int out_fmt;            // 0 fp16 hi; 1 fp16 hi + fp16 lo; 2 fp16 hi + e4m3 [lo8 | hi8] byte planes
   float out_scale;        // out_fmt 2: s of the consuming GEMM (hi8 = e4m3(hi*s), lo8 = e4m3(lo*2^11*s))
   const float* rot_cos; const float* rot_sin; int rot_T; int rot_dim;
+  int rot_half;           // 32: 64-wide head slots, tables [T, 32]; 64: 128-wide slots (one per N tile), tables [T, 64]
   int tiles_m, tiles_n;
   int prefetch;           // k-blocks of L2 look-ahead for the A operand (0 = off)
   // delta-operand mode (common.h GemmLaunch): shared base rows added before / subtracted after the activation, masked rows skipped
@@ -146,7 +147,23 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
         v1 = gelu_tanh(v1);
       }
     }
-    if (EPI == 3) {
+    if (EPI == 3 && p.rot_half == 64) {
+      // the same over one 128-wide slot per N tile: blocks j and j + 8 hold columns c and c + 64; cos/sin[t, c] for c in [0, 64)
+      const int t = static_cast<int>(row % p.rot_T);
+      if (col0 - (col0 & 127) < 2 * p.rot_dim) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = (col0 & 127) + 8 * j + e;
+            const float co = __ldg(p.rot_cos + static_cast<long long>(t) * 64 + c), s = __ldg(p.rot_sin + static_cast<long long>(t) * 64 + c);
+            const float a = acc[4 * j + 2 * h + e], b = acc[4 * (j + 8) + 2 * h + e];
+            acc[4 * j + 2 * h + e] = a * co - b * s;
+            acc[4 * (j + 8) + 2 * h + e] = b * co + a * s;
+          }
+        }
+      }
+    } else if (EPI == 3) {
       // rotary: x*cos + rotate_half(x)*sin over each 64-wide head (blocks j and j + 4 of one head hold columns c and c + 32);
       // cos/sin[t, c] for c in [0,32) (both halves equal)
       const int t = static_cast<int>(row % p.rot_T);
@@ -516,6 +533,8 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
     return set_error(PG_ERR_ARG, "gemm: the SwiGLU epilogue needs N % 16 == 0 (N/2 % 64 == 0 for out_fmt 2), no groups, planes >= N/2 apart");
   if (g.epi == 2 ? !g.resid : !g.out) return set_error(PG_ERR_ARG, "gemm: missing output");
   if (g.epi == 3 && (!g.rot_cos || !g.rot_sin || g.rot_T <= 0 || g.rot_dim % 64)) return set_error(PG_ERR_ARG, "gemm: bad rotary args");
+  if (g.epi == 3 && ((g.rot_half != 32 && g.rot_half != 64) || g.rot_dim % (2 * g.rot_half)))
+    return set_error(PG_ERR_ARG, "gemm: rotary slots must be 64 or 128 wide and divide rot_dim");
   if (g.nseg == 2 && (!g.w_inv || !(g.a_scale > 0.f))) return set_error(PG_ERR_ARG, "gemm: nseg 2 needs w_inv[N] and a_scale > 0");
   if (g.out_fmt < 0 || g.out_fmt > 2) return set_error(PG_ERR_ARG, "gemm: bad out_fmt");
   if ((g.base_pre || g.base_post || g.mask_pos) && (!g.base_pre || g.base_T <= 0 || g.N % 64 || g.M % g.base_T || g.grp_rows_a ||
@@ -593,7 +612,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   p.resid = g.resid; p.ldr = g.ldr;
   p.out_fmt = (g.epi == 2) ? 0 : g.out_fmt;
   p.out_scale = g.out_scale;
-  p.rot_cos = g.rot_cos; p.rot_sin = g.rot_sin; p.rot_T = g.rot_T; p.rot_dim = g.rot_dim;
+  p.rot_cos = g.rot_cos; p.rot_sin = g.rot_sin; p.rot_T = g.rot_T; p.rot_dim = g.rot_dim; p.rot_half = g.rot_half;
   p.tiles_m = cta2 ? (g.M + 2 * BM - 1) / (2 * BM) : (g.M + BM - 1) / BM;
   p.tiles_n = (g.N + BN - 1) / BN;
   p.prefetch = grouped ? 0 : gemm_prefetch();

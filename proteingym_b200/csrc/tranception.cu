@@ -2,7 +2,7 @@
 //   gather_embed_kernel   x[row] = wte[ids[row]]                                   (model_pytorch.py:526-532, no position table)
 //   qkv_conv_kernel       depthwise causal conv (k = 1,3,5,7 by head group) on q, k and v + the 1/sqrt(hd) query scale
 //                         (model_pytorch.py:73-88, :240-251, :158-159)
-//   ar_head_kernel        ln_f -> tied lm_head (no bias) -> log_softmax -> optional retrieval-prior fusion -> log p(next token)
+//   ar_head_kernel        ln_f -> lm_head (optional bias) -> log_softmax -> optional retrieval-prior fusion -> log p(next token)
 //                         (model_pytorch.py:612, :783, :806-830; utils/scoring_utils.py:121-128)
 //   seq_sum_kernel        per-sequence sum over the real (non-pad) predicted tokens, fixed order
 #include "common.h"
@@ -109,6 +109,8 @@ struct ArHeadParams {
   const float* x; int d; int T; int vocab;
   const int32_t* ids; const int32_t* lens;
   const float* lnf_g; const float* lnf_b; const float* wte;
+  const float* bias;  // [vocab] or null
+  int label_off;      // head column of token id v is v - label_off (ProGen2: the head holds vocabulary rows 5..29)
   ArFusion f;
   float* tok_logp;  // [B*T]
 };
@@ -130,7 +132,8 @@ __device__ __forceinline__ float fuse_logp(const ArFusion& f, int vocab, long lo
   return lp;
 }
 
-// One block (128 threads) per token row r = (b, t): log p(ids[b, t+1] | ids[b, <=t]); 0 for t >= len-1.
+// One block (128 threads) per token row r = (b, t): log p(ids[b, t+1] | ids[b, <=t]); 0 for t >= len-1, NaN for a next token outside
+// the head's columns.
 __global__ void ar_head_kernel(ArHeadParams p) {
   __shared__ float sh[33];
   extern __shared__ float dyn[];
@@ -148,14 +151,14 @@ __global__ void ar_head_kernel(ArHeadParams p) {
   block_ln_stats(xr, p.d, sh, mean, rstd);
   for (int j = threadIdx.x; j < p.d; j += blockDim.x) y[j] = (xr[j] - mean) * rstd * p.lnf_g[j] + p.lnf_b[j];
   __syncthreads();
-  const float lse = block_logits_lse(y, p.d, p.wte, nullptr, p.vocab, logits);
+  const float lse = block_logits_lse(y, p.d, p.wte, p.bias, p.vocab, logits);
   if (threadIdx.x < 32) {
     const int lane = threadIdx.x;
     if (p.f.out_logprobs)
       for (int v = lane; v < p.vocab; v += 32) p.f.out_logprobs[r * p.vocab + v] = fuse_logp(p.f, p.vocab, r, v, logits[v] - lse);
     if (lane == 0) {
-      const int label = p.ids[r + 1];
-      p.tok_logp[r] = fuse_logp(p.f, p.vocab, r, label, logits[label] - lse);
+      const int label = p.ids[r + 1] - p.label_off;
+      p.tok_logp[r] = (label < 0 || label >= p.vocab) ? NAN : fuse_logp(p.f, p.vocab, r, label, logits[label] - lse);
     }
   }
 }
@@ -206,9 +209,10 @@ int launch_qkv_conv(const __half* in, __half* out, int64_t ld, int64_t lo_off, i
 }
 
 int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t* ids, const int32_t* lens, const float* lnf_g,
-                   const float* lnf_b, const float* wte, const ArFusion& fusion, float* tok_logp, float* out_sum, cudaStream_t s) {
+                   const float* lnf_b, const float* wte, const float* bias, int label_off, const ArFusion& fusion, float* tok_logp,
+                   float* out_sum, cudaStream_t s) {
   if (B <= 0 || T <= 0) return PG_OK;
-  ArHeadParams p{x, d, T, vocab, ids, lens, lnf_g, lnf_b, wte, fusion, tok_logp};
+  ArHeadParams p{x, d, T, vocab, ids, lens, lnf_g, lnf_b, wte, bias, label_off, fusion, tok_logp};
   ar_head_kernel<<<static_cast<unsigned>(static_cast<long long>(B) * T), 128, (d + vocab) * sizeof(float), s>>>(p);
   seq_sum_kernel<<<(B + 3) / 4, 128, 0, s>>>(tok_logp, lens, B, T, out_sum);
   PG_CUDA_OK(cudaGetLastError());

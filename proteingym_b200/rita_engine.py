@@ -127,28 +127,23 @@ def plan(prots, wt: str | None = None, context: int = CONTEXT):
 PRECISIONS = {"f16": _lib.PG_PREC_F16, "f16x3": _lib.PG_PREC_F16X3, "f16f8": _lib.PG_PREC_F16F8}
 
 
-class RitaScorer:
+class ArScorer:
+    """A pg_ar_* handle on the GPU and the token-row machinery every autoregressive scorer shares: summed log-likelihoods of ragged
+    token rows, and wild-type prefix reuse for rows that share at least PREFIX_MIN_TOKEN leading tokens with a wild-type row. The head
+    of the handle scores ``head_vocab`` token ids from ``label_off`` on (RITA: all of them; ProGen2: ids 5..29)."""
     prefix_reuse = os.environ.get("PG_PREFIX_REUSE", "1") != "0"
     PREFIX_TILE = 128
     PREFIX_MIN_TOKEN = 128  # reuse a wild-type prefix when the first differing token is at least this far in
 
-    def __init__(self, conf: RitaConfig, state: dict, inv_freq: torch.Tensor, tokenizer: RitaTokenizer, precision: str = "f16f8",
-                 device: int = 0, max_rows: int = 0, context: int = CONTEXT):
+    def __init__(self, desc, tensors: dict, device: int = 0, head_vocab: int = 0, label_off: int = 0):
         if not torch.cuda.is_available():
             raise _lib.PgError("no CUDA device: the H100 scorer has no CPU fallback")
         self.lib = _lib.load()
         self.device = torch.device("cuda", device)
-        self.tok, self.context, self.conf = tokenizer, context, conf
-        self.max_T = context + tokenizer.n_special  # longest token row one chunk can give
-        desc = _lib.PgModelDesc(arch=_lib.PG_ARCH_RITA, layers=conf.layers, embed_dim=conf.embed_dim, heads=conf.heads, ffn_dim=conf.ffn_dim,
-                                vocab=conf.vocab, max_positions=self.max_T, token_dropout=0, emb_ln_before=0,
-                                precision=PRECISIONS[precision], device=device, max_rows=max_rows)
+        self.head_vocab, self.label_off = head_vocab or desc.vocab, label_off
         self.handle = C.c_void_p()
         _lib.check(self.lib.pg_create(C.byref(desc), C.byref(self.handle)))
         try:
-            cos, sin = rotary_tables(inv_freq, self.max_T)
-            tensors = dict(state)
-            tensors["rotary.cos"], tensors["rotary.sin"] = cos, sin
             gpu = [(n, t.to(self.device, torch.float32).contiguous()) for n, t in tensors.items()]
             arr = (_lib.PgTensor * len(gpu))()
             for i, (n, t) in enumerate(gpu):
@@ -210,7 +205,7 @@ class RitaScorer:
         T = len(ids)
         d_ids = torch.tensor(ids, dtype=torch.int32, device=self.device)
         d_tok = torch.zeros(T, dtype=torch.float32, device=self.device)
-        d_rows = torch.zeros((T, self.conf.vocab), dtype=torch.float32, device=self.device)
+        d_rows = torch.zeros((T, self.head_vocab), dtype=torch.float32, device=self.device)
         f = _lib.PgArFusion(out_logprobs=d_rows.data_ptr())
         _lib.check(self.lib.pg_ar_prefix_begin(self.handle, d_ids.data_ptr(), T, C.byref(f), d_tok.data_ptr(), self._stream()), self.handle)
         return d_tok.cpu().numpy(), d_rows.cpu().numpy()
@@ -274,9 +269,23 @@ class RitaScorer:
                 sfx = self.prefix_suffix_sums([toks[r] for r in members], start)
                 run += sum(len(toks[r]) - start for r in members)
                 for r, s in zip(members, sfx):
-                    out[r] = float(prefix_total(csum, wt_rows, start, toks[r][start], s))
+                    out[r] = float(prefix_total(csum, wt_rows, start, toks[r][start] - self.label_off, s))
         self.reuse_rows[1] += run
         return out
+
+
+class RitaScorer(ArScorer):
+    def __init__(self, conf: RitaConfig, state: dict, inv_freq: torch.Tensor, tokenizer: RitaTokenizer, precision: str = "f16f8",
+                 device: int = 0, max_rows: int = 0, context: int = CONTEXT):
+        self.tok, self.context, self.conf = tokenizer, context, conf
+        self.max_T = context + tokenizer.n_special  # longest token row one chunk can give
+        desc = _lib.PgModelDesc(arch=_lib.PG_ARCH_RITA, layers=conf.layers, embed_dim=conf.embed_dim, heads=conf.heads, ffn_dim=conf.ffn_dim,
+                                vocab=conf.vocab, max_positions=self.max_T, token_dropout=0, emb_ln_before=0,
+                                precision=PRECISIONS[precision], device=device, max_rows=max_rows)
+        cos, sin = rotary_tables(inv_freq, self.max_T)
+        tensors = dict(state)
+        tensors["rotary.cos"], tensors["rotary.sin"] = cos, sin
+        super().__init__(desc, tensors, device)
 
     def score(self, prots, wt: str | None = None) -> np.ndarray:
         """calc_fitness's score of every protein (float64): sum over (chunk, direction) of the mean target log-probability; NaN when a

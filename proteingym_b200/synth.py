@@ -612,3 +612,81 @@ def write_rita_tokenizer(folder: str, template: bool = False) -> str:
     with open(os.path.join(folder, "tokenizer_config.json"), "w") as fh:
         json.dump(dict(tokenizer_class="PreTrainedTokenizerFast", pad_token="<PAD>", eos_token="<EOS>", unk_token="<unk>"), fh, indent=1)
     return path
+
+
+# ---- ProGen2 (proteingym/baselines/progen2/models/progen/modeling_progen.py) --------------------------------------------------------
+@dataclass(frozen=True)
+class Progen2Arch:
+    layers: int
+    embed_dim: int
+    heads: int
+    rotary_dim: int | None
+    n_positions: int = 1024
+    n_inner: int | None = None
+    vocab: int = 32
+
+    @property
+    def head_dim(self) -> int:
+        return self.embed_dim // self.heads
+
+    @property
+    def ffn_dim(self) -> int:
+        return self.n_inner if self.n_inner is not None else 4 * self.embed_dim
+
+
+# Widths, head counts, layer counts, rotary_dim and n_positions as the released config.json files are commonly published (those files
+# are not reproduced here): small 151M, medium 764M (base: the same shape with n_positions 2048), large 2.7B. xlarge (4096 / 16 = 256-
+# wide heads) is refused by the library.
+PROGEN2_SMALL = Progen2Arch(12, 1024, 16, 32, 1024)
+PROGEN2_MEDIUM = Progen2Arch(27, 1536, 16, 48, 1024)
+PROGEN2_LARGE = Progen2Arch(32, 2560, 32, 64, 1024)
+
+
+def make_progen2_state(arch: Progen2Arch, seed: int = 0, buffers: bool = True) -> dict:
+    """ProGen2 state dict with the HF key names of ProGenForCausalLM (``transformer.`` prefix; with ``buffers`` the causal-mask buffers
+    ``attn.bias`` / ``attn.masked_bias`` that a saved state dict carries), drawn on the CPU from ``seed``: nn.Linear's U(+-1/sqrt(fan_in))
+    for the linear layers (qkv_proj and out_proj without bias), LayerNorm weights 1 + 0.1 N(0,1) and biases 0.1 N(0,1), the embedding
+    N(0, 1), and an lm_head of N(0, 4/d) rows with a 0.5 N(0,1) bias so that log-probabilities are a few nats apart."""
+    g = torch.Generator().manual_seed(seed)
+    d, f, V, n = arch.embed_dim, arch.ffn_dim, arch.vocab, arch.n_positions
+    ln_w = lambda: 1 + 0.1 * torch.randn(d, generator=g)
+    ln_b = lambda: 0.1 * torch.randn(d, generator=g)
+    st = {"transformer.wte.weight": torch.randn((V, d), generator=g)}
+    for i in range(arch.layers):
+        p = f"transformer.h.{i}."
+        st[p + "ln_1.weight"] = ln_w()
+        st[p + "ln_1.bias"] = ln_b()
+        if buffers:
+            st[p + "attn.bias"] = torch.tril(torch.ones((n, n), dtype=torch.bool)).view(1, 1, n, n)
+            st[p + "attn.masked_bias"] = torch.tensor(-1e9)
+        st[p + "attn.qkv_proj.weight"] = _uniform(g, (3 * d, d), 1 / math.sqrt(d))
+        st[p + "attn.out_proj.weight"] = _uniform(g, (d, d), 1 / math.sqrt(d))
+        st[p + "mlp.fc_in.weight"] = _uniform(g, (f, d), 1 / math.sqrt(d))
+        st[p + "mlp.fc_in.bias"] = _uniform(g, (f,), 1 / math.sqrt(d))
+        st[p + "mlp.fc_out.weight"] = _uniform(g, (d, f), 1 / math.sqrt(f))
+        st[p + "mlp.fc_out.bias"] = _uniform(g, (d,), 1 / math.sqrt(f))
+    st["transformer.ln_f.weight"] = ln_w()
+    st["transformer.ln_f.bias"] = ln_b()
+    st["lm_head.weight"] = (2 / math.sqrt(d)) * torch.randn((V, d), generator=g)
+    st["lm_head.bias"] = 0.5 * torch.randn(V, generator=g)
+    return st
+
+
+def write_progen2_checkpoint(folder: str, arch: Progen2Arch, seed: int = 0, state: dict | None = None, safetensors: bool = False,
+                             config_extra: dict | None = None) -> dict:
+    """A ProGen2 model directory: config.json (ProGenConfig's keys; ``rotary_dim`` null for full-head rotary) and pytorch_model.bin or
+    model.safetensors."""
+    os.makedirs(folder, exist_ok=True)
+    st = make_progen2_state(arch, seed, buffers=not safetensors) if state is None else state
+    cfg = dict(model_type="progen", vocab_size=arch.vocab, n_positions=arch.n_positions, n_ctx=arch.n_positions, n_embd=arch.embed_dim,
+               n_layer=arch.layers, n_head=arch.heads, rotary_dim=arch.rotary_dim, n_inner=arch.n_inner, activation_function="gelu_new",
+               resid_pdrop=0.0, embd_pdrop=0.0, attn_pdrop=0.0, layer_norm_epsilon=1e-5, bos_token_id=1, eos_token_id=2)
+    cfg.update(config_extra or {})
+    with open(os.path.join(folder, "config.json"), "w") as fh:
+        json.dump(cfg, fh, indent=1)
+    if safetensors:
+        from safetensors.torch import save_file
+        save_file({k: v.contiguous() for k, v in st.items()}, os.path.join(folder, "model.safetensors"))
+    else:
+        torch.save(st, os.path.join(folder, "pytorch_model.bin"))
+    return st

@@ -46,7 +46,7 @@ enum pg_arch {
                               "layers.{i}.mlp.{0,2}.*", "embedding.weight", "final_norm.*"), "lm_head.weight" [vocab, d] only for an
                               untied head (absent = the embedding), plus "rotary.cos" / "rotary.sin" [T, 32] = cos / sin(t * inv_freq[c])
                               from the checkpoint's rotary_embedding.inv_freq. */
-  PG_ARCH_PROGEN2 = 6      /* ProGen2 small / medium / base / large causal decoder (proteingym/baselines/progen2/models/progen/
+  PG_ARCH_PROGEN2 = 6,     /* ProGen2 small / medium / base / large causal decoder (proteingym/baselines/progen2/models/progen/
                               modeling_progen.py:60-282, 389-401, 541-548): parallel residual x + attn(ln_1(x)) + mlp(ln_1(x)), bias-free
                               fused qkv_proj in 8 [q | v | k] shards (heads % 8 == 0), interleaved (rotate_every_two) rotary on the first
                               rotary_dim dims of q and k, bias-free out_proj, tanh-GELU MLP (ffn_dim = n_inner or 4d) with biases, ln_f, and
@@ -61,6 +61,19 @@ enum pg_arch {
                               slot width: column i < rotary_dim / 2 holds cos / sin(t * 10000^(-2i / rotary_dim)) in fp32 as
                               fixed_pos_embedding computes it (rotary_dim = head_dim when the config has none), later columns cos = 1,
                               sin = 0. ln_1 / ln_f use eps 1e-5. */
+  PG_ARCH_PROTGPT2 = 7     /* ProtGPT2 = GPT-2 large causal decoder (proteingym/baselines/protgpt2/compute_fitness.py; transformers
+                              modeling_gpt2.py GPT2LMHeadModel): learned absolute positions (wpe) added to the token embedding, pre-LN blocks
+                              with c_attn / c_proj biases, causal attention without bias, tanh-GELU ("gelu_new") MLP (ffn_dim = n_inner or
+                              4d), ln_f, and the head tied to wte: a log-softmax over all `vocab` columns (50 257) that runs as one
+                              tensor-core GEMM whose epilogue keeps only per-tile (max, sum exp) partials (no logits are stored), in
+                              fp16 hi/lo x3 under PG_PREC_F16X3 and PG_PREC_F16F8 and single fp16 under PG_PREC_F16. head_dim 64 only;
+                              PG_PREC_F16D is refused. max_positions = the rows of wpe (n_positions); a row at position t of a call, or
+                              start + t after a recorded prefix, adds wpe[t] / wpe[start + t]. Scored through the pg_ar_* entry points
+                              without retrieval fusion; out_logprobs rows are `vocab` wide. Weights: the HF state-dict keys without
+                              "transformer." ("h.{i}.ln_{1,2}.*", "h.{i}.attn.c_attn.{weight [d, 3d], bias [3d]}", "h.{i}.attn.c_proj.*",
+                              "h.{i}.mlp.c_fc.{weight [d, ffn], bias}", "h.{i}.mlp.c_proj.{weight [ffn, d], bias}", "wte.weight" [vocab, d],
+                              "wpe.weight" [max_positions, d], "ln_f.*"): Conv1D weights are [in, out] as for PG_ARCH_TRANCEPTION, and
+                              no "lm_head.weight" (tied). LayerNorms use eps 1e-5. */
 };
 
 /* Tensor-core operand precision. The reference is strict fp32 (SURVEY.md §0.4). Every operand is an fp16 pair hi + lo.

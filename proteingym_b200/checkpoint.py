@@ -398,3 +398,69 @@ def progen2_rotary_tables(rotary_dim: int, slot: int, T: int):
     cos, sin = torch.ones((T, slot // 2)), torch.zeros((T, slot // 2))
     cos[:, :rotary_dim // 2], sin[:, :rotary_dim // 2] = torch.cos(sinusoid), torch.sin(sinusoid)
     return cos.contiguous(), sin.contiguous()
+
+
+@dataclass
+class Protgpt2Config:
+    layers: int
+    embed_dim: int
+    heads: int
+    ffn_dim: int
+    vocab: int
+    n_positions: int         # rows of the learned position table
+
+
+def load_protgpt2_checkpoint(folder: str):
+    """ProtGPT2 (GPT-2) model directory -> (Protgpt2Config, state). ``state`` has the key names of include/pgscore.h's PG_ARCH_PROTGPT2
+    (the ``transformer.`` prefix stripped; the tied ``lm_head.weight`` and the causal-mask buffers ``attn.bias`` / ``attn.masked_bias``
+    dropped) as fp32 CPU tensors; Conv1D weights stay [in, out].
+
+    config.json: ``n_embd``, ``n_layer``, ``n_head``, ``n_inner``, ``n_positions``, ``vocab_size``, ``layer_norm_epsilon``,
+    ``activation_function``, ``scale_attn_weights``, ``scale_attn_by_inverse_layer_idx`` and ``tie_word_embeddings``, with GPT2Config's
+    defaults for absent keys. Weights: pytorch_model.bin or *.safetensors. What the kernels do not implement is refused: an activation
+    other than gelu_new, LayerNorm eps other than 1e-5, attention scaled by the layer index or not scaled, head_dim other than 64, an
+    untied head."""
+    import json
+    cfg = json.load(open(os.path.join(folder, "config.json")))
+    d, layers, heads = int(cfg.get("n_embd", 768)), int(cfg.get("n_layer", 12)), int(cfg.get("n_head", 12))
+    vocab, npos = int(cfg.get("vocab_size", 50257)), int(cfg.get("n_positions", 1024))
+    ffn = int(cfg["n_inner"]) if cfg.get("n_inner") is not None else 4 * d
+    act = cfg.get("activation_function", "gelu_new")
+    eps = float(cfg.get("layer_norm_epsilon", 1e-5))
+    if act != "gelu_new":
+        raise NotImplementedError(f"ProtGPT2: activation_function {act!r}: the MLP epilogue implements gelu_new (tanh GELU)")
+    if eps != 1e-5:
+        raise NotImplementedError(f"ProtGPT2: layer_norm_epsilon {eps}: the LayerNorm kernels use eps 1e-5")
+    if cfg.get("scale_attn_by_inverse_layer_idx", False):
+        raise NotImplementedError("ProtGPT2: scale_attn_by_inverse_layer_idx: the attention scale is folded as 1/sqrt(head_dim) only")
+    if not cfg.get("scale_attn_weights", True):
+        raise NotImplementedError("ProtGPT2: scale_attn_weights false: the attention scale 1/sqrt(head_dim) is folded into q")
+    if not cfg.get("tie_word_embeddings", True):
+        raise NotImplementedError("ProtGPT2: tie_word_embeddings false: the fused head is the tied wte")
+    if d % heads or d // heads != 64:
+        raise NotImplementedError(f"ProtGPT2: head_dim {d / heads:g} (n_embd {d} / n_head {heads}): the kernels take 64-wide heads")
+    if d % 64 or ffn % 64:
+        raise NotImplementedError(f"ProtGPT2: n_embd {d} and n_inner {ffn} must be multiples of 64 (GEMM K tiles)")
+    raw = _read_hf_weights(folder)
+    state = {}
+    for k, v in raw.items():
+        name = k[len("transformer."):] if k.startswith("transformer.") else k
+        if name.endswith(".attn.bias") or name.endswith(".attn.masked_bias") or name == "lm_head.weight":
+            continue
+        state[name] = v.detach().float().contiguous()
+    want = {"wte.weight": (vocab, d), "wpe.weight": (npos, d), "ln_f.weight": (d,), "ln_f.bias": (d,)}
+    for i in range(layers):
+        p = f"h.{i}."
+        want.update({p + "ln_1.weight": (d,), p + "ln_1.bias": (d,), p + "ln_2.weight": (d,), p + "ln_2.bias": (d,),
+                     p + "attn.c_attn.weight": (d, 3 * d), p + "attn.c_attn.bias": (3 * d,), p + "attn.c_proj.weight": (d, d),
+                     p + "attn.c_proj.bias": (d,), p + "mlp.c_fc.weight": (d, ffn), p + "mlp.c_fc.bias": (ffn,),
+                     p + "mlp.c_proj.weight": (ffn, d), p + "mlp.c_proj.bias": (d,)})
+    for k, shape in want.items():
+        if k not in state:
+            raise ValueError(f"ProtGPT2 state dict: missing {k}")
+        if tuple(state[k].shape) != shape:
+            raise ValueError(f"ProtGPT2 state dict: {k} has shape {tuple(state[k].shape)}, expected {shape}")
+    extra = sorted(set(state) - set(want))
+    if extra:
+        raise ValueError(f"ProtGPT2 state dict: unexpected keys {extra[:5]}")
+    return Protgpt2Config(layers, d, heads, ffn, vocab, npos), state

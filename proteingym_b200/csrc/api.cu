@@ -268,6 +268,11 @@ struct pg_handle_s {
   float *hdw = nullptr, *hdb = nullptr, *hlng = nullptr, *hlnb = nullptr, *hbias = nullptr;
   float* outw = nullptr;  // untied output matrix [vocab, d] (ESM C sequence_head.3); null = the tied embedding
   int head_vocab = 0, label_off = 0;  // autoregressive head: columns (ProGen2: 25, vocabulary rows 5..29) and token id of column 0
+  // ProtGPT2's fused LM head (K16): the tied wte packed as a [vocab, dk] GEMM operand in fp16 hi [| lo] (never e4m3), and per pass the
+  // (max, sum exp) partials [max_rows, ceil(vocab / 128)] and target logits [max_rows] of GEMM epi 7
+  __half* lmw = nullptr;
+  float2* lm_part = nullptr;
+  float* lm_tgt = nullptr;
   float *rot_cos = nullptr, *rot_sin = nullptr;
   int rot_rows = 0;
   // workspace
@@ -307,7 +312,9 @@ struct pg_handle_s {
 namespace pg {
 namespace {
 
-bool is_ar(int arch) { return arch == PG_ARCH_TRANCEPTION || arch == PG_ARCH_RITA || arch == PG_ARCH_PROGEN2; }
+bool is_ar(int arch) {
+  return arch == PG_ARCH_TRANCEPTION || arch == PG_ARCH_RITA || arch == PG_ARCH_PROGEN2 || arch == PG_ARCH_PROTGPT2;
+}
 
 int fail(pg_handle h, int code, const std::string& msg) {
   if (h) h->err = msg;
@@ -624,28 +631,32 @@ int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const i
 //   ProGen2 (modeling_progen.py:244-282): RITA's rotary attention and tanh-GELU MLP as a parallel residual, x + attn(h) + mlp(h) with
 //   h = ln_1(x): fc_in runs on ln_1's output before attention overwrites it, then out_proj and fc_out add into x in that order (the
 //   reference adds (attn + mlp) + x: an fp32 reassociation).
+//   ProtGPT2 (GPT-2, transformers modeling_gpt2.py GPT2Model / GPT2Block): learned absolute positions added to the token embedding,
+//   c_attn with bias (q pre-scaled by 1/8 at load), causal attention without bias, c_proj, and RITA's tanh-GELU MLP.
 // mode 0: plain forward. mode 1 (B == 1): also record every layer's keys / values (Tranception: the raw q/k/v rows for the conv
-// look-back and the conv'd rows; RITA: the rotated rows) into the prefix caches.
+// look-back and the conv'd rows; the others: the (rotated) rows) into the prefix caches.
 // mode 2: the B sequences are rows [start, start + T) of sequences whose first `start` rows (multiple of 128) equal the recorded
-// wild type's: the keys / values of the prefix (and Tranception's conv look-back) come from the caches, and RITA's rotary runs at the
-// absolute positions start + t.
+// wild type's: the keys / values of the prefix (and Tranception's conv look-back) come from the caches, and the rotary or learned
+// positions are the absolute positions start + t.
 int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, int mode = 0, int start = 0) {
   const pg_model_desc& D = h->desc;
   const bool progen2 = D.arch == PG_ARCH_PROGEN2;
-  const bool rita = D.arch == PG_ARCH_RITA || progen2;  // rotary, no conv, no ALiBi, tanh-GELU
+  const bool tranception = D.arch == PG_ARCH_TRANCEPTION;  // conv'd q/k/v, grouped ALiBi, relu^2; the others: tanh-GELU, no attention bias
+  const bool rotary = D.arch == PG_ARCH_RITA || progen2;
   const int64_t ldq = h->op.ldq;
   const int rows = B * T;
   int rc;
-  { ProfScope ps(CAT_EMBED, s); rc = launch_gather_embed(ids, h->embed, rows, D.embed_dim, D.vocab, h->x, s); }
+  { ProfScope ps(CAT_EMBED, s);
+    rc = launch_gather_embed(ids, h->embed, rows, D.embed_dim, D.vocab, h->x, s, h->pos, T, mode == 2 ? start : 0); }  // pos: ProtGPT2's wpe
   if (rc) return rc;
   for (int l = 0; l < D.layers; ++l) {
     const Layer& L = h->layers[l];
     if ((rc = ln(h, h->x, L.ln1g, L.ln1b, rows, h->abuf, s))) return rc;
-    if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s, rita ? 3 : 0, 0.f, T, mode == 2 ? start : 0))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, rows, h->qkv, s, rotary ? 3 : 0, 0.f, T, mode == 2 ? start : 0))) return rc;
     if (progen2 && (rc = lin(h, L, FC1, h->abuf, S_LN, rows, h->fbuf, s, 6, S_GELU))) return rc;
     const size_t layer_off = static_cast<size_t>(l) * h->prefix_cap * ldq;
     const __half* kv = h->qkv;  // the q/k/v rows attention reads
-    if (!rita) {
+    if (tranception) {
       if (mode == 1)
         PG_CUDA_OK(cudaMemcpyAsync(h->raw_cache + layer_off, h->qkv, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
       { ProfScope ps(CAT_OTHER, s);
@@ -657,13 +668,13 @@ int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, in
     if (mode == 1)
       PG_CUDA_OK(cudaMemcpyAsync(h->kv_cache + layer_off, kv, static_cast<size_t>(T) * ldq * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     AttnLaunch a = attn_args(h, kv, h->abuf, B, T);
-    a.causal = 1; a.alibi_slopes = rita ? nullptr : h->slopes;
+    a.causal = 1; a.alibi_slopes = tranception ? h->slopes : nullptr;
     if (mode == 2) { a.prefix = h->kv_cache + layer_off; a.prefix_len = start; }
     { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc) return rc;
     if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
     if (progen2) rc = lin_add(h, L, FC2, h->fbuf, S_GELU, rows, h->x, s);
-    else rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, rita ? 6 : 4, rita ? S_GELU : S_RELU2, s);
+    else rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, tranception ? 4 : 6, tranception ? S_RELU2 : S_GELU, s);
     if (rc) return rc;
   }
   return PG_OK;
@@ -809,9 +820,27 @@ int compact_head(pg_handle h, int T, int Bc, float* out, int launches, cudaStrea
   return launch_head(hl, s);
 }
 
+// ProtGPT2's 50 257-way head on B sequences of T rows in h->x: ln_f into fp16 hi [| lo] operand rows (fmt 1 in both parity modes: no
+// LayerNorm follows the head, so it runs the x3 scheme, or single fp16 in PG_PREC_F16), the GEMM against the packed wte with the
+// log-softmax partial epilogue (epi 7, K16: no logit is stored unless f.out_logprobs asks for the rows), then the combine + sums.
+int lm_head_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, const ArFusion& f, float* tok_logp, float* out_sum,
+                  cudaStream_t s) {
+  const OpFmt& o = h->op;
+  const int d = h->desc.embed_dim, V = h->desc.vocab, rows = B * T;
+  int rc = launch_layernorm_f16(h->x, d, h->lnag, h->lnab, rows, d, h->abuf, o.ldd, o.lo_d, s, o.qfmt, 0.f, 0, 0, nullptr, 0, o.dk);
+  if (rc) return rc;
+  GemmLaunch g{};
+  g.a = h->abuf; g.lda = o.ldd; g.w = h->lmw; g.ldw = o.ldd; g.bias = nullptr;
+  g.M = rows; g.N = V; g.K = o.dk; g.nseg = o.pseg; g.epi = 7;
+  g.lm_part = h->lm_part; g.lm_tgt = h->lm_tgt; g.lm_logits = f.out_logprobs; g.lm_ids = ids; g.lm_lens = lens; g.lm_T = T;
+  if ((rc = launch_gemm(g, s))) return rc;
+  return launch_lm_head_combine(h->lm_part, (V + GEMM_BN - 1) / GEMM_BN, h->lm_tgt, ids, lens, B, T, V, f.out_logprobs, tok_logp, out_sum, s);
+}
+
 // The autoregressive head (ln_f, the handle's head matrix and bias, log-softmax) on B sequences of T rows in h->x.
 int ar_head(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, const ArFusion& f, float* tok_logp, float* out_sum,
             cudaStream_t s) {
+  if (h->desc.arch == PG_ARCH_PROTGPT2) return lm_head_fused(h, ids, lens, B, T, f, tok_logp, out_sum, s);
   return launch_ar_head(h->x, h->desc.embed_dim, B, T, h->head_vocab, ids, lens, h->lnag, h->lnab, h->outw ? h->outw : h->embed,
                         h->desc.arch == PG_ARCH_PROGEN2 ? h->hbias : nullptr, h->label_off, f, tok_logp, out_sum, s);
 }
@@ -826,7 +855,7 @@ int ar_passes(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T
     const long long off = static_cast<long long>(b0) * T;
     int rc = forward_ar(h, ids + off, Bc, T, s, mode, start);
     if (rc) return fail(h, rc, tls_error());
-    ProfScope ps(CAT_HEAD, s, 2);
+    ProfScope ps(CAT_HEAD, s, h->desc.arch == PG_ARCH_PROTGPT2 ? 4 : 2);
     ArFusion fc = fusion;
     if (fc.prior_row) fc.prior_row += off;
     if (fc.prior_row2) fc.prior_row2 += off;
@@ -903,11 +932,15 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   } else {
     if (D.arch == PG_ARCH_RITA && D.embed_dim != D.heads * 64)  // RITA XL (2048 / 16) has 128-wide heads
       return set_error(PG_ERR_UNSUPPORTED, "pg_create: RITA needs head_dim 64 (RITA S / M / L); 128-wide heads (RITA XL) have no attention tile");
+    if (D.arch == PG_ARCH_PROTGPT2 && D.embed_dim != D.heads * 64)  // the 1/8 q fold and the attention tile are for 64-wide heads
+      return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProtGPT2 needs head_dim 64 (GPT-2 large: 1280 / 20)");
+    if (D.arch == PG_ARCH_PROTGPT2 && D.max_positions <= 0)
+      return set_error(PG_ERR_ARG, "pg_create: ProtGPT2 needs max_positions = the rows of the position table (n_positions)");
     if (D.embed_dim != D.heads * 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: head_dim must be 64");
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
   }
   if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC &&
-      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2)
+      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2 && D.arch != PG_ARCH_PROTGPT2)
     return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
   if (D.arch == PG_ARCH_ESMC && D.heads > 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: the ESM C q/k LayerNorm kernel holds at most 24 heads");
   if (D.arch == PG_ARCH_TRANCEPTION && D.heads % 4) return set_error(PG_ERR_UNSUPPORTED, "pg_create: Tranception needs heads % 4 == 0 (model_pytorch.py:129-131)");
@@ -961,7 +994,13 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     A(&h->qkv2, static_cast<size_t>(h->max_rows) * 3 * d * np);
     A(&h->slopes, D.heads);
   }
-  if (D.arch == PG_ARCH_TRANCEPTION || D.arch == PG_ARCH_RITA || D.arch == PG_ARCH_PROGEN2) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
+  if (is_ar(D.arch)) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
+  if (D.arch == PG_ARCH_PROTGPT2) {  // 8 B per row and N tile: 412 MB at the default 131 072 rows and 50 257 columns
+    A(&h->lmw, static_cast<size_t>(D.vocab) * dk * np);
+    A(&h->lm_part, static_cast<size_t>(h->max_rows) * ((D.vocab + GEMM_BN - 1) / GEMM_BN));
+    A(&h->lm_tgt, static_cast<size_t>(h->max_rows));
+    A(&h->pos, static_cast<size_t>(D.max_positions) * d);
+  }
   if (h->op.nseg == 2) A(&h->pack_scratch, static_cast<size_t>(D.layers) * 6);
   A(&h->embed, static_cast<size_t>(D.vocab) * d);
   if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA) A(&h->pos, static_cast<size_t>(D.max_positions + 2) * d);
@@ -1022,12 +1061,12 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     scale_copy_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256>>>(src, dst, static_cast<int>(cnt), scale);
   };
   // A group of [N, K] weights that form one GEMM operand, packed into dst (inv: where the per-row 1/t of PG_PREC_F16F8 go).
-  // Conv1D weights are stored [in = K, out = N].
-  auto pack = [&](__half* dst, float* inv, std::initializer_list<PackSrc> group, int N, int K, bool conv1d = false) {
+  // Conv1D weights are stored [in = K, out = N]; conv_ld: their row pitch when the N columns are a slice of a wider matrix.
+  auto pack = [&](__half* dst, float* inv, std::initializer_list<PackSrc> group, int N, int K, bool conv1d = false, long long conv_ld = 0) {
     for (const PackSrc& m : group)
       if (!m.w) return;
     unsigned int* f8_scratch = h->op.nseg == 2 ? h->pack_scratch + (h->pack_used++ % (D.layers * 6)) : nullptr;
-    pack_weights(group, N, K, conv1d ? 1 : K, conv1d ? N : 1, np, f8_scratch, dst, inv, 0);
+    pack_weights(group, N, K, conv1d ? 1 : K, conv1d ? (conv_ld ? conv_ld : N) : 1, np, f8_scratch, dst, inv, 0);
   };
   // "rotary.cos" / "rotary.sin" [T, S/2] (ESM C, RITA: [T, 32]; ProGen2: half its slot width) -> the tables of the rotary GEMM epilogue
   auto rotary32 = [&]() -> int {
@@ -1157,6 +1196,35 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     else copy(h->outw, get("embedding.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
     if (int rc = rotary32()) return rc;
     if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
+  } else if (D.arch == PG_ARCH_PROTGPT2) {
+    // GPT-2 names without the "transformer." prefix (transformers modeling_gpt2.py GPT2Attention / GPT2MLP / GPT2Model), Conv1D weights
+    // [in, out]. c_attn's q, k and v column blocks form one GEMM operand with 1/sqrt(64) = 0.125 folded into the q columns and bias
+    // (exact: a power of two). The head is wte itself (tied), packed once more as a [vocab, d] operand for K16.
+    for (int l = 0; l < D.layers; ++l) {
+      Layer& L = h->layers[l];
+      const std::string p = "h." + std::to_string(l) + ".";
+      const float* wa = get(p + "attn.c_attn.weight", d, 3 * d);
+      pack(L.wqkv, L.iqkv, {{wa, 0.125f}, wa ? wa + d : nullptr, wa ? wa + 2 * d : nullptr}, d, d, true, 3 * d);
+      const float* ba = get(p + "attn.c_attn.bias", 3 * d, 1);
+      copy(L.bqkv, ba, d, 0.125f);
+      copy(L.bqkv + d, ba ? ba + d : nullptr, 2 * d);
+      pack(L.wo, L.io, {get(p + "attn.c_proj.weight", d, d)}, d, d, true);
+      copy(L.bo, get(p + "attn.c_proj.bias", d, 1), d);
+      pack(L.w1, L.i1, {get(p + "mlp.c_fc.weight", d, f)}, f, d, true);
+      copy(L.b1, get(p + "mlp.c_fc.bias", f, 1), f);
+      pack(L.w2, L.i2, {get(p + "mlp.c_proj.weight", f, d)}, d, f, true);
+      copy(L.b2, get(p + "mlp.c_proj.bias", d, 1), d);
+      copy(L.ln1g, get(p + "ln_1.weight", d, 1), d);
+      copy(L.ln1b, get(p + "ln_1.bias", d, 1), d);
+      copy(L.ln2g, get(p + "ln_2.weight", d, 1), d);
+      copy(L.ln2b, get(p + "ln_2.bias", d, 1), d);
+    }
+    const float* wte = get("wte.weight", D.vocab, d);
+    copy(h->embed, wte, static_cast<size_t>(D.vocab) * d);
+    if (wte) pack_weights({wte}, D.vocab, d, d, 1, np, nullptr, h->lmw, nullptr, 0);  // fp16 hi [| lo] in every mode
+    copy(h->pos, get("wpe.weight", D.max_positions, d), static_cast<size_t>(D.max_positions) * d);
+    copy(h->lnag, get("ln_f.weight", d, 1), d);
+    copy(h->lnab, get("ln_f.bias", d, 1), d);
   } else if (D.arch == PG_ARCH_PROGEN2) {
     // HF names without the "transformer." prefix (modeling_progen.py:84-95, 209-226, 389-401, 541-548). qkv_proj [3d, d] is placed
     // into the head slots by SL_PGQ / SL_PGK / SL_PGV (one GEMM operand, no bias) with head_dim^-1/2 folded into the q rows: exact
@@ -1378,6 +1446,8 @@ static int ar_fusion_args(pg_handle h, const pg_ar_fusion* f, ArFusion* base) {
     return fail(h, PG_ERR_ARG, "pg_ar_loglik: RITA has no retrieval fusion (pass no log_prior / log_prior2)");
   if (h->desc.arch == PG_ARCH_PROGEN2 && (f->log_prior || f->log_prior2))
     return fail(h, PG_ERR_ARG, "pg_ar_loglik: ProGen2 has no retrieval fusion (pass no log_prior / log_prior2)");
+  if (h->desc.arch == PG_ARCH_PROTGPT2 && (f->log_prior || f->log_prior2))
+    return fail(h, PG_ERR_ARG, "pg_ar_loglik: ProtGPT2 has no retrieval fusion (pass no log_prior / log_prior2)");
   base->log_prior = f->log_prior; base->prior_row = f->prior_row; base->alpha = f->alpha;
   base->log_prior2 = f->log_prior2; base->prior_row2 = f->prior_row2; base->beta = f->beta;
   base->first_col = f->first_col; base->out_logprobs = f->out_logprobs;
@@ -1426,7 +1496,7 @@ int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_f
   // per-token log p(ids[t+1] | ids[<=t]) of the wild type, t = 0 .. T-2 (and the fused rows in f->out_logprobs when asked for)
   int32_t* len_dev = h->row_sel;
   PG_CUDA_OK(cudaMemcpyAsync(len_dev, &T, sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  { ProfScope ps(CAT_HEAD, s, 2);
+  { ProfScope ps(CAT_HEAD, s, h->desc.arch == PG_ARCH_PROTGPT2 ? 4 : 2);
     rc = ar_head(h, ids, len_dev, 1, T, fu, out_tok_logp, h->tok_logp, s); }
   if (rc) return fail(h, rc, tls_error());
   h->prefix_T = T;

@@ -72,8 +72,15 @@ struct GemmLaunch {
   //   mask_pos  [M / base_T] (device): epi 2 only — row (row / base_T) * base_T + mask_pos[row / base_T] receives no update (its
   //                               exact value comes from the compact full-precision path)
   const float* base_pre = nullptr; const __half* base_post = nullptr; int base_T = 0; const int32_t* mask_pos = nullptr;
+  // LM-head log-softmax partials (epi 7, K16; internal): the accumulator holds the logits of rows (b, t) = (row / lm_T, row % lm_T)
+  // against N vocabulary columns, and no logit is stored. For every row with t + 1 < lm_lens[b] and every 128-column N tile the tile's
+  // (max, sum exp(l - max)) goes to lm_part[row * tiles_n + tile] (columns >= N count as -inf), and the logit of column
+  // lm_ids[row + 1] to lm_tgt[row]; lm_logits (optional, [M, N] fp32) receives every logit of those rows.
+  float2* lm_part = nullptr; float* lm_tgt = nullptr; float* lm_logits = nullptr;
+  const int32_t* lm_ids = nullptr; const int32_t* lm_lens = nullptr; int lm_T = 0;
 };
 int launch_gemm(const GemmLaunch& g, cudaStream_t s);
+constexpr int GEMM_BN = 128;  // N tile of launch_gemm (the granularity of the epi 7 partials)
 void set_gemm_kchunk(int v);    // tuning: see gemm_tc.cu
 void set_gemm_prefetch(int v);
 void set_gemm_cta2(int v);      // 1: clusters of two CTAs sharing the W tile (TMA multicast)
@@ -165,7 +172,9 @@ int launch_gather_rows(const float* x, const int32_t* row_sel, int B, int T, int
 // rotary per 64-wide head (t = row % T, cos/sin [T, 32]) and q *= 1/8 (elementwise.cu).
 int launch_qk_ln_rotary(__half* qkv, int64_t ld, int64_t lo_off, int rows, int heads, const float* q_gamma, const float* k_gamma,
                         const float* rot_cos, const float* rot_sin, int T, cudaStream_t s);
-int launch_gather_embed(const int32_t* ids, const float* wte, long long rows, int d, int vocab, float* x, cudaStream_t s);
+// x[row] = wte[ids[row]] (+ wpe[row % T + pos_off] when a position table is given; null keeps the token embedding alone)
+int launch_gather_embed(const int32_t* ids, const float* wte, long long rows, int d, int vocab, float* x, cudaStream_t s,
+                        const float* wpe = nullptr, int T = 1, int pos_off = 0);
 int launch_qkv_conv(const __half* in, __half* out, int64_t ld, int64_t lo_off, int B, int T, int heads, const float* taps,
                     float qscale, cudaStream_t s, const __half* prefix = nullptr);
 // Retrieval-prior fusion arguments of the autoregressive head (device pointers; see pg_ar_fusion in include/pgscore.h).
@@ -179,6 +188,11 @@ struct ArFusion {
 int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t* ids, const int32_t* lens, const float* lnf_g,
                    const float* lnf_b, const float* wte, const float* bias, int label_off, const ArFusion& fusion, float* tok_logp,
                    float* out_sum, cudaStream_t s);
+// After a GEMM epi 7 pass over B sequences of T rows: tok_logp[r] = lm_tgt[r] - logsumexp of the row's `tiles` partials combined in
+// tile order (0 for t >= lens[b] - 1, NaN for a next token outside [0, vocab)); out_logprobs (optional, [B*T, vocab], holding the logits
+// epi 7 wrote) becomes the log-softmax rows in place; out_sum[b] = the sequence sums (seq_sum_kernel).
+int launch_lm_head_combine(const float2* part, int tiles, const float* tgt, const int32_t* ids, const int32_t* lens, int B, int T, int vocab,
+                           float* out_logprobs, float* tok_logp, float* out_sum, cudaStream_t s);
 }  // namespace pg
 
 namespace pg {

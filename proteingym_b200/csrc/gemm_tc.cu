@@ -24,7 +24,8 @@
 //                 x 128 B of W, 128B swizzle; a row of 128 B is 64 fp16 or 128 e4m3 along K) into a 6-stage ring; 40 registers
 //   warpgroups 1-2 consumers, rows [0, 64) and [64, 128) of the tile: wgmma m64n128 (K = 16 fp16 / 32 e4m3: 32 B of each row) x4
 //                 per stage, then bias / erf-GELU / relu^2 / rotary / SwiGLU / tanh-GELU and fp16 hi [+ fp16 lo | + e4m3 planes for the next GEMM]
-//                 stored straight from the accumulator fragments, or added into the fp32 residual stream (one owner per element)
+//                 stored straight from the accumulator fragments, or added into the fp32 residual stream (one owner per element), or
+//                 (epi 7, K16) reduced to per-tile log-softmax partials of an LM head without storing the logits
 // Roofline: tensor bound. Algorithmic FLOPs = 2*M*N*K; issued tensor-pipe work = x1 / x2 / x3 by mode.
 #include <cstdlib>
 #include <cstring>
@@ -38,6 +39,7 @@ namespace pg {
 namespace {
 
 constexpr int BM = 128, BN = 128, BK = 64, STAGES = 6;
+static_assert(BN == GEMM_BN, "common.h GEMM_BN sizes the LM-head partial buffers");
 constexpr int GEMM_THREADS = 384;
 constexpr uint32_t A_BYTES = BM * BK * 2;  // 16 KiB
 constexpr uint32_t B_BYTES = BN * BK * 2;  // 16 KiB
@@ -73,6 +75,8 @@ struct GemmKParams {
   // delta-operand mode (common.h GemmLaunch): shared base rows added before / subtracted after the activation, masked rows skipped
   const float* base_pre; const __half* base_post; int base_T; const int* mask_pos;
   int grp_rows_a, grp_rows_b;  // grouped (block-diagonal) mode: A rows [g*grp_rows_a, (g+1)*grp_rows_a) pair with W rows g*grp_rows_b + n
+  // LM-head log-softmax partials (epi 7; common.h GemmLaunch)
+  float2* lm_part; float* lm_tgt; float* lm_logits; const int32_t* lm_ids; const int32_t* lm_lens; int lm_T;
 };
 
 // Exact-erf GELU (esm/modules.py:17-24): 0.5*x*(1+erf(x/sqrt2)) = 0.5*x + 0.5*|x|*erf(|x|/sqrt2).
@@ -184,7 +188,52 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
       }
     }
     if (row >= p.M) continue;
-    if (EPI == 2) {
+    if (EPI == 7) {
+      // LM-head partials (K16): the four threads of a quad (lanes 4g .. 4g+3) hold the 128 columns of this row's N tile, 32 each; the
+      // row, and so every branch below, is uniform over the quad. No logit leaves the registers unless lm_logits asks for them.
+      const int t = static_cast<int>(row % p.lm_T);
+      if (t + 1 >= __ldg(p.lm_lens + row / p.lm_T)) continue;
+      const unsigned quad = 0xFu << (threadIdx.x & 28);
+      float m = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = col0 + 8 * j;
+        if (col < p.N) m = fmaxf(m, acc[4 * j + 2 * h]);
+        if (col + 1 < p.N) m = fmaxf(m, acc[4 * j + 2 * h + 1]);
+      }
+      m = fmaxf(m, __shfl_xor_sync(quad, m, 1));
+      m = fmaxf(m, __shfl_xor_sync(quad, m, 2));
+      float se = 0.f;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = col0 + 8 * j;
+        if (col < p.N) se += expf(acc[4 * j + 2 * h] - m);
+        if (col + 1 < p.N) se += expf(acc[4 * j + 2 * h + 1] - m);
+      }
+      se += __shfl_xor_sync(quad, se, 1);
+      se += __shfl_xor_sync(quad, se, 2);
+      if ((threadIdx.x & 3) == 0) p.lm_part[row * p.tiles_n + col0 / BN] = make_float2(m, se);
+      const int label = __ldg(p.lm_ids + row + 1);
+      const int jl = label - col0;  // this thread's columns are col0 + 8j + e, j < 16, e < 2
+      if (jl >= 0 && jl < 128 && (jl & 7) < 2 && label < p.N) {
+        float v = 0.f;  // selected, not indexed: an index into acc that depends on the label would move acc to local memory
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+          v = (jl == 8 * j) ? a0 : ((jl == 8 * j + 1) ? a1 : v);
+        }
+        p.lm_tgt[row] = v;
+      }
+      if (p.lm_logits != nullptr) {
+        float* lr = p.lm_logits + row * p.N;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = col0 + 8 * j;
+          if (col < p.N) lr[col] = acc[4 * j + 2 * h];
+          if (col + 1 < p.N) lr[col + 1] = acc[4 * j + 2 * h + 1];
+        }
+      }
+    } else if (EPI == 2) {
       // the masked row of each copy is updated by the compact exact path instead (delta-operand mode)
       if (p.mask_pos != nullptr && trow == __ldg(p.mask_pos + row / p.base_T)) continue;
       float* r = p.resid + row * p.ldr;
@@ -528,10 +577,12 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return set_error(PG_ERR_ARG, "gemm: empty problem");
   if (g.K % BK) return set_error(PG_ERR_ARG, "gemm: K must be a multiple of 64");
   if (g.nseg < 1 || g.nseg > 3) return set_error(PG_ERR_ARG, "gemm: nseg must be 1, 2 (fp16 + e4m3 cross terms) or 3");
-  if (g.epi < 0 || g.epi > 6) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
+  if (g.epi < 0 || g.epi > 7) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
+  if (g.epi == 7 && (!g.lm_part || !g.lm_tgt || !g.lm_ids || !g.lm_lens || g.lm_T <= 0 || g.M % g.lm_T || g.grp_rows_a || g.bias))
+    return set_error(PG_ERR_ARG, "gemm: the LM-head epilogue needs partial, target, ids and lens buffers, rows a multiple of lm_T, no groups or bias");
   if (g.epi == 5 && (g.N % 16 || (g.out_fmt == 2 && (g.N / 2) % 64) || g.grp_rows_a || (g.out_fmt >= 1 && g.out_lo_off < g.N / 2)))
     return set_error(PG_ERR_ARG, "gemm: the SwiGLU epilogue needs N % 16 == 0 (N/2 % 64 == 0 for out_fmt 2), no groups, planes >= N/2 apart");
-  if (g.epi == 2 ? !g.resid : !g.out) return set_error(PG_ERR_ARG, "gemm: missing output");
+  if (g.epi != 7 && (g.epi == 2 ? !g.resid : !g.out)) return set_error(PG_ERR_ARG, "gemm: missing output");
   if (g.epi == 3 && (!g.rot_cos || !g.rot_sin || g.rot_T <= 0 || g.rot_dim % 64)) return set_error(PG_ERR_ARG, "gemm: bad rotary args");
   if (g.epi == 3 && ((g.rot_half != 32 && g.rot_half != 64) || g.rot_dim % (2 * g.rot_half)))
     return set_error(PG_ERR_ARG, "gemm: rotary slots must be 64 or 128 wide and divide rot_dim");
@@ -545,7 +596,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   if (g.epi != 2 && g.out_fmt >= 1 && g.out_lo_off <= 0) return set_error(PG_ERR_ARG, "gemm: out_fmt 1/2 need out_lo_off > 0");
   if ((g.base_pre || g.base_post || g.mask_pos) && g.epi > 2)
     return set_error(PG_ERR_UNSUPPORTED, "gemm: the delta-operand form runs with epilogues 0, 1, 2");
-  if (g.epi == 2 ? (g.ldr % 2 || (reinterpret_cast<uintptr_t>(g.resid) & 7)) : (g.ldo % 2 || (reinterpret_cast<uintptr_t>(g.out) & 3) || g.out_lo_off % 2))
+  if (g.epi != 7 && (g.epi == 2 ? (g.ldr % 2 || (reinterpret_cast<uintptr_t>(g.resid) & 7)) : (g.ldo % 2 || (reinterpret_cast<uintptr_t>(g.out) & 3) || g.out_lo_off % 2)))
     return set_error(PG_ERR_ARG, "gemm: output pitches must be even and the output 8-byte (fp32) / 4-byte (fp16) aligned");
   int dev = 0;
   PG_CUDA_OK(cudaGetDevice(&dev));
@@ -554,7 +605,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
 #define PG_SET_SMEM(E)                                                                                           \
   PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM)); \
   PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM))
-    PG_SET_SMEM(0); PG_SET_SMEM(1); PG_SET_SMEM(2); PG_SET_SMEM(3); PG_SET_SMEM(4); PG_SET_SMEM(5); PG_SET_SMEM(6);
+    PG_SET_SMEM(0); PG_SET_SMEM(1); PG_SET_SMEM(2); PG_SET_SMEM(3); PG_SET_SMEM(4); PG_SET_SMEM(5); PG_SET_SMEM(6); PG_SET_SMEM(7);
 #undef PG_SET_SMEM
     attr_set[dev] = true;
   }
@@ -618,6 +669,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   p.prefetch = grouped ? 0 : gemm_prefetch();
   p.grp_rows_a = g.grp_rows_a; p.grp_rows_b = g.grp_rows_b;
   p.base_pre = g.base_pre; p.base_post = g.base_post; p.base_T = g.base_T; p.mask_pos = g.mask_pos;
+  p.lm_part = g.lm_part; p.lm_tgt = g.lm_tgt; p.lm_logits = g.lm_logits; p.lm_ids = g.lm_ids; p.lm_lens = g.lm_lens; p.lm_T = g.lm_T;
   const int ntiles = p.tiles_m * p.tiles_n;
   cudaLaunchConfig_t cfg{};
   cudaLaunchAttribute attr[1];
@@ -644,7 +696,8 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
     case 3: e = PG_LAUNCH(3); break;
     case 4: e = PG_LAUNCH(4); break;
     case 5: e = PG_LAUNCH(5); break;
-    default: e = PG_LAUNCH(6); break;
+    case 6: e = PG_LAUNCH(6); break;
+    default: e = PG_LAUNCH(7); break;
   }
 #undef PG_LAUNCH
   PG_CUDA_OK(e);

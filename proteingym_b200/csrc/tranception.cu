@@ -1,9 +1,11 @@
 // Tranception-specific helper kernels (HBM-bound, fp32 arithmetic):
-//   gather_embed_kernel   x[row] = wte[ids[row]]                                   (model_pytorch.py:526-532, no position table)
+//   gather_embed_kernel   x[row] = wte[ids[row]] (+ wpe[pos])                      (model_pytorch.py:526-532, no position table;
+//                         GPT-2 modeling_gpt2.py GPT2Model.forward: inputs_embeds + position_embeds)
 //   qkv_conv_kernel       depthwise causal conv (k = 1,3,5,7 by head group) on q, k and v + the 1/sqrt(hd) query scale
 //                         (model_pytorch.py:73-88, :240-251, :158-159)
 //   ar_head_kernel        ln_f -> lm_head (optional bias) -> log_softmax -> optional retrieval-prior fusion -> log p(next token)
 //                         (model_pytorch.py:612, :783, :806-830; utils/scoring_utils.py:121-128)
+//   lm_combine_kernel     the per-tile (max, sum exp) partials of the fused LM head (GEMM epi 7) -> log p(next token)
 //   seq_sum_kernel        per-sequence sum over the real (non-pad) predicted tokens, fixed order
 #include "common.h"
 #include "operand.cuh"
@@ -13,14 +15,23 @@ namespace pg {
 
 namespace {
 
+// wpe (optional): learned positions, row r at position r % T + pos_off (a suffix after a shared prefix starts at pos_off).
 __global__ void gather_embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ wte, int d, int vocab,
-                                    float* __restrict__ x) {
+                                    float* __restrict__ x, const float* __restrict__ wpe, int T, int pos_off) {
   const long long r = blockIdx.x;
   int tok = ids[r];
   tok = tok < 0 ? 0 : (tok >= vocab ? vocab - 1 : tok);
   const float4* src = reinterpret_cast<const float4*>(wte + static_cast<long long>(tok) * d);
   float4* dst = reinterpret_cast<float4*>(x + r * d);
-  for (int j = threadIdx.x; j < d / 4; j += blockDim.x) dst[j] = src[j];
+  if (wpe == nullptr) {
+    for (int j = threadIdx.x; j < d / 4; j += blockDim.x) dst[j] = src[j];
+    return;
+  }
+  const float4* pe = reinterpret_cast<const float4*>(wpe + (r % T + pos_off) * d);
+  for (int j = threadIdx.x; j < d / 4; j += blockDim.x) {
+    const float4 a = src[j], b = pe[j];
+    dst[j] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
 }
 
 // Depthwise conv: the block stages a [CV_T + 6 rows] x [CV_C channels] tile (hi and lo planes) in shared memory with cp.async —
@@ -163,6 +174,44 @@ __global__ void ar_head_kernel(ArHeadParams p) {
   }
 }
 
+// One warp per token row r = (b, t) of the fused LM head: the row's (max, sum exp) partials of `tiles` N tiles merged in fixed order
+// (lane k takes tiles k, k + 32, ..., then a fixed shuffle tree), lse = max + log(sum), log p = target logit - lse. out_logprobs rows
+// hold the row's logits (epi 7's lm_logits) and are turned into log-probabilities in place.
+__global__ void lm_combine_kernel(const float2* __restrict__ part, int tiles, const float* __restrict__ tgt, const int32_t* __restrict__ ids,
+                                  const int32_t* __restrict__ lens, long long rows, int T, int vocab, float* __restrict__ out_logprobs,
+                                  float* __restrict__ tok_logp) {
+  const long long r = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  const int lane = threadIdx.x & 31;
+  const int t = static_cast<int>(r % T);
+  if (t + 1 >= lens[r / T]) {
+    if (lane == 0) tok_logp[r] = 0.f;
+    return;
+  }
+  float m = -INFINITY, s = 0.f;
+  for (int k = lane; k < tiles; k += 32) {
+    const float2 q = part[r * tiles + k];
+    const float mn = fmaxf(m, q.x);
+    s = s * expf(m - mn) + q.y * expf(q.x - mn);
+    m = mn;
+  }
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float mo = __shfl_xor_sync(0xffffffffu, m, o), so = __shfl_xor_sync(0xffffffffu, s, o);
+    const float mn = fmaxf(m, mo);
+    // lanes with no tile (tiles < 32) carry m = -inf, s = 0: exp(-inf - mn) = 0, and mn is finite as soon as one lane has a tile
+    s = (m == -INFINITY ? 0.f : s * expf(m - mn)) + (mo == -INFINITY ? 0.f : so * expf(mo - mn));
+    m = mn;
+  }
+  const float lse = m + logf(s);
+  if (out_logprobs)
+    for (int v = lane; v < vocab; v += 32) out_logprobs[r * vocab + v] -= lse;
+  if (lane == 0) {
+    const int label = ids[r + 1];
+    tok_logp[r] = (label < 0 || label >= vocab) ? NAN : tgt[r] - lse;
+  }
+}
+
 // One warp per sequence: sum tok_logp[b, 0 .. len-2] (lane-strided partials, then a fixed shuffle tree).
 __global__ void seq_sum_kernel(const float* __restrict__ tok_logp, const int32_t* __restrict__ lens, int B, int T,
                                float* __restrict__ out) {
@@ -178,9 +227,11 @@ __global__ void seq_sum_kernel(const float* __restrict__ tok_logp, const int32_t
 
 }  // namespace
 
-int launch_gather_embed(const int32_t* ids, const float* wte, long long rows, int d, int vocab, float* x, cudaStream_t s) {
+int launch_gather_embed(const int32_t* ids, const float* wte, long long rows, int d, int vocab, float* x, cudaStream_t s, const float* wpe,
+                        int T, int pos_off) {
   if (rows <= 0) return PG_OK;
-  gather_embed_kernel<<<static_cast<unsigned>(rows), 128, 0, s>>>(ids, wte, d, vocab, x);
+  if (T <= 0) return set_error(PG_ERR_ARG, "gather_embed: T must be positive");
+  gather_embed_kernel<<<static_cast<unsigned>(rows), 128, 0, s>>>(ids, wte, d, vocab, x, wpe, T, pos_off);
   PG_CUDA_OK(cudaGetLastError());
   return PG_OK;
 }
@@ -214,6 +265,16 @@ int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t
   if (B <= 0 || T <= 0) return PG_OK;
   ArHeadParams p{x, d, T, vocab, ids, lens, lnf_g, lnf_b, wte, bias, label_off, fusion, tok_logp};
   ar_head_kernel<<<static_cast<unsigned>(static_cast<long long>(B) * T), 128, (d + vocab) * sizeof(float), s>>>(p);
+  seq_sum_kernel<<<(B + 3) / 4, 128, 0, s>>>(tok_logp, lens, B, T, out_sum);
+  PG_CUDA_OK(cudaGetLastError());
+  return PG_OK;
+}
+
+int launch_lm_head_combine(const float2* part, int tiles, const float* tgt, const int32_t* ids, const int32_t* lens, int B, int T, int vocab,
+                           float* out_logprobs, float* tok_logp, float* out_sum, cudaStream_t s) {
+  if (B <= 0 || T <= 0) return PG_OK;
+  const long long rows = static_cast<long long>(B) * T;
+  lm_combine_kernel<<<static_cast<unsigned>((rows + 3) / 4), 128, 0, s>>>(part, tiles, tgt, ids, lens, rows, T, vocab, out_logprobs, tok_logp);
   seq_sum_kernel<<<(B + 3) / 4, 128, 0, s>>>(tok_logp, lens, B, T, out_sum);
   PG_CUDA_OK(cudaGetLastError());
   return PG_OK;

@@ -690,3 +690,73 @@ def write_progen2_checkpoint(folder: str, arch: Progen2Arch, seed: int = 0, stat
     else:
         torch.save(st, os.path.join(folder, "pytorch_model.bin"))
     return st
+
+
+# ---- ProtGPT2 (GPT-2 large shape; transformers modeling_gpt2.py) -----------------------------------------------------------------------
+@dataclass(frozen=True)
+class Protgpt2Arch:
+    layers: int
+    embed_dim: int
+    heads: int
+    n_positions: int = 1024
+    vocab: int = 50257
+    n_inner: int | None = None
+
+    @property
+    def ffn_dim(self) -> int:
+        return self.n_inner if self.n_inner is not None else 4 * self.embed_dim
+
+
+PROTGPT2 = Protgpt2Arch(36, 1280, 20)  # nferruz/ProtGPT2: GPT-2 large, 738M parameters
+
+
+def make_protgpt2_state(arch: Protgpt2Arch, seed: int = 0, buffers: bool = False) -> dict:
+    """GPT2LMHeadModel state dict (``transformer.`` prefix, Conv1D weights [in, out], ``lm_head.weight`` tied to wte; with ``buffers``
+    the causal-mask buffers ``attn.bias`` a saved state dict of older transformers releases carries), drawn on the CPU from ``seed``:
+    GPT-2's N(0, 0.02) initialisation with larger embedding rows (N(0, 0.15)) and LayerNorm weights 1 + 0.1 N(0,1), biases 0.05 N(0,1),
+    so that the 50 257-way log-probabilities spread over several nats."""
+    g = torch.Generator().manual_seed(seed)
+    d, f, V, n = arch.embed_dim, arch.ffn_dim, arch.vocab, arch.n_positions
+    ln_w = lambda: 1 + 0.1 * torch.randn(d, generator=g)  # noqa: E731
+    ln_b = lambda: 0.05 * torch.randn(d, generator=g)  # noqa: E731
+    st = {"transformer.wte.weight": 0.15 * torch.randn((V, d), generator=g), "transformer.wpe.weight": 0.05 * torch.randn((n, d), generator=g)}
+    for i in range(arch.layers):
+        p = f"transformer.h.{i}."
+        st[p + "ln_1.weight"], st[p + "ln_1.bias"] = ln_w(), ln_b()
+        if buffers:
+            st[p + "attn.bias"] = torch.tril(torch.ones((n, n), dtype=torch.bool)).view(1, 1, n, n)
+            st[p + "attn.masked_bias"] = torch.tensor(-1e4)
+        st[p + "attn.c_attn.weight"] = 0.05 * torch.randn((d, 3 * d), generator=g)
+        st[p + "attn.c_attn.bias"] = 0.02 * torch.randn(3 * d, generator=g)
+        st[p + "attn.c_proj.weight"] = 0.02 * torch.randn((d, d), generator=g)
+        st[p + "attn.c_proj.bias"] = 0.02 * torch.randn(d, generator=g)
+        st[p + "ln_2.weight"], st[p + "ln_2.bias"] = ln_w(), ln_b()
+        st[p + "mlp.c_fc.weight"] = 0.02 * torch.randn((d, f), generator=g)
+        st[p + "mlp.c_fc.bias"] = 0.02 * torch.randn(f, generator=g)
+        st[p + "mlp.c_proj.weight"] = 0.02 * torch.randn((f, d), generator=g)
+        st[p + "mlp.c_proj.bias"] = 0.02 * torch.randn(d, generator=g)
+    st["transformer.ln_f.weight"], st["transformer.ln_f.bias"] = ln_w(), ln_b()
+    st["lm_head.weight"] = st["transformer.wte.weight"]
+    return st
+
+
+def write_protgpt2_checkpoint(folder: str, arch: Protgpt2Arch, seed: int = 0, state: dict | None = None, safetensors: bool = False,
+                              config_extra: dict | None = None) -> dict:
+    """A GPT-2 model directory as ProtGPT2 is published: config.json (GPT2Config keys) and pytorch_model.bin or model.safetensors
+    (safetensors stores the tied head once, without lm_head.weight)."""
+    os.makedirs(folder, exist_ok=True)
+    st = make_protgpt2_state(arch, seed) if state is None else state
+    cfg = dict(model_type="gpt2", architectures=["GPT2LMHeadModel"], vocab_size=arch.vocab, n_positions=arch.n_positions, n_ctx=arch.n_positions,
+               n_embd=arch.embed_dim, n_layer=arch.layers, n_head=arch.heads, n_inner=arch.n_inner, activation_function="gelu_new",
+               resid_pdrop=0.0, embd_pdrop=0.0, attn_pdrop=0.0, layer_norm_epsilon=1e-5, initializer_range=0.02,
+               scale_attn_weights=True, scale_attn_by_inverse_layer_idx=False, reorder_and_upcast_attn=False, use_cache=True,
+               bos_token_id=0, eos_token_id=0, tie_word_embeddings=True)
+    cfg.update(config_extra or {})
+    with open(os.path.join(folder, "config.json"), "w") as fh:
+        json.dump(cfg, fh, indent=1)
+    if safetensors:
+        from safetensors.torch import save_file
+        save_file({k: v.contiguous() for k, v in st.items() if k != "lm_head.weight"}, os.path.join(folder, "model.safetensors"))
+    else:
+        torch.save(st, os.path.join(folder, "pytorch_model.bin"))
+    return st

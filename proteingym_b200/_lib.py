@@ -5,12 +5,15 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpgscore.so")
 
 PG_ARCH_ESM1B, PG_ARCH_ESM2, PG_ARCH_TRANCEPTION, PG_ARCH_MSA, PG_ARCH_ESMC, PG_ARCH_RITA, PG_ARCH_PROGEN2 = 0, 1, 2, 3, 4, 5, 6
 PG_ARCH_PROTGPT2 = 7
 PG_PREC_F16, PG_PREC_F16X3, PG_PREC_F16F8, PG_PREC_F16D = 0, 1, 2, 3
+PRECISIONS = {"f16": PG_PREC_F16, "f16x3": PG_PREC_F16X3, "f16f8": PG_PREC_F16F8, "f16d": PG_PREC_F16D}
 
 
 class PgModelDesc(C.Structure):
@@ -114,3 +117,47 @@ def check(rc: int, handle=None):
     if rc != 0:
         msg = load().pg_last_error(handle)
         raise PgError(f"libpgscore error {rc}: {msg.decode() if msg else '?'}")
+
+
+class Model:
+    """Owner of one libpgscore handle: ``pg_create`` from a PgModelDesc, then ``pg_load_weights`` from fp32 tensors staged on the device
+    (the library repacks them; the staging copy is freed before the constructor returns). ``close()`` (also on garbage collection)
+    destroys the handle; it is safe on an object whose constructor never ran."""
+    handle = None
+
+    def __init__(self, desc: PgModelDesc, tensors: dict, device: int = 0):
+        if not torch.cuda.is_available():
+            raise PgError("no CUDA device: the H100 scorer has no CPU fallback")
+        self.lib = load()
+        self.device = torch.device("cuda", device)
+        self.handle = C.c_void_p()
+        check(self.lib.pg_create(C.byref(desc), C.byref(self.handle)))
+        try:
+            gpu = [(n, t.to(self.device, torch.float32).contiguous()) for n, t in tensors.items()]
+            arr = (PgTensor * len(gpu))()
+            for i, (n, t) in enumerate(gpu):
+                arr[i].name = n.encode()
+                arr[i].data = t.data_ptr()
+                arr[i].shape[0] = t.shape[0]
+                arr[i].shape[1] = t.shape[1] if t.dim() == 2 else 1
+            torch.cuda.synchronize(self.device)
+            check(self.lib.pg_load_weights(self.handle, arr, len(gpu)), self.handle)
+            del gpu
+            torch.cuda.empty_cache()
+        except Exception:
+            self.close()
+            raise
+
+    def stream(self):
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def close(self):
+        if self.handle:
+            self.lib.pg_destroy(self.handle)
+            self.handle = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

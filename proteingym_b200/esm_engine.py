@@ -8,18 +8,16 @@ PyTorch is used for device memory and streams only; all arithmetic happens in th
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 import torch
 
 from . import _lib
+from ._lib import PRECISIONS
 from .alphabet import ALPHABET
 from .checkpoint import EsmConfig, esmc_rotary_tables, rotary_tables
 from .mutants import parse_esmc_mutants, parse_mutants
 from .windows import esmc_window_rows, optimal_window_starts
 
-PRECISIONS = {"f16": _lib.PG_PREC_F16, "f16x3": _lib.PG_PREC_F16X3, "f16f8": _lib.PG_PREC_F16F8, "f16d": _lib.PG_PREC_F16D}
 ARCHS = {"esm1b": _lib.PG_ARCH_ESM1B, "esm2": _lib.PG_ARCH_ESM2, "esmc": _lib.PG_ARCH_ESMC}
 
 
@@ -56,13 +54,9 @@ def choose_precision(config: EsmConfig, mutants=None, strategy: str = "masked-ma
     return "f16f8"
 
 
-class EsmScorer:
+class EsmScorer(_lib.Model):
     def __init__(self, config: EsmConfig, state: dict, precision: str = "f16f8", device: int = 0, max_rows: int = 0):
-        if not torch.cuda.is_available():
-            raise _lib.PgError("no CUDA device: the H100 scorer has no CPU fallback")
-        self.lib = _lib.load()
         self.config = config
-        self.device = torch.device("cuda", device)
         self.precision = precision
         desc = _lib.PgModelDesc(
             arch=ARCHS[config.arch], layers=config.layers,
@@ -70,46 +64,14 @@ class EsmScorer:
             max_positions=config.max_positions, token_dropout=int(config.token_dropout),
             emb_ln_before=int(config.emb_layer_norm_before), precision=PRECISIONS[precision], device=device,
             max_rows=max_rows)
-        self.handle = C.c_void_p()
-        _lib.check(self.lib.pg_create(C.byref(desc), C.byref(self.handle)))
-        try:
-            self._upload(state)
-        except Exception:
-            self.close()
-            raise
-
-    def _upload(self, state: dict):
-        cfg = self.config
         tensors = {k: v for k, v in state.items() if "rot_emb.inv_freq" not in k}
-        if cfg.arch == "esm2":
+        if config.arch == "esm2":
             inv = state["layers.0.self_attn.rot_emb.inv_freq"]
             cos, sin = rotary_tables(inv, 16384)  # rotary has no length limit in the reference; 16384 tokens covers every ProteinGym target (max 3423)
             tensors["rotary.cos"], tensors["rotary.sin"] = cos, sin
-        elif cfg.arch == "esmc":
+        elif config.arch == "esmc":
             tensors["rotary.cos"], tensors["rotary.sin"] = esmc_rotary_tables(1024)  # every ESM C window is <= 1024 tokens
-        # fp32 staging copy on the device (ESM-1v 2.6 GB, ESM2-3B 11 GB); the library repacks and we free it
-        gpu = [(n, t.to(self.device, torch.float32).contiguous()) for n, t in tensors.items()]
-        arr = (_lib.PgTensor * len(gpu))()
-        for i, (n, t) in enumerate(gpu):
-            arr[i].name = n.encode()
-            arr[i].data = t.data_ptr()
-            arr[i].shape[0] = t.shape[0]
-            arr[i].shape[1] = t.shape[1] if t.dim() == 2 else 1
-        torch.cuda.synchronize(self.device)
-        _lib.check(self.lib.pg_load_weights(self.handle, arr, len(gpu)), self.handle)
-        del gpu
-        torch.cuda.empty_cache()
-
-    def close(self):
-        if getattr(self, "handle", None) is not None and self.handle:
-            self.lib.pg_destroy(self.handle)
-            self.handle = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(desc, tensors, device)  # fp32 staging copy on the device: ESM-1v 2.6 GB, ESM2-3B 11 GB
 
     # ------------------------------------------------------------------------------------------------------------
     def masked_marginal_rows(self, tokens: torch.Tensor, positions, model_window: int = 1024) -> torch.Tensor:

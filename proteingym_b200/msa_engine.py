@@ -4,7 +4,6 @@ esm/data.py:300-336 MSABatchConverter). PyTorch is used for device memory and st
 """
 from __future__ import annotations
 
-import ctypes as C
 import itertools
 import random
 
@@ -14,7 +13,6 @@ import torch
 from . import _lib
 from .alphabet import ALPHABET
 from .checkpoint import EsmConfig
-from .esm_engine import PRECISIONS
 from .mutants import parse_mutants
 from .windows import optimal_window_starts
 
@@ -97,48 +95,17 @@ def default_max_rows(config: EsmConfig, R: int, Cw: int, np_planes: int = 2, bud
     return n * per_msa
 
 
-class MsaScorer:
+class MsaScorer(_lib.Model):
     def __init__(self, config: EsmConfig, state: dict, precision: str = "f16x3", device: int = 0, max_rows: int = 0):
-        if not torch.cuda.is_available():
-            raise _lib.PgError("no CUDA device: the H100 scorer has no CPU fallback")
         if config.arch != "msa":
             raise ValueError("MsaScorer needs an MSA Transformer configuration")
-        self.lib = _lib.load()
         self.config = config
-        self.device = torch.device("cuda", device)
         self.precision = precision
         self.max_rows = int(max_rows)
         desc = _lib.PgModelDesc(arch=_lib.PG_ARCH_MSA, layers=config.layers, embed_dim=config.embed_dim, heads=config.heads,
                                 ffn_dim=config.ffn_dim, vocab=config.vocab, max_positions=config.max_positions, token_dropout=0,
-                                emb_ln_before=1, precision=PRECISIONS[precision], device=device, max_rows=max_rows)
-        self.handle = C.c_void_p()
-        _lib.check(self.lib.pg_create(C.byref(desc), C.byref(self.handle)))
-        try:
-            gpu = [(n, t.to(self.device, torch.float32).contiguous()) for n, t in state.items()]
-            arr = (_lib.PgTensor * len(gpu))()
-            for i, (n, t) in enumerate(gpu):
-                arr[i].name = n.encode()
-                arr[i].data = t.data_ptr()
-                arr[i].shape[0] = t.shape[0]
-                arr[i].shape[1] = t.shape[1] if t.dim() == 2 else 1
-            torch.cuda.synchronize(self.device)
-            _lib.check(self.lib.pg_load_weights(self.handle, arr, len(gpu)), self.handle)
-            del gpu
-            torch.cuda.empty_cache()
-        except Exception:
-            self.close()
-            raise
-
-    def close(self):
-        if getattr(self, "handle", None) is not None and self.handle:
-            self.lib.pg_destroy(self.handle)
-            self.handle = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+                                emb_ln_before=1, precision=_lib.PRECISIONS[precision], device=device, max_rows=max_rows)
+        super().__init__(desc, state, device)
 
     # ------------------------------------------------------------------------------------------------------------
     def masked_marginal_rows(self, tokens: np.ndarray, positions, shard=None) -> torch.Tensor:

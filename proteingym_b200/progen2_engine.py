@@ -3,8 +3,8 @@
 ``calc_fitness`` (:34-86) cuts a protein into chunks of ``n_positions`` characters, and scores every chunk read left to right and
 reversed by the MEAN log-probability of its targets ``ids[1:]`` given ``ids[:-1]``, taken over the 25 amino-acid logits 5..29 only; a
 last target that is a terminal ('1' = 3 or '2' = 4) is dropped first. The protein's score is the sum over chunks and directions,
-divided by 2 and by len(prot). ``Progen2Scorer`` plans every distinct (chunk, direction) row once, through RITA's planner and prefix
-machinery (rita_engine.plan / ArScorer): a row that drops its last target is scored as the token row ids[:-1], which the causal
+divided by 2 and by len(prot). ``Progen2Scorer`` plans every distinct (chunk, direction) row once, through the shared decoder planner and
+prefix machinery (decoder.plan / ArScorer): a row that drops its last target is scored as the token row ids[:-1], which the causal
 decoder computes identically.
 """
 from __future__ import annotations
@@ -13,7 +13,7 @@ import numpy as np
 
 from . import _lib
 from .checkpoint import Progen2Config, progen2_rotary_tables
-from .rita_engine import PRECISIONS, ArScorer, plan
+from .decoder import ArScorer, plan
 
 FIRST_COL, LAST_COL = 5, 29  # compute_fitness.py:71: the scored logits
 TERMINALS = (3, 4)           # '1' / '2' (:63)
@@ -53,7 +53,7 @@ class Progen2Scorer(ArScorer):
         slot = 64 if conf.head_dim == 64 else 128
         desc = _lib.PgModelDesc(arch=_lib.PG_ARCH_PROGEN2, layers=conf.layers, embed_dim=conf.embed_dim, heads=conf.heads,
                                 ffn_dim=conf.ffn_dim, vocab=conf.vocab, max_positions=conf.n_positions, token_dropout=0, emb_ln_before=0,
-                                precision=PRECISIONS[precision], device=device, max_rows=max_rows)
+                                precision=_lib.PRECISIONS[precision], device=device, max_rows=max_rows)
         tensors = dict(state)
         tensors["rotary.cos"], tensors["rotary.sin"] = progen2_rotary_tables(conf.rotary_dim, slot, conf.n_positions)
         super().__init__(desc, tensors, device, head_vocab=LAST_COL - FIRST_COL + 1, label_off=FIRST_COL)

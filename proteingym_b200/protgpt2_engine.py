@@ -1,9 +1,9 @@
 """Host-side driver of the H100 ProtGPT2 scorer (reference: proteingym/baselines/protgpt2/compute_fitness.py).
 
-``calc_fitness`` (:13-43) cuts a protein into chunks of 1023 characters (RITA's chunking, rita_engine.chunks), and scores every chunk
+``calc_fitness`` (:13-43) cuts a protein into chunks of 1023 characters (RITA's chunking, decoder.chunks), and scores every chunk
 read left to right and reversed by the MEAN log-probability of the tokens ``encode(p)[1:]`` given ``encode(p)[:-1]``; GPT-2's tokenizer
 adds no special tokens. The protein's score is the sum over chunks and directions divided by 2 * n_chunks. ``Protgpt2Scorer`` plans every
-distinct (chunk, direction) row once through RITA's planner and ArScorer's wild-type prefix reuse: the first differing TOKEN decides the
+distinct (chunk, direction) row once through decoder.plan and ArScorer's wild-type prefix reuse: the first differing TOKEN decides the
 reusable prefix, which is exact for a causal decoder with absolute positions.
 """
 from __future__ import annotations
@@ -16,7 +16,7 @@ import numpy as np
 
 from . import _lib
 from .checkpoint import Protgpt2Config
-from .rita_engine import CONTEXT, PRECISIONS, ArScorer, plan
+from .decoder import CONTEXT, ArScorer, plan
 
 
 class Protgpt2Tokenizer:
@@ -121,7 +121,7 @@ class Protgpt2Scorer(ArScorer):
         self.conf, self.tok, self.context = conf, tokenizer, context
         desc = _lib.PgModelDesc(arch=_lib.PG_ARCH_PROTGPT2, layers=conf.layers, embed_dim=conf.embed_dim, heads=conf.heads,
                                 ffn_dim=conf.ffn_dim, vocab=conf.vocab, max_positions=conf.n_positions, token_dropout=0, emb_ln_before=0,
-                                precision=PRECISIONS[precision], device=device, max_rows=max_rows)
+                                precision=_lib.PRECISIONS[precision], device=device, max_rows=max_rows)
         super().__init__(desc, state, device)
 
     def score(self, prots, wt: str | None = None) -> np.ndarray:

@@ -4,11 +4,11 @@
 slice (``get_sequence_slices``, utils/scoring_utils.py:152-203), score every distinct slice left-to-right and on the reversed
 string (``get_tranception_scores_mutated_sequences``, :77-150), divide by the full sequence length, subtract the wild type
 scored in the same window, average the two directions, append the WT row. The forward + token log-likelihood runs in the
-CUDA library (``pg_ar_loglik``); pandas is used only for the same bookkeeping the reference does with it.
+CUDA library through the shared decoder driver (decoder.ArScorer: ragged batches, retrieval fusion, wild-type prefix reuse); pandas is
+used only for the same bookkeeping the reference does with it.
 """
 from __future__ import annotations
 
-import ctypes as C
 import json
 import math
 import os
@@ -18,6 +18,7 @@ import pandas as pd
 import torch
 
 from . import _lib
+from .decoder import CHUNK_ROWS, ArScorer, Fusion, prefix_split, reuse_plan
 
 VOCAB = ["[UNK]", "[CLS]", "[SEP]", "[PAD]", "[MASK]"] + list("ACDEFGHIKLMNPQRSTVWY")
 TOK = {t: i for i, t in enumerate(VOCAB)}
@@ -117,22 +118,6 @@ def replace_ambiguous(seq: str) -> str:
     return seq
 
 
-def prefix_split(x, w, offset: int = 1, tile: int = 128):
-    """Exact wild-type-prefix reuse in a causal decoder: for a sequence ``x`` and the wild type ``w`` it shares a prefix with (both strings
-    or token lists, in scoring order) -> (fd, start): fd = the token index of the first difference (``offset`` tokens precede element 0,
-    e.g. 1 for [CLS]) and start = fd rounded down to the attention tile, the first row the transformer has to run for ``x``."""
-    diff = next((k for k, (c, e) in enumerate(zip(x, w)) if c != e), len(x))
-    fd = offset + diff
-    return fd, (fd // tile) * tile
-
-
-def prefix_total(wt_csum, wt_rows, start: int, label: int, suffix_sum) -> np.float32:
-    """A sequence's summed log-likelihood recombined from its suffix pass (rows >= start) and the wild type's pass: rows < start - 1
-    predict shared tokens (``wt_csum[k]`` = sum of the wild type's rows 0 .. k-1), row start - 1 has the wild type's state but predicts
-    the sequence's own token ``label`` (``wt_rows`` [T, vocab]: the wild type's log-probability rows)."""
-    return np.float32(wt_csum[start - 1] + float(wt_rows[start - 1, label]) + float(suffix_sum))
-
-
 def prior_rows(prow, prow2, ws, we, msa_start, msa_end, flip, nonfocus=None):
     """Index arithmetic of the retrieval fusion for one sequence slice [ws, we) of the full protein (Tranception
     model_pytorch.py:811-830; TranceptEVE model_pytorch.py:1085-1133): fill ``prow`` (and ``prow2`` for the EVE table) with the prior
@@ -166,12 +151,10 @@ def prior_rows(prow, prow2, ws, we, msa_start, msa_end, flip, nonfocus=None):
             prow[ix] = -2
 
 
-class TranceptionScorer:
+class TranceptionScorer(ArScorer):
+    """Tranception on a pg_ar_* handle. Its token rows are residue strings, scored as ``[CLS] s [SEP]``."""
+
     def __init__(self, config: dict, state: dict, precision: str = "f16f8", device: int = 0, max_rows: int = 0):
-        if not torch.cuda.is_available():
-            raise _lib.PgError("no CUDA device: the H100 scorer has no CPU fallback")
-        self.lib = _lib.load()
-        self.device = torch.device("cuda", device)
         d, heads, layers = int(config["n_embd"]), int(config["n_head"]), int(config["n_layer"])
         ffn = int(config["n_inner"]) if config.get("n_inner") else 4 * d
         self.n_ctx = int(config.get("n_ctx", config.get("n_positions", 1024)))
@@ -182,103 +165,96 @@ class TranceptionScorer:
         self.vocab = int(config.get("vocab_size", 25))
         self.config = config
         desc = _lib.PgModelDesc(arch=_lib.PG_ARCH_TRANCEPTION, layers=layers, embed_dim=d, heads=heads, ffn_dim=ffn, vocab=self.vocab,
-                                max_positions=self.n_ctx, token_dropout=0, emb_ln_before=0,
-                                precision={"f16": _lib.PG_PREC_F16, "f16x3": _lib.PG_PREC_F16X3, "f16f8": _lib.PG_PREC_F16F8}[precision], device=device,
-                                max_rows=max_rows)
-        self.handle = C.c_void_p()
-        _lib.check(self.lib.pg_create(C.byref(desc), C.byref(self.handle)))
-        try:
-            tensors = {k: v for k, v in state.items() if "depthwiseconv" not in k}
-            for l in range(layers):
-                tensors[f"h.{l}.attn.conv_taps"] = conv_taps(state, l, heads)
-            tensors["alibi_slopes"] = torch.tensor(alibi_slopes(heads), dtype=torch.float32).view(-1, 1)
-            gpu = [(n, t.to(self.device, torch.float32).contiguous()) for n, t in tensors.items()]
-            arr = (_lib.PgTensor * len(gpu))()
-            for i, (n, t) in enumerate(gpu):
-                arr[i].name = n.encode()
-                arr[i].data = t.data_ptr()
-                arr[i].shape[0] = t.shape[0]
-                arr[i].shape[1] = t.shape[1] if t.dim() == 2 else 1
-            torch.cuda.synchronize(self.device)
-            _lib.check(self.lib.pg_load_weights(self.handle, arr, len(gpu)), self.handle)
-            del gpu
-        except Exception:
-            self.close()
-            raise
+                                max_positions=self.n_ctx, token_dropout=0, emb_ln_before=0, precision=_lib.PRECISIONS[precision],
+                                device=device, max_rows=max_rows)
+        tensors = {k: v for k, v in state.items() if "depthwiseconv" not in k}
+        for l in range(layers):
+            tensors[f"h.{l}.attn.conv_taps"] = conv_taps(state, l, heads)
+        tensors["alibi_slopes"] = torch.tensor(alibi_slopes(heads), dtype=torch.float32).view(-1, 1)
+        super().__init__(desc, tensors, device)
 
-    def close(self):
-        if getattr(self, "handle", None) is not None and self.handle:
-            self.lib.pg_destroy(self.handle)
-            self.handle = C.c_void_p()
+    def row_len(self, row) -> int:
+        return len(row) + 2
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def row_ids(self, rows, idx, T: int, start: int = 0) -> np.ndarray:
+        ids, _ = tokenize_batch([replace_ambiguous(rows[k]) for k in idx], T)
+        return np.ascontiguousarray(ids[:, start:])
+
+    def row_token(self, row, t: int) -> int:
+        return TOK.get(row[t - 1], 0)  # token t of [CLS] s [SEP] is character t - 1
+
+    def fusion(self, seqs, windows, flip, prior=None, alpha=0.6, msa_start=0, msa_end=None, prior2=None, beta=0.0, first_col=0,
+               nonfocus_fallback=False):
+        """The retrieval fusion of model_pytorch.py:806-830 (TranceptEVE: the three-way fusion, see ``prior_rows``) for the strings
+        ``seqs`` scored in ``windows`` [(start, end)] of the full protein; None without a prior."""
+        if prior is None:
+            return None
+        msa_end = prior.shape[0] if msa_end is None else msa_end
+        nonfocus = None
+        if prior2 is not None and nonfocus_fallback and beta > 0:  # rows whose EVE prior is -inf drag the fused value to -inf (:1118)
+            nonfocus = np.asarray(prior2)[:, 5:].min(axis=1) == -np.inf
+
+        def rows(k):
+            prow = np.full(len(seqs[k]) + 2, -1, dtype=np.int32)
+            prow2 = prow.copy() if prior2 is not None else None
+            prior_rows(prow, prow2, windows[k][0], windows[k][1], msa_start, msa_end, flip, nonfocus)
+            return prow, prow2
+
+        def dev(a):
+            return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(self.device) if a is not None else None
+        return Fusion(dev(prior), rows, float(alpha), dev(prior2), float(beta), int(first_col))
 
     # ------------------------------------------------------------------------------------------------------------
-    def sequence_logprobs(self, seqs, prior=None, windows=None, flip=False, alpha=0.6, msa_start=0, msa_end=None, chunk_rows=1 << 17,
+    def sequence_logprobs(self, seqs, prior=None, windows=None, flip=False, alpha=0.6, msa_start=0, msa_end=None, chunk_rows=CHUNK_ROWS,
                           prior2=None, beta=0.0, first_col=0, nonfocus_fallback=False, return_rows=False):
         """sum_t log p(tok_{t+1} | tok_<=t) of ``[CLS] s [SEP]`` for every string in ``seqs`` (float32 numpy).
         ``prior`` ([L_full, vocab] log-probabilities) with per-sequence ``windows`` [(start, end)] enables the retrieval
         fusion of model_pytorch.py:806-830; ``flip`` marks right-to-left scoring (the strings are already reversed).
         ``prior2`` / ``beta`` / ``first_col`` / ``nonfocus_fallback``: the TranceptEVE three-way fusion (see ``prior_rows``).
         ``return_rows``: also return, per sequence, the fused log-probabilities [len(s) + 1, vocab] of every predicted position."""
-        n = len(seqs)
-        out = np.zeros(n, dtype=np.float32)
-        rows_out = [None] * n
-        if n == 0:
-            return (out, rows_out) if return_rows else out
         # the reference tokenises with truncation=True, max_length=n_ctx (model_pytorch.py:930-938 -> scoring_utils.py:97-101): a
         # string longer than n_ctx - 2 residues (indel mode, sliding windows never produce one) is cut, [CLS] and [SEP] stay
         seqs = [s[:self.n_ctx - 2] for s in seqs]
-        order = np.argsort([len(s) for s in seqs], kind="stable")
+        fusion = self.fusion(seqs, windows, flip, prior, alpha, msa_start, msa_end, prior2, beta, first_col, nonfocus_fallback)
+        res = self.token_sums(seqs, fusion, return_rows, chunk_rows)
+        return (res[0].astype(np.float32), res[1]) if return_rows else res.astype(np.float32)
 
-        def dev32(a):
-            return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(self.device) if a is not None else None
+    # ------------------------------------------------------------------------------------------------------------
+    # Exact wild-type-prefix reuse (decoder.py). A mutant slice that has the same length as the wild type cut with the same window shares
+    # every token before its first change with it; with the attention tile of 128 rows, all rows before start = 128 * (first changed
+    # token // 128) are taken from ONE wild-type pass per window.
+    def reuse_policy(self, strings, windows, wts):
+        """Tranception's reuse policy for the strings of one direction, ``wts[i]`` the wild-type string scored in the same window as
+        strings[i] (or None) -> (rows, row_windows, plain, groups) for ArScorer.reuse_sums: ``rows`` = the strings followed by one wild-type
+        string per reused (wild type, window), the groups' partners. A string reuses its wild type when the two differ, have the same
+        length of more than 126 residues and no X/B/J/Z (those are re-drawn at random per call). A window pays for its extra wild-type pass
+        (T rows) only when its mutants skip clearly more rows than that (sum of starts >= 2 T); otherwise (e.g. proteins longer than the
+        context, where every mutant has its own window) its strings run whole."""
+        tile = self.PREFIX_TILE
+        key, start, saved = [None] * len(strings), [0] * len(strings), {}
+        for i, (x, w) in enumerate(zip(strings, wts)):
+            if (self.prefix_reuse and w is not None and x != w and len(x) == len(w) and len(x) + 2 > tile
+                    and not any(c in "XBJZ" for c in x) and not any(c in "XBJZ" for c in w)):
+                s = prefix_split(x, w, 1, tile)[1]          # token index of the first change is 1 + diff ([CLS] is token 0)
+                if s:
+                    key[i], start[i] = (w, windows[i]), s
+                    saved[key[i]] = saved.get(key[i], 0) + s
+        kept = [k for k, rows in saved.items() if rows >= 2 * (len(k[0]) + 2)]
+        partner = {k: len(strings) + j for j, k in enumerate(kept)}
+        start = [s if key[i] in partner else 0 for i, s in enumerate(start)]
+        plain, groups = reuse_plan(range(len(strings)), [partner.get(k) for k in key], start)
+        return list(strings) + [k[0] for k in kept], list(windows) + [k[1] for k in kept], plain, groups
 
-        d_prior, d_prior2 = dev32(prior), dev32(prior2)
-        msa_end = (prior.shape[0] if msa_end is None else msa_end) if prior is not None else None
-        nonfocus = None
-        if prior2 is not None and nonfocus_fallback and beta > 0:  # rows whose EVE prior is -inf drag the fused value to -inf (:1118)
-            nonfocus = np.asarray(prior2)[:, 5:].min(axis=1) == -np.inf
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        i = 0
-        while i < n:
-            # grow the chunk while the padded row count stays within budget (sequences are sorted by length)
-            j = i
-            while j < n and (j - i + 1) * (len(seqs[order[j]]) + 2) <= chunk_rows:
-                j += 1
-            j = max(j, i + 1)
-            idx = order[i:j]
-            T = len(seqs[idx[-1]]) + 2
-            ids, lens = tokenize_batch([replace_ambiguous(seqs[k]) for k in idx], T)
-            prow = np.full((len(idx), T), -1, dtype=np.int32) if prior is not None else None
-            prow2 = np.full((len(idx), T), -1, dtype=np.int32) if prior2 is not None else None
-            if prior is not None:
-                for r, k in enumerate(idx):
-                    prior_rows(prow[r], prow2[r] if prow2 is not None else None, windows[k][0], windows[k][1], msa_start, msa_end, flip, nonfocus)
-            d_ids = torch.from_numpy(ids).to(self.device)
-            d_lens = torch.from_numpy(lens).to(self.device)
-            d_prow = torch.from_numpy(prow).to(self.device) if prow is not None else None
-            d_prow2 = torch.from_numpy(prow2).to(self.device) if prow2 is not None else None
-            d_out = torch.empty(len(idx), dtype=torch.float32, device=self.device)
-            d_rows = torch.zeros((len(idx), T, self.vocab), dtype=torch.float32, device=self.device) if return_rows else None
-            f = _lib.PgArFusion(log_prior=d_prior.data_ptr() if d_prior is not None else None,
-                                prior_row=d_prow.data_ptr() if d_prow is not None else None, alpha=float(alpha),
-                                log_prior2=d_prior2.data_ptr() if d_prior2 is not None else None,
-                                prior_row2=d_prow2.data_ptr() if d_prow2 is not None else None, beta=float(beta),
-                                first_col=int(first_col), out_logprobs=d_rows.data_ptr() if d_rows is not None else None)
-            _lib.check(self.lib.pg_ar_loglik_fused(self.handle, d_ids.data_ptr(), d_lens.data_ptr(), len(idx), T, C.byref(f),
-                                                   d_out.data_ptr(), stream), self.handle)
-            out[idx] = d_out.cpu().numpy()
-            if return_rows:
-                h_rows = d_rows.cpu().numpy()
-                for r, k in enumerate(idx):
-                    rows_out[k] = h_rows[r, :lens[r] - 1]
-            i = j
-        return (out, rows_out) if return_rows else out
+    def _logprobs_with_reuse(self, strings, windows, wts, flip, prior_kw):
+        """``sequence_logprobs(strings, windows=windows, flip=flip, **prior_kw)`` with wild-type prefix reuse (``reuse_policy``); the strings
+        that run whole go through sequence_logprobs."""
+        rows, row_windows, plain, groups = self.reuse_policy(strings, windows, wts)
+        fusion = self.fusion(rows, row_windows, flip, **prior_kw) if groups else None
+
+        def plain_sums(idx):
+            return self.sequence_logprobs([strings[i] for i in idx], windows=[windows[i] for i in idx], flip=flip, **prior_kw)
+        out = self.reuse_sums(rows, range(len(strings)), plain, groups, fusion, plain_sums)
+        return out[:len(strings)].astype(np.float32)
 
     # ------------------------------------------------------------------------------------------------------------
     @staticmethod
@@ -320,135 +296,6 @@ class TranceptionScorer:
             raise ValueError(scoring_window)
         out = pd.DataFrame(recs, columns=["mutated_sequence", "sliced_mutated_sequence", "window_start", "window_end"])
         return out.drop_duplicates().reset_index(drop=True)
-
-    # ------------------------------------------------------------------------------------------------------------
-    # Exact wild-type-prefix reuse (include/pgscore.h: pg_ar_prefix_begin / pg_ar_loglik_prefix). A mutant slice that has the same
-    # length as the wild type cut with the same window shares every token before its first change with it; with the attention tile
-    # of 128 rows, all rows before start = 128 * (first_changed_token // 128) are taken from ONE wild-type pass per window.
-    prefix_reuse = os.environ.get("PG_PREFIX_REUSE", "1") != "0"
-    PREFIX_TILE = 128
-    reuse_rows = None  # [token rows a plain pass would run, token rows actually run], accumulated over calls (bench / tests)
-
-    def _logprobs_with_reuse(self, strings, windows, wts, flip, prior_kw):
-        """``sequence_logprobs(strings)`` where ``wts[i]`` is the wild-type string scored in the same window as strings[i] (or None).
-        Strings eligible for reuse are grouped by (wild type, start) and scored as suffixes; the rest take the plain path."""
-        n = len(strings)
-        out = np.zeros(n, dtype=np.float32)
-        tile = self.PREFIX_TILE
-        groups, plain = {}, []
-        for i, (x, w) in enumerate(zip(strings, wts)):
-            start = 0
-            if (self.prefix_reuse and w is not None and x != w and len(x) == len(w) and len(x) + 2 > tile
-                    and not any(c in "XBJZ" for c in x) and not any(c in "XBJZ" for c in w)):  # those are re-drawn at random per call
-                start = prefix_split(x, w, 1, tile)[1]          # token index of the first change is 1 + diff ([CLS] is token 0)
-            if start > 0:
-                groups.setdefault((w, windows[i], start), []).append(i)
-            else:
-                plain.append(i)
-        by_wt = {}
-        for (w, win, start), members in groups.items():
-            by_wt.setdefault((w, win), []).append((start, members))
-        # a window pays for its extra wild-type pass (T rows) only when its mutants skip clearly more rows than that; otherwise
-        # (e.g. proteins longer than the context, where every mutant has its own window) its members take the plain path
-        for key in list(by_wt):
-            T = len(key[0]) + 2
-            if sum(start * len(members) for start, members in by_wt[key]) < 2 * T:
-                plain += [i for _, members in by_wt.pop(key) for i in members]
-        plain.sort()
-        rows_full = sum(len(x) + 2 for x in strings)
-        rows_run = sum(len(strings[i]) + 2 for i in plain)
-        if plain:
-            out[plain] = self.sequence_logprobs([strings[i] for i in plain], windows=[windows[i] for i in plain], flip=flip, **prior_kw)
-        for (w, win), lst in by_wt.items():
-            rows_run += len(w) + 2
-            wt_tok, wt_rows = self._prefix_begin(w, win, flip, prior_kw)
-            csum = np.concatenate([[0.0], np.cumsum(wt_tok.astype(np.float64))])    # csum[k] = sum of rows 0 .. k-1
-            for start, members in sorted(lst):
-                rows_run += len(members) * (len(w) + 2 - start)
-                suffix = self._prefix_suffix([strings[i] for i in members], win, start, flip, prior_kw)
-                for i, sfx in zip(members, suffix):
-                    tok_s = TOK.get(strings[i][start - 1], 0)                         # token `start` of [CLS] x [SEP] is character start-1
-                    out[i] = prefix_total(csum, wt_rows, start, tok_s, sfx)
-        if self.reuse_rows is None:
-            self.reuse_rows = [0, 0]
-        self.reuse_rows[0] += rows_full
-        self.reuse_rows[1] += rows_run
-        return out
-
-    def _fusion(self, prior_kw, win, T, flip, n=1):
-        """(PgArFusion, keep-alive tensors, prow, prow2) for ``n`` identical rows of T tokens in window ``win``."""
-        prior, prior2 = prior_kw.get("prior"), prior_kw.get("prior2")
-        keep = []
-        if prior is None:
-            return None, keep, None, None
-        msa_start = prior_kw.get("msa_start", 0)
-        msa_end = prior_kw.get("msa_end")
-        msa_end = prior.shape[0] if msa_end is None else msa_end
-        beta = prior_kw.get("beta", 0.0)
-        nonfocus = None
-        if prior2 is not None and prior_kw.get("nonfocus_fallback") and beta > 0:
-            nonfocus = np.asarray(prior2)[:, 5:].min(axis=1) == -np.inf
-        prow = np.full((T,), -1, dtype=np.int32)
-        prow2 = np.full((T,), -1, dtype=np.int32) if prior2 is not None else None
-        prior_rows(prow, prow2, win[0], win[1], msa_start, msa_end, flip, nonfocus)
-        return (prior, prior2, beta), keep, prow, prow2
-
-    def _prefix_begin(self, wt, win, flip, prior_kw):
-        """Wild-type pass that records the prefix caches -> (token log-probs [T], fused rows [T, vocab]) as numpy."""
-        T = len(wt) + 2
-        ids, _ = tokenize_batch([replace_ambiguous(wt)], T)
-        d_ids = torch.from_numpy(ids).to(self.device)
-        meta, _, prow, prow2 = self._fusion(prior_kw, win, T, flip)
-        d_tok = torch.zeros(T, dtype=torch.float32, device=self.device)
-        d_rows = torch.zeros((T, self.vocab), dtype=torch.float32, device=self.device)
-        f, keep = self._fusion_struct(meta, prow[None] if prow is not None else None, prow2[None] if prow2 is not None else None, prior_kw, d_rows)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(self.lib.pg_ar_prefix_begin(self.handle, d_ids.data_ptr(), T, C.byref(f), d_tok.data_ptr(), stream), self.handle)
-        return d_tok.cpu().numpy(), d_rows.cpu().numpy()
-
-    def _fusion_struct(self, meta, prow, prow2, prior_kw, d_rows=None):
-        keep = []
-
-        def dev(a, dt):
-            t = torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(self.device)
-            keep.append(t)
-            return t
-        f = _lib.PgArFusion()
-        f.alpha = float(prior_kw.get("alpha", 0.6))
-        f.first_col = int(prior_kw.get("first_col", 0))
-        if meta is not None:
-            prior, prior2, beta = meta
-            f.log_prior = dev(prior, np.float32).data_ptr()
-            f.prior_row = dev(prow, np.int32).data_ptr()
-            if prior2 is not None:
-                f.log_prior2 = dev(prior2, np.float32).data_ptr()
-                f.prior_row2 = dev(prow2, np.int32).data_ptr()
-                f.beta = float(beta)
-        if d_rows is not None:
-            f.out_logprobs = d_rows.data_ptr()
-        return f, keep
-
-    def _prefix_suffix(self, seqs, win, start, flip, prior_kw, chunk_rows=1 << 17):
-        """Suffix sums (rows >= start) of equal-length strings sharing tokens 0 .. start-1 with the recorded wild type."""
-        T = len(seqs[0]) + 2
-        Ts = T - start
-        meta, _, prow, prow2 = self._fusion(prior_kw, win, T, flip)
-        out = np.zeros(len(seqs), dtype=np.float32)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        per = max(1, chunk_rows // Ts)
-        for i in range(0, len(seqs), per):
-            part = seqs[i:i + per]
-            ids, _ = tokenize_batch([replace_ambiguous(x) for x in part], T)
-            d_ids = torch.from_numpy(np.ascontiguousarray(ids[:, start:])).to(self.device)
-            d_lens = torch.full((len(part),), Ts, dtype=torch.int32, device=self.device)
-            pr = np.repeat(prow[None, start:], len(part), axis=0) if prow is not None else None
-            pr2 = np.repeat(prow2[None, start:], len(part), axis=0) if prow2 is not None else None
-            f, keep = self._fusion_struct(meta, pr, pr2, prior_kw)
-            d_out = torch.empty(len(part), dtype=torch.float32, device=self.device)
-            _lib.check(self.lib.pg_ar_loglik_prefix(self.handle, d_ids.data_ptr(), d_lens.data_ptr(), len(part), Ts, start, C.byref(f),
-                                                    d_out.data_ptr(), stream), self.handle)
-            out[i:i + len(part)] = d_out.cpu().numpy()
-        return out
 
     shard = None  # (rank, world) with an initialised torch.distributed group: split the sequence rows of each direction over the ranks
 
@@ -526,34 +373,6 @@ class TranceptionScorer:
             cols = [col, "avg_score_L_to_R", "avg_score_R_to_L", "avg_score"] if scoring_mirror else [col, "avg_score_L_to_R", "avg_score"]
             out = pd.concat([out, pd.DataFrame([[target_seq] + [0] * (len(cols) - 1)], columns=cols)], ignore_index=True)
         return out
-
-
-def prefix_reuse_plan(slices: pd.DataFrame, target_seq: str, tile: int = 128) -> pd.DataFrame:
-    """Planning aid for exact wild-type-prefix reuse (DESIGN.md §8.3; not used by the scorer yet). In a causal decoder every hidden
-    state of a mutant before its first changed token equals the wild type's, so with the WT scored in the same window
-
-        score(mutant) - score(WT) = [ lp_WT[fd-1, tok_m[fd]] - lp_WT[fd-1, tok_WT[fd]] ]            (row fd-1: same state, other label)
-                                   + sum_{t >= fd} lp_m[t, label_m[t]] - sum_{t >= fd} lp_WT[t, label_WT[t]]
-
-    where fd is the first token index at which the two ``[CLS] slice [SEP]`` strings differ and lp[t] the log-probability row that
-    predicts token t+1. Only rows >= fd need the transformer (keys / values of earlier rows come from the WT run). For every
-    (mutant slice, direction) this returns fd, the tile-aligned start the kernels would use, and the rows to compute, so the
-    saving can be read off an assay before any kernel exists. ``slices``: output of ``TranceptionScorer.slices`` (optimal windows)."""
-    wt_by_window = {(a, b): s for ms, s, a, b in zip(slices["mutated_sequence"], slices["sliced_mutated_sequence"], slices["window_start"],
-                                                    slices["window_end"]) if ms == target_seq}
-    recs = []
-    for ms, s, a, b in zip(slices["mutated_sequence"], slices["sliced_mutated_sequence"], slices["window_start"], slices["window_end"]):
-        if ms == target_seq:
-            continue
-        wt = wt_by_window.get((a, b))
-        if wt is None or len(wt) != len(s):
-            continue  # indels: no position-wise correspondence with a WT slice
-        T = len(s) + 2
-        for direction, x, y in (("L_to_R", s, wt), ("R_to_L", s[::-1], wt[::-1])):
-            fd, start = prefix_split(x, y, 1, tile)          # token index ([CLS] is token 0)
-            recs.append((ms, a, b, direction, T, fd, start, T - fd, T - start))
-    return pd.DataFrame(recs, columns=["mutated_sequence", "window_start", "window_end", "direction", "tokens", "first_diff_token",
-                                       "aligned_start", "rows_exact", "rows_tile_aligned"])
 
 
 def apply_substitutions(focus_seq: str, mutant: str, start_idx: int = 1) -> str:

@@ -23,7 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from proteingym_b200 import _lib, checkpoint, synth  # noqa: E402
 from proteingym_b200.protgpt2_engine import Protgpt2Scorer, Protgpt2Tokenizer  # noqa: E402
-from proteingym_b200.rita_engine import plan  # noqa: E402
+from proteingym_b200.decoder import plan  # noqa: E402
 
 TOK_DIR = os.path.join(ROOT, "tests", "golden", "protgpt2_tokenizer")
 

@@ -5,8 +5,11 @@ with --compare. A change that only moves device code between files must leave ev
     python scripts/check_refactor_bits.py --compare a.npz b.npz
 
 ESM-1v scores in f16x3 / f16f8 / f16d / f16, an ESM2 of the 35M release's shape (480 wide, 24-wide heads: the padded LayerNorm) in
-f16f8, Tranception mutant scores with and without prefix reuse and rows with a three-way retrieval fusion in f16x3 / f16f8, and a
-two-layer MSA Transformer table (a full and a pruned last layer) in f16x3 / f16f8."""
+f16f8, Tranception mutant scores with and without prefix reuse and rows with a three-way retrieval fusion in f16x3 / f16f8, a
+two-layer MSA Transformer table (a full and a pruned last layer) in f16x3 / f16f8, and RITA, ProGen2 and ProtGPT2 scores of a 900-residue
+wild type's substitutions and indels with and without prefix reuse in f16f8. Every run with prefix reuse also records its token-row
+counts (reuse_rows)."""
+import os
 import sys
 
 import numpy as np
@@ -44,6 +47,7 @@ def collect():
             sc.prefix_reuse = reuse
             df = sc.score_mutants(dms, wt)
             out[f"tranception.{mode}.reuse{int(reuse)}"] = df.select_dtypes("number").to_numpy()
+            out[f"tranception.{mode}.reuse{int(reuse)}.rows"] = np.asarray(sc.reuse_rows)
             sc.close()
         sc = TranceptionScorer(cfg, st, precision=mode)
         sums, rows = sc.sequence_logprobs([wt[:L]], prior=prior, windows=[(0, L)], alpha=0.6, msa_start=40, msa_end=L - 30, prior2=prior2,
@@ -60,6 +64,52 @@ def collect():
     for mode in ("f16x3", "f16f8"):
         sc = msa_engine.MsaScorer(cfg, st, precision=mode, max_rows=msa_engine.default_max_rows(cfg, R, Cc, want=4))
         out[f"msa.{mode}"] = sc.masked_marginal_rows(toks, pos).cpu().numpy()
+        sc.close()
+    out.update(decoders())
+    return out
+
+
+def decoders():
+    """RITA, ProGen2 and ProtGPT2 on seeded two-layer models: score() of substitutions (first change before and after token 128) and
+    indels of one wild type, with prefix reuse on and off."""
+    from proteingym_b200 import checkpoint, synth
+    from proteingym_b200.progen2_engine import Progen2Scorer
+    from proteingym_b200.protgpt2_engine import Protgpt2Scorer, Protgpt2Tokenizer
+    from proteingym_b200.rita_engine import RitaScorer, RitaTokenizer
+    golden = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
+    wt = synth.random_protein(900, 12)
+    prots = [synth.apply_mutant(wt, m) for m in synth.sample_mutants(wt, 48, 13, multi_frac=0.25)] + synth.random_indels(wt, 16, 14)
+
+    def rita():
+        arch = synth.RitaArch(2, 256, 4)
+        st = synth.make_rita_state(arch, 15)
+        ws = {k[len("transformer."):] if k.startswith("transformer.") else k: v for k, v in st.items()
+              if "inv_freq" not in k and k != "lm_head.weight"}
+        conf = checkpoint.RitaConfig(arch.layers, arch.embed_dim, arch.heads, arch.ffn_dim, arch.vocab, True)
+        return RitaScorer(conf, ws, st["transformer.layers.0.self_attention.rotary_embedding.inv_freq"],
+                          RitaTokenizer(os.path.join(golden, "rita_tokenizer_plain")), precision="f16f8")
+
+    def progen2():
+        a = synth.Progen2Arch(2, 512, 8, 32)
+        st = synth.make_progen2_state(a, 16, buffers=False)
+        ws = {k[len("transformer."):] if k.startswith("transformer.") else k: v for k, v in st.items()}
+        return Progen2Scorer(checkpoint.Progen2Config(a.layers, a.embed_dim, a.heads, a.ffn_dim, a.vocab, a.rotary_dim, a.n_positions), ws,
+                             precision="f16f8")
+
+    def protgpt2():
+        a = synth.Protgpt2Arch(2, 256, 4)
+        st = synth.make_protgpt2_state(a, 17)
+        ws = {k[len("transformer."):] if k.startswith("transformer.") else k: v for k, v in st.items() if k != "lm_head.weight"}
+        return Protgpt2Scorer(checkpoint.Protgpt2Config(a.layers, a.embed_dim, a.heads, a.ffn_dim, a.vocab, a.n_positions), ws,
+                              Protgpt2Tokenizer(os.path.join(golden, "protgpt2_tokenizer")), precision="f16f8")
+    out = {}
+    for name, make in (("rita", rita), ("progen2", progen2), ("protgpt2", protgpt2)):
+        sc = make()
+        for reuse in (True, False):
+            sc.prefix_reuse = reuse
+            sc.reuse_rows = [0, 0]
+            out[f"{name}.f16f8.reuse{int(reuse)}"] = sc.score(prots, wt=wt)
+            out[f"{name}.f16f8.reuse{int(reuse)}.rows"] = np.asarray(sc.reuse_rows)
         sc.close()
     return out
 

@@ -213,11 +213,12 @@ def test_cli_flag_surface_matches_reference(tag):
         assert mine[k] == v, k
 
 
-def test_prefix_reuse_identity_and_expected_saving():
-    """The identity behind exact wild-type-prefix reuse (DESIGN.md §8.3), checked with the oracle's CPU forward, and the row counts the
-    planner predicts for a config-4-like assay (L = 512 single substitutions)."""
+def test_prefix_reuse_identity_and_policy_saving():
+    """The identity behind exact wild-type-prefix reuse, checked with the oracle's CPU forward, and the row counts Tranception's reuse
+    policy plans for a config-4-like assay (L = 512 single substitutions)."""
     from oracle import tranception_oracle as O
-    from proteingym_b200.tranception_engine import TranceptionScorer, prefix_reuse_plan, tokenize
+    from proteingym_b200.decoder import prefix_split
+    from proteingym_b200.tranception_engine import TranceptionScorer, tokenize
     arch = synth.TranceptionArch(2, 128, 4, 256)
     st = synth.make_tranception_state(arch, 3)
     wt = synth.random_protein(40, 8)
@@ -234,16 +235,31 @@ def test_prefix_reuse_identity_and_expected_saving():
             tail = lambda r, t: sum(float(r[k, t[k + 1]]) for k in range(fd, len(t) - 1))  # noqa: E731
             delta = (float(rows_y[fd - 1, tx[fd]]) - float(rows_y[fd - 1, ty[fd]])) + tail(rows_x, tx) - tail(rows_y, ty)
             assert abs(delta - (tot_x - tot_y)) < 1e-4
-    # planner on a 512-residue protein with 400 random single substitutions
+    # the policy on a 512-residue protein with 400 random single substitutions, both directions
     seq = synth.random_protein(512, 1)
     muts = synth.sample_mutants(seq, 400, 2)
     df = pd.DataFrame({"mutant": muts, "mutated_sequence": [synth.apply_mutant(seq, m) for m in muts]})
     sc = TranceptionScorer.__new__(TranceptionScorer)
     sc.n_ctx = 1024
-    plan = prefix_reuse_plan(sc.slices(df, seq), seq)
-    assert len(plan) == 2 * len(muts) and (plan["tokens"] == 514).all()
-    exact, aligned = plan["rows_exact"].sum() / plan["tokens"].sum(), plan["rows_tile_aligned"].sum() / plan["tokens"].sum()
+    sl = sc.slices(df, seq)
+    is_mut = (sl["mutated_sequence"] != seq).to_numpy()
+    tokens = rows_exact = rows_aligned = 0
+    for rev in (False, True):
+        strings = [s[::-1] if rev else s for s in sl["sliced_mutated_sequence"]]
+        w = seq[::-1] if rev else seq
+        rows, _, plain, groups = sc.reuse_policy(strings, list(zip(sl["window_start"], sl["window_end"])), [w if m else None for m in is_mut])
+        assert rows[len(strings):] == [w] and list(groups) == [len(strings)]     # one window: one wild-type pass
+        start = dict.fromkeys(plain, 0)
+        start.update({r: s for s, members in groups[len(strings)].items() for r in members})
+        mut = np.flatnonzero(is_mut)
+        assert len(mut) == len(muts) and set(start) == set(range(len(strings)))
+        assert all(len(strings[i]) + 2 == 514 for i in mut)
+        fds = [prefix_split(strings[i], w, 1, 128)[0] for i in mut]
+        tokens += 514 * len(mut)
+        rows_exact += sum(514 - fd for fd in fds)
+        rows_aligned += sum(514 - start[i] for i in mut)
+        if not rev:
+            i0 = int(np.flatnonzero(sl["mutated_sequence"] == synth.apply_mutant(seq, muts[0]))[0])
+            assert fds[list(mut).index(i0)] == int(muts[0][1:-1])  # residue i (1-based) is token i
+    exact, aligned = rows_exact / tokens, rows_aligned / tokens
     assert 0.45 < exact < 0.55 and 0.55 < aligned < 0.70   # half the rows exactly; ~5/8 with 128-row tile alignment
-    lr = plan[plan.direction == "L_to_R"].set_index("mutated_sequence")
-    m0 = muts[0]
-    assert lr.loc[synth.apply_mutant(seq, m0), "first_diff_token"] == int(m0[1:-1])  # residue i (1-based) is token i

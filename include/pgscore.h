@@ -61,7 +61,7 @@ enum pg_arch {
                               slot width: column i < rotary_dim / 2 holds cos / sin(t * 10000^(-2i / rotary_dim)) in fp32 as
                               fixed_pos_embedding computes it (rotary_dim = head_dim when the config has none), later columns cos = 1,
                               sin = 0. ln_1 / ln_f use eps 1e-5. */
-  PG_ARCH_PROTGPT2 = 7     /* ProtGPT2 = GPT-2 large causal decoder (proteingym/baselines/protgpt2/compute_fitness.py; transformers
+  PG_ARCH_PROTGPT2 = 7,    /* ProtGPT2 = GPT-2 large causal decoder (proteingym/baselines/protgpt2/compute_fitness.py; transformers
                               modeling_gpt2.py GPT2LMHeadModel): learned absolute positions (wpe) added to the token embedding, pre-LN blocks
                               with c_attn / c_proj biases, causal attention without bias, tanh-GELU ("gelu_new") MLP (ffn_dim = n_inner or
                               4d), ln_f, and the head tied to wte: a log-softmax over all `vocab` columns (50 257) that runs as one
@@ -74,6 +74,17 @@ enum pg_arch {
                               "h.{i}.mlp.c_fc.{weight [d, ffn], bias}", "h.{i}.mlp.c_proj.{weight [ffn, d], bias}", "wte.weight" [vocab, d],
                               "wpe.weight" [max_positions, d], "ln_f.*"): Conv1D weights are [in, out] as for PG_ARCH_TRANCEPTION, and
                               no "lm_head.weight" (tied). LayerNorms use eps 1e-5. */
+  PG_ARCH_POET = 8         /* PoET (proteingym/baselines/PoET/poet/models/poet.py:687-730, modules/transformer.py TieredTransformerEncoderLayer):
+                              token embedding without positions; per layer x += self_attn(norm1 x) causal within each sequence, x +=
+                              multihead_attn(norm2 x) causal over the whole sequence of sequences, x += linear2(erf-GELU(linear1(norm3 x)));
+                              q/k/v without bias, out_proj with bias, interleaved rotary over 64-wide heads (positions restart at 0 in
+                              every sequence), then `norm` (LayerNorm, or identity when the state has no "norm.*") and the 24-way
+                              `linear` head with bias. vocab = 24 (Uniprot21 with gap, start 21, stop 22, mask 23), head_dim 64 only,
+                              PG_PREC_F16D refused; max_positions = the rotary table rows = the longest sequence a call may pass. Scored
+                              through pg_poet_context / pg_poet_loglik. Weights: the state-dict keys without "model." (
+                              "decoder.layers.{i}.{self_attn,multihead_attn}.{q,k,v}_proj.weight", "...out_proj.{weight,bias}",
+                              "decoder.layers.{i}.linear{1,2}.*", "decoder.layers.{i}.norm{1,2,3}.*", "token_embed.weight", "linear.*",
+                              optional "norm.*") plus "rotary.cos" / "rotary.sin" [T, 32] = cos / sin(t * inv_freq[2c]) in fp32. */
 };
 
 /* Tensor-core operand precision. The reference is strict fp32 (SURVEY.md §0.4). Every operand is an fp16 pair hi + lo.
@@ -210,6 +221,25 @@ int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int
 int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_fusion* f, float* out_tok_logp, pg_stream stream);
 int pg_ar_loglik_prefix(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t start,
                         const pg_ar_fusion* f, float* out_sum_logp, pg_stream stream);
+
+/* PoET scoring (PoET scripts/score.py get_logps_tiered_fast):
+ *   pg_poet_context: replaces model.embed of one sampled context. ids [sum seg_lens] int32 (device): the packed sequences, each
+ *                    <start> residues <stop>; seg_lens [n_seg] int32 (HOST). Keeps, per layer, the context's multi-sequence attention
+ *                    keys (rotated) and values in a record owned by the handle, replaced by the next call. n_seg = 0 records an empty
+ *                    context (the reference's memory=None path). The last layer stops once its keys and values are recorded.
+ *   pg_poet_loglik : replaces logits + CrossEntropyLoss(ignore_index = 23, reduction = "none") summed per row, against the current record.
+ *                    ids [B, T] int32 (device): right-padded rows; lens [B]: real tokens per row. out_sum_logp[b] = sum over t < lens[b]-1
+ *                    of log p(ids[b, t+1] | record, ids[b, <= t]), a next token 23 (mask) counting 0; out_tok_logp [B, T] (device, or
+ *                    NULL): the per-token terms (0 where ignored and at t >= lens[b]-1). Results do not depend on how rows are split
+ *                    into passes. */
+int pg_poet_context(pg_handle h, const int32_t* ids, const int32_t* seg_lens, int32_t n_seg, pg_stream stream);
+int pg_poet_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, float* out_sum_logp, float* out_tok_logp,
+                   pg_stream stream);
+/* The record of one layer as the library holds it, for checking: mem_T rows of the multi-attention q/k/v operand rows copied to `out`
+ * (device, pitch ld_bytes >= the row): fp16 [q | k | v] hi planes of d columns each, then (every mode but PG_PREC_F16) the fp16 lo
+ * planes in the same order; value = hi + lo. Within each 64-wide head the q/k columns hold the reference's dims (0, 2, .., 62,
+ * 1, 3, .., 63) (the rotary pairs on the slot pairs (i, 32 + i)). mem_T = the context length of the last pg_poet_context. */
+int pg_poet_record(pg_handle h, int32_t layer, void* out, int64_t ld_bytes, pg_stream stream);
 
 /* Replaces label_row over the whole DMS frame (compute_fitness.py:240-250, :505-514):
  *   score[m] = sum_{s in [row_offsets[m], row_offsets[m+1])} table[site_row[s], site_mt[s]] - table[site_row[s], site_wt[s]]

@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libpgscore.so")
 
 PG_ARCH_ESM1B, PG_ARCH_ESM2, PG_ARCH_TRANCEPTION, PG_ARCH_MSA, PG_ARCH_ESMC, PG_ARCH_RITA, PG_ARCH_PROGEN2 = 0, 1, 2, 3, 4, 5, 6
 PG_ARCH_PROTGPT2 = 7
+PG_ARCH_POET = 8
 PG_PREC_F16, PG_PREC_F16X3, PG_PREC_F16F8, PG_PREC_F16D = 0, 1, 2, 3
 PRECISIONS = {"f16": PG_PREC_F16, "f16x3": PG_PREC_F16X3, "f16f8": PG_PREC_F16F8, "f16d": PG_PREC_F16D}
 
@@ -73,6 +74,9 @@ SIGNATURES = {
     "pg_ar_prefix_begin": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(PgArFusion), C.c_void_p, C.c_void_p]),
     "pg_ar_loglik_prefix": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(PgArFusion),
                                       C.c_void_p, C.c_void_p]),
+    "pg_poet_context": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p]),
+    "pg_poet_loglik": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_poet_record": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "pg_gemm": (C.c_int, [C.POINTER(PgGemmArgs), C.c_void_p]),
     "pg_layernorm_f16": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                    C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]),

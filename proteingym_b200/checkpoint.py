@@ -464,3 +464,33 @@ def load_protgpt2_checkpoint(folder: str):
     if extra:
         raise ValueError(f"ProtGPT2 state dict: unexpected keys {extra[:5]}")
     return Protgpt2Config(layers, d, heads, ffn, vocab, npos), state
+
+
+@dataclass
+class PoetConfig:
+    layers: int
+    hidden_dim: int
+    heads: int
+    ff_dim: int
+    norm: bool
+
+
+def load_poet_checkpoint(path: str):
+    """PoET checkpoint (the layout PoET scripts/score.py reads) -> (PoetConfig, state). ``state`` has the key names of include/pgscore.h's
+    PG_ARCH_POET: ``state_dict`` with its first key component (``model.``) stripped, as fp32 CPU tensors (``norm.*`` only when
+    norm=True). ``hyper_parameters.model_spec.init_args`` gives the shapes. What the kernels do not implement is refused: head_dim other
+    than 64, use_multi_rotary=False and a vocabulary other than the 24 Uniprot21 tokens."""
+    import torch
+    ckpt = torch.load(path, map_location="cpu", weights_only=True)
+    a = ckpt["hyper_parameters"]["model_spec"]["init_args"]
+    d, heads = int(a.get("hidden_dim", 768)), int(a.get("nhead", 12))
+    conf = PoetConfig(layers=int(a.get("num_layers", 6)), hidden_dim=d, heads=heads, ff_dim=int(a.get("ff_dim") or 4 * d),
+                      norm=bool(a.get("norm", False)))
+    if int(a["n_vocab"]) != 24:
+        raise NotImplementedError(f"PoET n_vocab {a['n_vocab']}: the head and the tokenizer are the 24-token Uniprot21 alphabet")
+    if d % heads or d // heads != 64:
+        raise NotImplementedError(f"PoET head_dim {d / heads:g}: the attention kernels run 64-wide heads")
+    if not a.get("use_multi_rotary", True):
+        raise NotImplementedError("PoET use_multi_rotary=False: the multi-sequence attention is built with rotary positions")
+    state = {k.split(".", 1)[1]: v.float() for k, v in ckpt["state_dict"].items()}
+    return conf, state

@@ -214,11 +214,14 @@ OpFmt op_fmt(const pg_model_desc& D) {
 // h % (heads/8) of shard h / (heads/8). SL_PGQ / SL_PGK place its q / k rows with each rotate_every_two pair (2i, 2i+1) on the slot
 // pair (Sh + i, Sh + S/2 + i), i < hd/2, which turns the interleaved rotation into the epilogue's rotate-half; SL_PGV places v dim c
 // at Sh + c. For these maps n = d.
-enum SlotMap { SL_PAD = 0, SL_HEAD, SL_ROT, SL_PGQ, SL_PGK, SL_PGV };
+// SL_ILV (PoET q/k rows, hd == S == 64): the interleaved rotary pair (2i, 2i+1) of poet/models/modules/embedding.py's rotate_half on
+// the slot pair (Sh + i, Sh + S/2 + i), a row permutation that turns it into the epilogue's rotate-half.
+enum SlotMap { SL_PAD = 0, SL_HEAD, SL_ROT, SL_PGQ, SL_PGK, SL_PGV, SL_ILV };
 __device__ __forceinline__ int slot_src(int i, int map, int n, int hd, int S) {
   if (map == SL_PAD) return i < n ? i : -1;
   const int h = i / S, c = i % S, half = hd >> 1, hs = S >> 1;
   if (map == SL_HEAD) return c < hd ? h * hd + c : -1;
+  if (map == SL_ILV) return h * hd + (c < hs ? 2 * c : 2 * (c - hs) + 1);
   if (map == SL_ROT) {
     if (c < half) return h * hd + c;
     if (c >= hs && c < hs + half) return h * hd + half + (c - hs);
@@ -307,6 +310,14 @@ struct pg_handle_s {
   size_t base_alloc_bytes = 0;  // allocated for `base`
   int base_T = 0;
   __half* cq = nullptr;
+  // PoET (pg_poet_context / pg_poet_loglik): the context record, per layer the multi-sequence attention's q/k/v rows of the context
+  // ([layers][mem_T][3da*np] fp16; the rotated k and the v columns are read), regrown on demand (not in `allocs`); rotary positions and
+  // segment starts of the context rows [max_rows]; whether the head has its LayerNorm (norm=True)
+  __half* mem = nullptr;
+  size_t mem_bytes = 0;
+  int mem_T = -1;  // rows of the current record; -1 = none, 0 = an empty context
+  int32_t *ctx_pos = nullptr, *ctx_seg = nullptr;
+  bool head_norm = false;
 };
 
 namespace pg {
@@ -376,13 +387,16 @@ GemmLaunch proj_gemm(pg_handle h, const Layer& L, Proj p, const __half* a, float
   }
   g.a = a; g.lda = static_cast<int64_t>(g.K) * h->op.np; g.ldw = g.lda; g.M = M; g.nseg = h->op.nseg;
   g.a_scale = a_scale; g.w_uniform = 1;  // pg_load_weights: one e4m3 scale per (fused) weight matrix
+  // PoET's score is a SUM over every target, so the tensor core's truncating accumulation must stay short: 64-element chunks (at most
+  // MAX_SEGS - 2 pieces) took the 12 x 1024 golden from 1.3e-3 to 2.0e-4 (DESIGN.md §2)
+  if (h->desc.arch == PG_ARCH_POET) g.kchunk = 64;
   return g;
 }
 // ... written as operand rows to `out` through epilogue `epi`: q/k/v in the q/k/v format (epi 0, or 3: rotary embedding over windows of
 // rot_T rows, row t of a window at position rot_start + t), fc1 in the GEMM-input format (epi: the MLP's activation, out_scale: the e4m3
 // scale of its output; SwiGLU, epi 5, writes half as many columns as the GEMM has).
 int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int M, __half* out, cudaStream_t s, int epi = 0,
-        float out_scale = 0.f, int rot_T = 0, int rot_start = 0) {
+        float out_scale = 0.f, int rot_T = 0, int rot_start = 0, const int32_t* rot_pos = nullptr) {
   GemmLaunch g = proj_gemm(h, L, p, a, a_scale, M);
   const int n_out = epi == 5 ? g.N / 2 : g.N;
   g.epi = epi;
@@ -391,7 +405,7 @@ int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int
   if (epi == 3) {  // q and k slots; tables [T, S/2]
     const int hs = h->op.slot / 2;
     g.rot_cos = h->rot_cos + static_cast<int64_t>(rot_start) * hs; g.rot_sin = h->rot_sin + static_cast<int64_t>(rot_start) * hs;
-    g.rot_T = rot_T; g.rot_dim = h->op.da; g.rot_half = hs;
+    g.rot_T = rot_T; g.rot_dim = h->op.da; g.rot_half = hs; g.rot_pos = rot_pos;
   }
   ProfScope ps(p, s);
   return launch_gemm(g, s);
@@ -866,6 +880,70 @@ int ar_passes(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T
   return PG_OK;
 }
 
+// PoET (poet/models/poet.py:687-730, modules/transformer.py TieredTransformerEncoderLayer): per layer x += out(self_attn(norm1 x)),
+// causal within each sequence; x += out(multihead_attn(norm2 x)), causal over the sequence of sequences; x += linear2(gelu(linear1(
+// norm3 x))). h->layers[l] holds self_attn (ln1 = norm1), linear1 / linear2 (ln2 = norm3); h->col_layers[l] multihead_attn (ln1 = norm2).
+// Rotary positions restart at 0 in every sequence.
+
+// The context: Tm packed rows, row t at position ctx_pos[t] of the segment that starts at ctx_seg[t]. Each layer's multihead_attn
+// q/k/v rows go straight into the record; the last layer stops there (its multi-attention output, MLP and the head are never read).
+int forward_poet_context(pg_handle h, const int32_t* ids, int Tm, cudaStream_t s) {
+  const pg_model_desc& D = h->desc;
+  const size_t ldq = static_cast<size_t>(h->op.ldq);
+  int rc;
+  { ProfScope ps(CAT_EMBED, s);
+    rc = launch_gather_embed(ids, h->embed, Tm, D.embed_dim, D.vocab, h->x, s); }
+  if (rc) return rc;
+  for (int l = 0; l < D.layers; ++l) {
+    const Layer& L = h->layers[l];
+    const Layer& C = h->col_layers[l];
+    if ((rc = ln(h, h->x, L.ln1g, L.ln1b, Tm, h->abuf, s))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, Tm, h->qkv, s, 3, 0.f, 1, 0, h->ctx_pos))) return rc;
+    AttnLaunch a = attn_args(h, h->qkv, h->abuf, 1, Tm);
+    a.causal = 1; a.seg_start = h->ctx_seg;
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
+    if (rc || (rc = lin_add(h, L, OUT, h->abuf, S_ATT, Tm, h->x, s))) return rc;
+    __half* mem = h->mem + static_cast<size_t>(l) * Tm * ldq;
+    if ((rc = ln(h, h->x, C.ln1g, C.ln1b, Tm, h->abuf, s))) return rc;
+    if ((rc = lin(h, C, QKV, h->abuf, S_LN, Tm, mem, s, 3, 0.f, 1, 0, h->ctx_pos))) return rc;
+    if (l + 1 == D.layers) break;
+    a = attn_args(h, mem, h->abuf, 1, Tm);
+    a.causal = 1;
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
+    if (rc || (rc = lin_add(h, C, OUT, h->abuf, S_ATT, Tm, h->x, s))) return rc;
+    if ((rc = mlp(h, L, h->x, Tm, h->abuf, h->fbuf, 1, S_GELU, s))) return rc;
+  }
+  return PG_OK;
+}
+
+// B variant rows of T tokens (positions 0 .. T-1) against the record: the multi-attention keys of a row are the mem_T record rows, all
+// visible, then its own rows up to itself (flash-attn varlen's bottom-right causal alignment).
+int forward_poet_rows(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s) {
+  const pg_model_desc& D = h->desc;
+  const int rows = B * T;
+  const size_t ldq = static_cast<size_t>(h->op.ldq);
+  int rc;
+  { ProfScope ps(CAT_EMBED, s);
+    rc = launch_gather_embed(ids, h->embed, rows, D.embed_dim, D.vocab, h->x, s); }
+  if (rc) return rc;
+  for (int l = 0; l < D.layers; ++l) {
+    const Layer& L = h->layers[l];
+    const Layer& C = h->col_layers[l];
+    for (int k = 0; k < 2; ++k) {
+      const Layer& A = k ? C : L;
+      if ((rc = ln(h, h->x, A.ln1g, A.ln1b, rows, h->abuf, s))) return rc;
+      if ((rc = lin(h, A, QKV, h->abuf, S_LN, rows, h->qkv, s, 3, 0.f, T, 0))) return rc;
+      AttnLaunch a = attn_args(h, h->qkv, h->abuf, B, T);
+      a.causal = 1;
+      if (k && h->mem_T > 0) { a.prefix = h->mem + static_cast<size_t>(l) * h->mem_T * ldq; a.prefix_len = h->mem_T; a.prefix_mem = 1; }
+      { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
+      if (rc || (rc = lin_add(h, A, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
+    }
+    if ((rc = mlp(h, L, h->x, rows, h->abuf, h->fbuf, 1, S_GELU, s))) return rc;
+  }
+  return PG_OK;
+}
+
 }  // namespace
 }  // namespace pg
 
@@ -940,8 +1018,11 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
   }
   if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC &&
-      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2 && D.arch != PG_ARCH_PROTGPT2)
+      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2 && D.arch != PG_ARCH_PROTGPT2 && D.arch != PG_ARCH_POET)
     return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
+  if (D.arch == PG_ARCH_POET && D.vocab != 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: PoET needs the 24-token Uniprot21 vocabulary");
+  if (D.arch == PG_ARCH_POET && D.max_positions <= 0)
+    return set_error(PG_ERR_ARG, "pg_create: PoET needs max_positions = the rotary table rows (the longest sequence of a context or variant)");
   if (D.arch == PG_ARCH_ESMC && D.heads > 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: the ESM C q/k LayerNorm kernel holds at most 24 heads");
   if (D.arch == PG_ARCH_TRANCEPTION && D.heads % 4) return set_error(PG_ERR_UNSUPPORTED, "pg_create: Tranception needs heads % 4 == 0 (model_pytorch.py:129-131)");
   if (D.precision != PG_PREC_F16 && D.precision != PG_PREC_F16X3 && D.precision != PG_PREC_F16F8 && D.precision != PG_PREC_F16D)
@@ -973,14 +1054,27 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   for (auto& L : h->layers) {
     A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
     A(&L.w1, static_cast<size_t>(f1) * dk * np); A(&L.w2, static_cast<size_t>(d) * f * np);
-    if (!esmc && D.arch != PG_ARCH_PROGEN2) { A(&L.bqkv, 3 * da); A(&L.bo, d); }  // ESM C and ProGen2 attention: no bias (null = none)
+    if (!esmc && D.arch != PG_ARCH_PROGEN2) {  // ESM C and ProGen2 attention: no bias (null = none); PoET: out_proj only
+      if (D.arch != PG_ARCH_POET) A(&L.bqkv, 3 * da);
+      A(&L.bo, d);
+    }
     if (!esmc) { A(&L.b1, f); A(&L.b2, d); }  // ESM C MLP: no bias
     A(&L.ln1g, d); A(&L.ln1b, d); A(&L.ln2g, d); A(&L.ln2b, d);
     if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); A(&L.i1, f1); A(&L.i2, d); }
     if (D.arch == PG_ARCH_TRANCEPTION) A(&L.conv_taps, 3 * 4 * 64 * 8);
     if (esmc) { A(&L.qlng, d); A(&L.klng, d); }
   }
-  if (esmc || D.arch == PG_ARCH_RITA || D.arch == PG_ARCH_PROGEN2) A(&h->outw, static_cast<size_t>(D.vocab) * d);
+  if (esmc || D.arch == PG_ARCH_RITA || D.arch == PG_ARCH_PROGEN2 || D.arch == PG_ARCH_POET) A(&h->outw, static_cast<size_t>(D.vocab) * d);
+  if (D.arch == PG_ARCH_POET) {  // multihead_attn blocks; context positions and segment starts
+    h->col_layers.resize(D.layers);
+    for (auto& L : h->col_layers) {
+      A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
+      A(&L.bo, d); A(&L.ln1g, d); A(&L.ln1b, d);
+      if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); }
+    }
+    A(&h->ctx_pos, static_cast<size_t>(h->max_rows)); A(&h->ctx_seg, static_cast<size_t>(h->max_rows));
+    A(&h->tok_logp, static_cast<size_t>(h->max_rows));
+  }
   if (D.arch == PG_ARCH_MSA) {
     h->col_layers.resize(D.layers);
     for (auto& L : h->col_layers) {
@@ -1033,6 +1127,7 @@ int pg_destroy(pg_handle h) {
   for (void* p : h->allocs) cudaFree(p);
   if (h->tied_ws) cudaFree(h->tied_ws);
   if (h->base) cudaFree(h->base);
+  if (h->mem) cudaFree(h->mem);
   delete h;
   return PG_OK;
 }
@@ -1090,7 +1185,7 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
   // A [n_src, k_src] source weight placed in the padded operand layout [N, K] (OpFmt, slot maps rmap / cmap), in a scratch buffer
   // freed on return; the source itself when the layout is unpadded. The ProGen2 maps read rows of the fused [3d, d] qkv_proj.
   auto slots = [&](const float* w, int n_src, int k_src, int N, int K, int rmap, int cmap) -> const float* {
-    if (!w || (N == n_src && K == k_src)) return w;
+    if (!w || (N == n_src && K == k_src && rmap != SL_ILV)) return w;
     float* p = nullptr;
     const cudaError_t e = cudaMalloc(&p, static_cast<size_t>(N) * K * sizeof(float));
     if (e != cudaSuccess) {
@@ -1225,6 +1320,41 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     copy(h->pos, get("wpe.weight", D.max_positions, d), static_cast<size_t>(D.max_positions) * d);
     copy(h->lnag, get("ln_f.weight", d, 1), d);
     copy(h->lnab, get("ln_f.bias", d, 1), d);
+  } else if (D.arch == PG_ARCH_POET) {
+    // PoET names (poet/models/poet.py without the checkpoint's "model." prefix). q, k and v of each attention form one GEMM operand
+    // without bias, the q rows scaled by 1/sqrt(64) = 0.125 (flash-attn's default softmax scale; exact), the q and k rows permuted by
+    // SL_ILV. norm=False checkpoints carry no "norm.*": the head then reads the residual stream directly.
+    auto attn = [&](Layer& L, const std::string& pa, const std::string& pn) {
+      const float* wq = slots(get(pa + "q_proj.weight", d, d), d, d, d, d, SL_ILV, SL_PAD);
+      const float* wk = slots(get(pa + "k_proj.weight", d, d), d, d, d, d, SL_ILV, SL_PAD);
+      pack(L.wqkv, L.iqkv, {{wq, 0.125f}, wk, get(pa + "v_proj.weight", d, d)}, d, d);
+      pack(L.wo, L.io, {get(pa + "out_proj.weight", d, d)}, d, d);
+      copy(L.bo, get(pa + "out_proj.bias", d, 1), d);
+      copy(L.ln1g, get(pn + ".weight", d, 1), d);
+      copy(L.ln1b, get(pn + ".bias", d, 1), d);
+    };
+    for (int l = 0; l < D.layers; ++l) {
+      Layer& L = h->layers[l];
+      const std::string p = "decoder.layers." + std::to_string(l) + ".";
+      attn(L, p + "self_attn.", p + "norm1");
+      attn(h->col_layers[l], p + "multihead_attn.", p + "norm2");
+      pack(L.w1, L.i1, {get(p + "linear1.weight", f, d)}, f, d);
+      copy(L.b1, get(p + "linear1.bias", f, 1), f);
+      pack(L.w2, L.i2, {get(p + "linear2.weight", d, f)}, d, f);
+      copy(L.b2, get(p + "linear2.bias", d, 1), d);
+      copy(L.ln2g, get(p + "norm3.weight", d, 1), d);
+      copy(L.ln2b, get(p + "norm3.bias", d, 1), d);
+    }
+    copy(h->embed, get("token_embed.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    copy(h->outw, get("linear.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
+    copy(h->hbias, get("linear.bias", D.vocab, 1), D.vocab);
+    h->head_norm = by_name.count("norm.weight") > 0;
+    if (h->head_norm) {
+      copy(h->lnag, get("norm.weight", d, 1), d);
+      copy(h->lnab, get("norm.bias", d, 1), d);
+    }
+    if (int rc = rotary32()) return rc;
+    if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
   } else if (D.arch == PG_ARCH_PROGEN2) {
     // HF names without the "transformer." prefix (modeling_progen.py:84-95, 209-226, 389-401, 541-548). qkv_proj [3d, d] is placed
     // into the head slots by SL_PGQ / SL_PGK / SL_PGV (one GEMM operand, no bias) with head_dim^-1/2 folded into the q rows: exact
@@ -1528,6 +1658,79 @@ int pg_ar_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B
   pg_ar_fusion f = {};
   f.log_prior = log_prior; f.prior_row = prior_row; f.alpha = alpha;
   return pg_ar_loglik_fused(h, ids, lens, B, T, &f, out_sum_logp, stream);
+}
+
+int pg_poet_context(pg_handle h, const int32_t* ids, const int32_t* seg_lens, int32_t n_seg, pg_stream stream) {
+  if (!h) return set_error(PG_ERR_ARG, "pg_poet_context: null handle");
+  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_poet_context: weights not loaded");
+  if (h->desc.arch != PG_ARCH_POET) return fail(h, PG_ERR_STATE, "pg_poet_context: handle is not a PoET model");
+  if (n_seg < 0 || (n_seg > 0 && (!ids || !seg_lens))) return fail(h, PG_ERR_ARG, "pg_poet_context: bad arguments");
+  std::vector<int32_t> pos, seg;
+  for (int i = 0; i < n_seg; ++i) {
+    if (seg_lens[i] <= 0 || seg_lens[i] > h->rot_rows) return fail(h, PG_ERR_ARG, "pg_poet_context: segment length outside 1 .. max_positions");
+    const int32_t start = static_cast<int32_t>(pos.size());
+    for (int t = 0; t < seg_lens[i]; ++t) { pos.push_back(t); seg.push_back(start); }
+    if (static_cast<long long>(pos.size()) > h->max_rows) return fail(h, PG_ERR_ARG, "pg_poet_context: context longer than the workspace (max_rows)");
+  }
+  const int Tm = static_cast<int>(pos.size());
+  PG_CUDA_OK(cudaSetDevice(h->desc.device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  h->mem_T = -1;
+  if (Tm == 0) { h->mem_T = 0; return PG_OK; }
+  const size_t need = static_cast<size_t>(h->desc.layers) * Tm * h->op.ldq * sizeof(__half);
+  if (need > h->mem_bytes) {
+    PG_CUDA_OK(cudaStreamSynchronize(s));  // the old record may still be read by work queued on s
+    if (h->mem) cudaFree(h->mem);
+    h->mem = nullptr; h->mem_bytes = 0;
+    PG_CUDA_OK(cudaMalloc(&h->mem, need));
+    h->mem_bytes = need;
+  }
+  PG_CUDA_OK(cudaMemcpyAsync(h->ctx_pos, pos.data(), Tm * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  PG_CUDA_OK(cudaMemcpyAsync(h->ctx_seg, seg.data(), Tm * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  PG_CUDA_OK(cudaStreamSynchronize(s));  // pos / seg are pageable host vectors
+  const int rc = forward_poet_context(h, ids, Tm, s);
+  if (rc) return fail(h, rc, tls_error());
+  h->mem_T = Tm;
+  return PG_OK;
+}
+
+int pg_poet_record(pg_handle h, int32_t layer, void* out, int64_t ld_bytes, pg_stream stream) {
+  if (!h) return set_error(PG_ERR_ARG, "pg_poet_record: null handle");
+  if (h->desc.arch != PG_ARCH_POET || h->mem_T < 0) return fail(h, PG_ERR_STATE, "pg_poet_record: no PoET context recorded");
+  if (layer < 0 || layer >= h->desc.layers || !out) return fail(h, PG_ERR_ARG, "pg_poet_record: bad layer or null buffer");
+  const size_t row = static_cast<size_t>(h->op.ldq) * sizeof(__half);
+  if (ld_bytes < static_cast<int64_t>(row)) return fail(h, PG_ERR_ARG, "pg_poet_record: pitch shorter than a record row");
+  if (h->mem_T == 0) return PG_OK;
+  PG_CUDA_OK(cudaSetDevice(h->desc.device));
+  PG_CUDA_OK(cudaMemcpy2DAsync(out, ld_bytes, h->mem + static_cast<size_t>(layer) * h->mem_T * h->op.ldq, row, row, h->mem_T,
+                               cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+  return PG_OK;
+}
+
+int pg_poet_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, float* out_sum_logp, float* out_tok_logp,
+                   pg_stream stream) {
+  if (!h) return set_error(PG_ERR_ARG, "pg_poet_loglik: null handle");
+  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_poet_loglik: weights not loaded");
+  if (h->desc.arch != PG_ARCH_POET) return fail(h, PG_ERR_STATE, "pg_poet_loglik: handle is not a PoET model");
+  if (h->mem_T < 0) return fail(h, PG_ERR_STATE, "pg_poet_loglik: no context recorded (call pg_poet_context first)");
+  if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_poet_loglik: bad B/T");
+  if (B == 0) return PG_OK;
+  if (!ids || !lens || !out_sum_logp) return fail(h, PG_ERR_ARG, "pg_poet_loglik: null buffer");
+  if (T > h->rot_rows || T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_poet_loglik: rows longer than max_positions / the workspace");
+  PG_CUDA_OK(cudaSetDevice(h->desc.device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long per = balanced_per(B, h->max_rows / T);
+  for (int b0 = 0; b0 < B; b0 += static_cast<int>(per)) {
+    const int Bc = (B - b0) < per ? (B - b0) : static_cast<int>(per);
+    const long long off = static_cast<long long>(b0) * T;
+    int rc = forward_poet_rows(h, ids + off, Bc, T, s);
+    if (rc) return fail(h, rc, tls_error());
+    ProfScope ps(CAT_HEAD, s, 2);
+    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->head_norm ? h->lnag : nullptr, h->lnab,
+                        h->outw, h->hbias, 0, ArFusion{}, out_tok_logp ? out_tok_logp + off : h->tok_logp, out_sum_logp + b0, s, 23);
+    if (rc) return fail(h, rc, tls_error());
+  }
+  return PG_OK;
 }
 
 int pg_score_mutants(const float* table, int32_t n_rows, int32_t vocab, const int32_t* site_row, const int32_t* site_wt,

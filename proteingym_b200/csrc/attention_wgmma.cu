@@ -44,6 +44,9 @@ struct AttnWParams {
   int perm_C;                    // > 0: sequence b is column (b / perm_C, b % perm_C) of an alignment; output rows go to (., r, c) order
   // delta-operand mode (common.h AttnLaunch): out = attention - base_o[row]; full-precision hi / lo copy of row mask_pos[b] to cout[b]
   const __half* base_o; const int* mask_pos; __half* cout; long long ldc; long long c_lo_off;
+  int p_valid;            // prefix rows that exist (keys [p_valid, s_blocks * 64) are masked): s_blocks * 64 except in the memory form
+  int head_major;         // work items ordered (head, sequence, tile) instead of (sequence, head, tile)
+  const int* seg_start;   // segment-causal form (B == 1): first row of each row's segment, or null
 };
 
 __device__ __forceinline__ float ex2a(float x) {
@@ -52,7 +55,10 @@ __device__ __forceinline__ float ex2a(float x) {
   return y;
 }
 
-template <int NP, int DELTA, int HD>
+// RNACC (memory form): each key block's P V goes to a fresh accumulator that is added to O in round-to-nearest fp32, as the GEMM's K
+// chunks are (gemm_tc.cu): the tensor core's own fp32 accumulation does not round to nearest, and over the ~385 key blocks of a 24 640-row
+// record its error grows with the number of blocks.
+template <int NP, int DELTA, int HD, int RNACC = 0>
 __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tm,
                                                                  const __grid_constant__ CUtensorMap tmP, const AttnWParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -71,13 +77,17 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
   const int item = blockIdx.x;
   const int qt_l = item % p.nqt, bh = item / p.nqt;
   const int qt = qt_l + p.s_blocks;  // tile index within the full sequence
-  const int h = bh % p.heads, b = bh / p.heads;
+  const int nb = p.B;
+  const int h = p.head_major ? bh / nb : bh % p.heads, b = p.head_major ? bh % nb : bh / p.heads;
   const int row0 = b * p.Tq;
   const int cq = h * HD, ck = p.d + h * HD, cv = 2 * p.d + h * HD;
-  const int nkb = p.causal ? min(qt + 1, p.nkb) : p.nkb;  // causal: query tile qt needs key blocks 0 .. qt
+  // segment-causal: the tile's first row has the smallest segment start; blocks before it hold no visible key
+  const int j0 = p.seg_start ? __ldg(p.seg_start + qt_l * QT) / KT : 0;
+  const int nkb = (p.causal ? min(qt + 1, p.nkb) : p.nkb) - j0;  // causal: query tile qt needs key blocks 0 .. qt
 
-  auto load_block = [&](int j) {  // K and V of key block j of the full sequence: shared prefix rows or this sequence's own rows
-    const int slot = j % NSLOT;
+  auto load_block = [&](int i) {  // K and V of key block j0 + i of the full sequence: shared prefix rows or this sequence's own rows
+    const int j = j0 + i;
+    const int slot = i % NSLOT;
     mbar_arrive_expect_tx(&kv_full[slot], 2 * NP * PLANE);
     const CUtensorMap* src = j < p.s_blocks ? &tmP : &tm;
     const int r = j < p.s_blocks ? j * KT : row0 + (j - p.s_blocks) * KT;
@@ -106,6 +116,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
   constexpr float LOG2E = 1.4426950408889634f;
   const float slope2 = slope * LOG2E;
   const int qrow = qt * QT + warp * 16 + g;  // this thread's rows qrow and qrow + 8 (full-sequence index)
+  int sq[2] = {0, 0};                        // segment-causal: first visible key of rows qrow, qrow + 8
+  if (p.seg_start)
+    for (int r = 0; r < 2; ++r) sq[r] = qrow + 8 * r < p.T ? __ldg(p.seg_start + qrow + 8 * r) : 0;
+  const int pad0 = p.p_valid, pad1 = p.s_blocks * KT;  // masked prefix rows [pad0, pad1) of the memory form
   float o[NB][32];  // o[bx]: head-dim columns [64 bx, 64 bx + 64)
 #pragma unroll
   for (int bx = 0; bx < NB; ++bx)
@@ -115,9 +129,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
   const uint32_t q_addr = smem_u32(sQ);
   mbar_wait(q_full, 0);
 
-  for (int j = 0; j < nkb; ++j) {
-    const int slot = j % NSLOT;
-    mbar_wait(&kv_full[slot], (j / NSLOT) & 1);
+  for (int i = 0; i < nkb; ++i) {
+    const int j = j0 + i;
+    const int slot = i % NSLOT;
+    mbar_wait(&kv_full[slot], (i / NSLOT) & 1);
     const uint32_t k_addr = smem_u32(sKV) + slot * 2 * NP * PLANE;
     const uint32_t v_addr = k_addr + NP * PLANE;
     // ---- S = Q K^T (64 x 64), hi*hi [+ lo*hi + hi*lo]; 4 k16 steps per 64-column box ----
@@ -152,7 +167,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
         const int kidx = j * KT + n * 8 + 2 * t + (c & 1);
         const int qidx = qrow + (c >> 1) * 8;
         float v = fmaf(s[4 * n + c], LOG2E, slope2 * static_cast<float>(kidx));
-        if (kidx >= p.T || (p.causal && kidx > qidx)) v = -INFINITY;
+        if (kidx >= p.T || (p.causal && kidx > qidx) || (kidx >= pad0 && kidx < pad1) || kidx < sq[c >> 1]) v = -INFINITY;
         s[4 * n + c] = v;
         mx[c >> 1] = fmaxf(mx[c >> 1], v);
       }
@@ -168,10 +183,12 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
       m_run[r] = mn;
       l[r] *= alpha[r];
     }
+    if (!RNACC) {
 #pragma unroll
-    for (int bx = 0; bx < NB; ++bx)
+      for (int bx = 0; bx < NB; ++bx)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) o[bx][i] *= alpha[(i >> 1) & 1];
+        for (int i = 0; i < 32; ++i) o[bx][i] *= alpha[(i >> 1) & 1];
+    }
     // ---- P = 2^(s - m) as fp16 hi [+ lo] A fragments, O += P V ----
     uint32_t ph[4][4], pl[4][4];
 #pragma unroll
@@ -189,27 +206,37 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
         }
       }
     }
+    float pv[RNACC ? NB : 1][RNACC ? 32 : 1];
+    auto& acc = [&]() -> float(&)[NB][32] {
+      if constexpr (RNACC) return pv; else return o;
+    }();
     wgmma_fence();
 #pragma unroll
-    for (int bx = 0; bx < NB; ++bx) wgmma_fence_regs(o[bx]);
+    for (int bx = 0; bx < NB; ++bx) wgmma_fence_regs(acc[bx]);
 #pragma unroll
     for (int bx = 0; bx < NB; ++bx) {
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
         const uint64_t vh = make_desc_sw128(v_addr + bx * TILE + kk * 2048);  // 16 key rows of 128 B per k-step
-        wgmma_m64n64k16_f16_rs_tb(o[bx], ph[kk], vh, 1u);
+        wgmma_m64n64k16_f16_rs_tb(acc[bx], ph[kk], vh, (RNACC && kk == 0) ? 0u : 1u);
         if (NP == 2) {
-          wgmma_m64n64k16_f16_rs_tb(o[bx], pl[kk], vh, 1u);
-          wgmma_m64n64k16_f16_rs_tb(o[bx], ph[kk], make_desc_sw128(v_addr + PLANE + bx * TILE + kk * 2048), 1u);
+          wgmma_m64n64k16_f16_rs_tb(acc[bx], pl[kk], vh, 1u);
+          wgmma_m64n64k16_f16_rs_tb(acc[bx], ph[kk], make_desc_sw128(v_addr + PLANE + bx * TILE + kk * 2048), 1u);
         }
       }
     }
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
-    for (int bx = 0; bx < NB; ++bx) wgmma_fence_regs(o[bx]);
+    for (int bx = 0; bx < NB; ++bx) wgmma_fence_regs(acc[bx]);
+    if (RNACC) {
+#pragma unroll
+      for (int bx = 0; bx < NB; ++bx)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[bx][i] = __fmaf_rn(o[bx][i], alpha[(i >> 1) & 1], acc[bx][i]);
+    }
     __syncthreads();  // every warp is done with this slot
-    if (threadIdx.x == 0 && j + NSLOT < nkb) load_block(j + NSLOT);
+    if (threadIdx.x == 0 && i + NSLOT < nkb) load_block(i + NSLOT);
   }
 
   // ---- epilogue: O / l -> fp16 hi [+ lo | + e4m3 planes]; rows qrow, qrow + 8, head-dim columns 8n + 2t (+1) ----
@@ -266,15 +293,19 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
   if (a.ld % 8 || a.lo_off % 8 || a.ldo % 8 || a.out_lo_off % 8 || (reinterpret_cast<uintptr_t>(a.out) & 15))
     return set_error(PG_ERR_ARG, "attention_wgmma: pitches must be multiples of 8 elements and out 16-byte aligned");
   if (a.q_begin != 0) return set_error(PG_ERR_ARG, "attention_wgmma: q_begin is only supported by the mma.sync kernel");
-  if (a.prefix && (!a.causal || a.prefix_len <= 0 || a.prefix_len % 128))
+  if (a.prefix && (!a.causal || a.prefix_len <= 0 || (!a.prefix_mem && a.prefix_len % 128)))
     return set_error(PG_ERR_ARG, "attention_wgmma: a shared prefix needs causal attention and a length that is a multiple of 128");
+  if ((a.prefix_mem && (!a.prefix || a.head_dim != 64)) || (a.seg_start && (a.B != 1 || a.prefix || !a.causal)))
+    return set_error(PG_ERR_ARG, "attention_wgmma: the memory form needs a prefix and 64-wide heads; the segment-causal form one causal sequence");
   if (a.head_dim != 64 && a.head_dim != 128) return set_error(PG_ERR_ARG, "attention_wgmma: head width must be 64 or 128");
   const int HDw = a.head_dim;
   if (HDw == 128 && (a.base_o || a.mask_pos || a.perm_C))
     return set_error(PG_ERR_UNSUPPORTED, "attention_wgmma: the delta-operand and column-attention forms run on 64-wide heads only");
   AttnWParams p{};
   p.B = a.B; p.heads = a.heads; p.d = a.heads * HDw;
-  p.Tq = a.T; p.s_blocks = a.prefix ? a.prefix_len / KT : 0;
+  p.Tq = a.T; p.s_blocks = a.prefix ? (a.prefix_len + KT - 1) / KT : 0;
+  p.p_valid = a.prefix_mem ? a.prefix_len : p.s_blocks * KT;
+  p.head_major = a.prefix_mem; p.seg_start = a.seg_start;
   p.T = a.T + p.s_blocks * KT;
   p.nqt = (a.T + QT - 1) / QT; p.nkb = (p.T + KT - 1) / KT;
   p.lo_off = a.lo_off; p.out = a.out; p.ldo = a.ldo; p.out_lo_off = a.out_lo_off;
@@ -310,6 +341,8 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
     PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<1, 0, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<1, 64>::TOTAL));
     PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 0, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2, 64>::TOTAL));
     PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2, 64>::TOTAL));
+    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 0, 64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2, 64>::TOTAL));
+    PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<1, 0, 64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<1, 64>::TOTAL));
     PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<1, 0, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<1, 128>::TOTAL));
     PG_CUDA_OK(cudaFuncSetAttribute(attn_wgmma_kernel<2, 0, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemW<2, 128>::TOTAL));
     attr_set[dev] = true;
@@ -317,6 +350,8 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
   const bool delta = a.base_o != nullptr || a.mask_pos != nullptr;
   if (delta && np != 2) return set_error(PG_ERR_UNSUPPORTED, "attention_wgmma: the delta-operand form runs on fp16 hi/lo operands (nseg 3)");
   if (delta) attn_wgmma_kernel<2, 1, 64><<<grid, ATT_THREADS, SmemW<2, 64>::TOTAL, s>>>(tmQ, tm, tmP, p);
+  else if (a.prefix_mem && np == 2) attn_wgmma_kernel<2, 0, 64, 1><<<grid, ATT_THREADS, SmemW<2, 64>::TOTAL, s>>>(tmQ, tm, tmP, p);
+  else if (a.prefix_mem) attn_wgmma_kernel<1, 0, 64, 1><<<grid, ATT_THREADS, SmemW<1, 64>::TOTAL, s>>>(tmQ, tm, tmP, p);
   else if (HDw == 128 && np == 1) attn_wgmma_kernel<1, 0, 128><<<grid, ATT_THREADS, SmemW<1, 128>::TOTAL, s>>>(tmQ, tm, tmP, p);
   else if (HDw == 128) attn_wgmma_kernel<2, 0, 128><<<grid, ATT_THREADS, SmemW<2, 128>::TOTAL, s>>>(tmQ, tm, tmP, p);
   else if (np == 1) attn_wgmma_kernel<1, 0, 64><<<grid, ATT_THREADS, SmemW<1, 64>::TOTAL, s>>>(tmQ, tm, tmP, p);

@@ -56,8 +56,10 @@ struct GemmLaunch {
   float* resid; int64_t ldr;
   const float* rot_cos; const float* rot_sin; int rot_T; int rot_dim;
   int rot_half = 32;              // epi 3: half the head slot; 64 = 128-wide slots, tables [T, 64] (internal: pg_gemm keeps 32)
+  const int32_t* rot_pos = nullptr; // epi 3: [M] (device) table row of each output row (positions that restart per segment); null = row % rot_T
   float a_scale = 0.f;            // nseg 2: s used by the producer of a's e4m3 planes
   const float* w_inv = nullptr;   // nseg 2: [N] 1 / t_n of the weight rows
+  int kchunk = 0;                 // hi*hi K-chunk length of this launch (elements); 0 = the process-wide gemm_kchunk
   int w_uniform = 0;              // nseg 2: all w_inv[n] are equal (one scale per matrix, as pg_load_weights / pg_pack_weight produce)
   int out_fmt = 0;                // epi != 2: 0, 1 or 2 (see above); planes at out_lo_off
   float out_scale = 0.f;          // out_fmt 2: s of the GEMM that will consume `out`
@@ -115,6 +117,13 @@ struct AttnLaunch {
   const __half* base_o = nullptr; const int32_t* mask_pos = nullptr; __half* cout = nullptr; int64_t ldc = 0; int64_t c_lo_off = 0;
   // Width of a head's q / k / v / output slot (wgmma kernel): 64, or 128 for the 128-wide slots of ProGen2's 80- and 96-wide heads.
   int head_dim = 64;
+  // Memory form of the prefix (wgmma kernel, 64-wide heads; PoET's variant rows against the context record): `prefix` holds prefix_len
+  // rows of any length, all visible to every query; they take ceil(prefix_len / 64) key blocks, the rows past prefix_len masked. Work
+  // items run head-major, so that one head's prefix rows stay in L2 while every sequence reads them.
+  int prefix_mem = 0;
+  // Segment-causal form (wgmma kernel, B == 1): seg_start[t] (device) = first row of row t's segment; row t sees keys seg_start[t] .. t.
+  // Key blocks before the query tile's first segment start are skipped.
+  const int32_t* seg_start = nullptr;
 };
 int launch_attention(const AttnLaunch& a, cudaStream_t s);
 
@@ -185,9 +194,11 @@ struct ArFusion {
   float* out_logprobs = nullptr;
 };
 // wte: the head [vocab, d]; bias: [vocab] or null; the label of token id v is head column v - label_off.
+// lnf_g null: no LayerNorm before the head (PoET's norm=False). ignore_id >= 0: a next token equal to it contributes 0 (cross entropy's
+// ignore_index).
 int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t* ids, const int32_t* lens, const float* lnf_g,
                    const float* lnf_b, const float* wte, const float* bias, int label_off, const ArFusion& fusion, float* tok_logp,
-                   float* out_sum, cudaStream_t s);
+                   float* out_sum, cudaStream_t s, int ignore_id = -1);
 // After a GEMM epi 7 pass over B sequences of T rows: tok_logp[r] = lm_tgt[r] - logsumexp of the row's `tiles` partials combined in
 // tile order (0 for t >= lens[b] - 1, NaN for a next token outside [0, vocab)); out_logprobs (optional, [B*T, vocab], holding the logits
 // epi 7 wrote) becomes the log-softmax rows in place; out_sum[b] = the sequence sums (seq_sum_kernel).

@@ -70,6 +70,7 @@ struct GemmKParams {
   float out_scale;        // out_fmt 2: s of the consuming GEMM (hi8 = e4m3(hi*s), lo8 = e4m3(lo*2^11*s))
   const float* rot_cos; const float* rot_sin; int rot_T; int rot_dim;
   int rot_half;           // 32: 64-wide head slots, tables [T, 32]; 64: 128-wide slots (one per N tile), tables [T, 64]
+  const int32_t* rot_pos; // [M] table row of each row, or null (row % rot_T)
   int tiles_m, tiles_n;
   int prefetch;           // k-blocks of L2 look-ahead for the A operand (0 = off)
   // delta-operand mode (common.h GemmLaunch): shared base rows added before / subtracted after the activation, masked rows skipped
@@ -153,7 +154,7 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
     }
     if (EPI == 3 && p.rot_half == 64) {
       // the same over one 128-wide slot per N tile: blocks j and j + 8 hold columns c and c + 64; cos/sin[t, c] for c in [0, 64)
-      const int t = static_cast<int>(row % p.rot_T);
+      const int t = p.rot_pos ? (row < p.M ? __ldg(p.rot_pos + row) : 0) : static_cast<int>(row % p.rot_T);
       if (col0 - (col0 & 127) < 2 * p.rot_dim) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -170,7 +171,7 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
     } else if (EPI == 3) {
       // rotary: x*cos + rotate_half(x)*sin over each 64-wide head (blocks j and j + 4 of one head hold columns c and c + 32);
       // cos/sin[t, c] for c in [0,32) (both halves equal)
-      const int t = static_cast<int>(row % p.rot_T);
+      const int t = p.rot_pos ? (row < p.M ? __ldg(p.rot_pos + row) : 0) : static_cast<int>(row % p.rot_T);
 #pragma unroll
       for (int hd = 0; hd < 2; ++hd) {
         if (col0 - (col0 & 63) + 64 * hd >= 2 * p.rot_dim) continue;
@@ -639,7 +640,8 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
     ++ns;
   };
   // hi*hi pieces: as equal as possible, each <= kchunk along K, at most what the segment table holds
-  int pieces = (g.K + gemm_kchunk() - 1) / gemm_kchunk();
+  const int kchunk = g.kchunk >= BK ? g.kchunk : gemm_kchunk();
+  int pieces = (g.K + kchunk - 1) / kchunk;
   if (pieces < 1) pieces = 1;
   if (pieces > MAX_SEGS - 2) pieces = MAX_SEGS - 2;
   if (pieces > kblocks) pieces = kblocks;
@@ -663,7 +665,7 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   p.resid = g.resid; p.ldr = g.ldr;
   p.out_fmt = (g.epi == 2) ? 0 : g.out_fmt;
   p.out_scale = g.out_scale;
-  p.rot_cos = g.rot_cos; p.rot_sin = g.rot_sin; p.rot_T = g.rot_T; p.rot_dim = g.rot_dim; p.rot_half = g.rot_half;
+  p.rot_cos = g.rot_cos; p.rot_sin = g.rot_sin; p.rot_T = g.rot_T; p.rot_dim = g.rot_dim; p.rot_half = g.rot_half; p.rot_pos = g.rot_pos;
   p.tiles_m = cta2 ? (g.M + 2 * BM - 1) / (2 * BM) : (g.M + BM - 1) / BM;
   p.tiles_n = (g.N + BN - 1) / BN;
   p.prefetch = grouped ? 0 : gemm_prefetch();

@@ -124,6 +124,7 @@ struct ArHeadParams {
   int label_off;      // head column of token id v is v - label_off (ProGen2: the head holds vocabulary rows 5..29)
   ArFusion f;
   float* tok_logp;  // [B*T]
+  int ignore_id;    // >= 0: a next token equal to it scores 0
 };
 
 // Retrieval fusion of one log-probability (Tranception model_pytorch.py:806-830; TranceptEVE model_pytorch.py:1100-1116, and the
@@ -153,14 +154,18 @@ __global__ void ar_head_kernel(ArHeadParams p) {
   const long long r = blockIdx.x;
   const int b = static_cast<int>(r / p.T), t = static_cast<int>(r % p.T);
   const int len = p.lens[b];
-  if (t + 1 >= len) {  // block-uniform
+  if (t + 1 >= len || (p.ignore_id >= 0 && p.ids[r + 1] == p.ignore_id)) {  // block-uniform
     if (threadIdx.x == 0) p.tok_logp[r] = 0.f;
     return;
   }
   const float* xr = p.x + r * p.d;
-  float mean, rstd;
-  block_ln_stats(xr, p.d, sh, mean, rstd);
-  for (int j = threadIdx.x; j < p.d; j += blockDim.x) y[j] = (xr[j] - mean) * rstd * p.lnf_g[j] + p.lnf_b[j];
+  if (p.lnf_g) {
+    float mean, rstd;
+    block_ln_stats(xr, p.d, sh, mean, rstd);
+    for (int j = threadIdx.x; j < p.d; j += blockDim.x) y[j] = (xr[j] - mean) * rstd * p.lnf_g[j] + p.lnf_b[j];
+  } else {
+    for (int j = threadIdx.x; j < p.d; j += blockDim.x) y[j] = xr[j];
+  }
   __syncthreads();
   const float lse = block_logits_lse(y, p.d, p.wte, p.bias, p.vocab, logits);
   if (threadIdx.x < 32) {
@@ -261,9 +266,9 @@ int launch_qkv_conv(const __half* in, __half* out, int64_t ld, int64_t lo_off, i
 
 int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t* ids, const int32_t* lens, const float* lnf_g,
                    const float* lnf_b, const float* wte, const float* bias, int label_off, const ArFusion& fusion, float* tok_logp,
-                   float* out_sum, cudaStream_t s) {
+                   float* out_sum, cudaStream_t s, int ignore_id) {
   if (B <= 0 || T <= 0) return PG_OK;
-  ArHeadParams p{x, d, T, vocab, ids, lens, lnf_g, lnf_b, wte, bias, label_off, fusion, tok_logp};
+  ArHeadParams p{x, d, T, vocab, ids, lens, lnf_g, lnf_b, wte, bias, label_off, fusion, tok_logp, ignore_id};
   ar_head_kernel<<<static_cast<unsigned>(static_cast<long long>(B) * T), 128, (d + vocab) * sizeof(float), s>>>(p);
   seq_sum_kernel<<<(B + 3) / 4, 128, 0, s>>>(tok_logp, lens, B, T, out_sum);
   PG_CUDA_OK(cudaGetLastError());

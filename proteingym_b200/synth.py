@@ -760,3 +760,82 @@ def write_protgpt2_checkpoint(folder: str, arch: Protgpt2Arch, seed: int = 0, st
     else:
         torch.save(st, os.path.join(folder, "pytorch_model.bin"))
     return st
+
+
+@dataclass
+class PoetArch:
+    layers: int
+    hidden_dim: int
+    heads: int
+    ff_dim: int | None = None  # None: 4 * hidden_dim (poet.py PoET.__init__)
+    norm: bool = False
+
+
+POET = PoetArch(12, 1024, 16)  # the released 201M-parameter checkpoint (shapes from the parameter count)
+
+
+def make_poet_state(arch: PoetArch, seed: int = 0, qk_gain: float = 2.0) -> dict:
+    """PoET state dict with the reference's key names (poet/models/poet.py PoET, without the checkpoint's ``model.`` prefix), drawn on
+    the CPU from ``seed`` and rounded to fp16-representable values, so that the reference's ``.half()`` changes only the activations:
+    nn.Linear's U(+-1/sqrt(fan_in)) with q/k scaled by ``qk_gain`` (attention far from uniform), LayerNorm weights 1 + 0.1 N(0,1) and
+    biases 0.1 N(0,1), the embedding N(0, 1), a head of N(0, 4/d) rows with a 0.5 N(0,1) bias, and the rotary inv_freq buffers the
+    reference registers (base 10 000 over the 64-wide head, each frequency twice)."""
+    g = torch.Generator().manual_seed(seed)
+    d = arch.hidden_dim
+    f = arch.ff_dim or 4 * d
+    hd = d // arch.heads
+    ln_w = lambda: 1 + 0.1 * torch.randn(d, generator=g)
+    ln_b = lambda: 0.1 * torch.randn(d, generator=g)
+    inv = 1.0 / (10000 ** (torch.div(torch.arange(hd), 2, rounding_mode="floor") * 2.0 / hd))
+    st = {"token_embed.weight": torch.randn((24, d), generator=g), "rotary_emb.inv_freq": inv.clone()}
+    for i in range(arch.layers):
+        p = f"decoder.layers.{i}."
+        for a in ("self_attn.", "multihead_attn."):
+            st[p + a + "q_proj.weight"] = qk_gain * _uniform(g, (d, d), 1 / math.sqrt(d))
+            st[p + a + "k_proj.weight"] = qk_gain * _uniform(g, (d, d), 1 / math.sqrt(d))
+            st[p + a + "v_proj.weight"] = _uniform(g, (d, d), 1 / math.sqrt(d))
+            st[p + a + "out_proj.weight"] = _uniform(g, (d, d), 1 / math.sqrt(d))
+            st[p + a + "out_proj.bias"] = _uniform(g, (d,), 1 / math.sqrt(d))
+            st[p + a + "rotary_emb.inv_freq"] = inv.clone()
+        st[p + "linear1.weight"] = _uniform(g, (f, d), 1 / math.sqrt(d))
+        st[p + "linear1.bias"] = _uniform(g, (f,), 1 / math.sqrt(d))
+        st[p + "linear2.weight"] = _uniform(g, (d, f), 1 / math.sqrt(f))
+        st[p + "linear2.bias"] = _uniform(g, (d,), 1 / math.sqrt(f))
+        for n in ("norm1", "norm2", "norm3"):
+            st[p + n + ".weight"], st[p + n + ".bias"] = ln_w(), ln_b()
+    if arch.norm:
+        st["norm.weight"], st["norm.bias"] = ln_w(), ln_b()
+    st["linear.weight"] = (2 / math.sqrt(d)) * torch.randn((24, d), generator=g)
+    st["linear.bias"] = 0.5 * torch.randn(24, generator=g)
+    return {k: (v if k.endswith("inv_freq") else v.half().float()) for k, v in st.items()}
+
+
+def write_poet_checkpoint(path: str, arch: PoetArch, seed: int = 0, state: dict | None = None) -> dict:
+    """A PoET checkpoint in the layout scripts/score.py reads: ``hyper_parameters.model_spec.init_args`` and a state dict whose keys carry
+    one leading component (``model.``) that the script strips."""
+    st = make_poet_state(arch, seed) if state is None else state
+    init_args = dict(n_vocab=24, hidden_dim=arch.hidden_dim, ff_dim=arch.ff_dim, num_layers=arch.layers, nhead=arch.heads, dropout=0,
+                     use_multi_rotary=True, norm=arch.norm, mask_token=23)
+    torch.save({"hyper_parameters": {"model_spec": {"init_args": init_args}}, "state_dict": {"model." + k: v for k, v in st.items()}}, path)
+    return st
+
+
+def poet_a3m(target_seq: str, n: int, seed: int, sub_rate=(0.05, 0.9), gap_rate=0.1, insert_rate=0.03, lower_x: float = 0.01) -> list[str]:
+    """Synthetic a3m rows (first row = the target): substitutions, '-' gaps and lower-case insertions between match columns."""
+    rng = np.random.RandomState(seed)
+    rows = [target_seq]
+    for _ in range(n - 1):
+        r = rng.uniform(*sub_rate)
+        out = []
+        for c in target_seq:
+            u = rng.rand()
+            if u < gap_rate:
+                out.append("-")
+            elif u < gap_rate + r:
+                out.append(AA20[rng.randint(0, 20)] if rng.rand() > lower_x else "X")
+            else:
+                out.append(c)
+            if rng.rand() < insert_rate:
+                out.append("".join(AA20[i] for i in rng.randint(0, 20, size=rng.randint(1, 4))).lower())
+        rows.append("".join(out))
+    return rows

@@ -286,6 +286,25 @@ typedef struct {
 } pg_gemm_args;
 int pg_gemm(const pg_gemm_args* args, pg_stream stream);
 
+/* The GEMM forms the model stacks launch beyond pg_gemm (pg_gemm is this call with form = NULL). An all-zero field keeps the plain
+ * behaviour, except rot_half, where 0 means 32.
+ *   rot_pos    epi 3: [M] int32 (device) table row of each output row (positions that restart per segment); NULL = row % rot_T
+ *   rot_half   epi 3: half the rotary head slot: 32 (64-wide slots, tables [rot_T, 32]) or 64 (128-wide slots, tables [rot_T, 64])
+ *   kchunk     longest run of K (elements, >= 64) one hi*hi chunk accumulates for this launch; 0 = the process-wide "gemm_kchunk"
+ *   w_uniform  nseg 2: 1 when every w_inv[n] is equal (one scale per matrix, as pg_pack_weight fmt 2 writes): one factor per tile
+ *   lm_*       epi 7, the LM-head log-softmax partials (no bias, no output buffer): rows are (b, t) = (row / lm_T, row % lm_T) and
+ *              M a multiple of lm_T. For every row with t + 1 < lm_lens[b] and every 128-column tile of N, lm_part[row * tiles + tile]
+ *              (float pairs, tiles = ceil(N / 128)) = (max, sum exp(l - max)) over the tile's columns < N, and lm_tgt[row] = the logit
+ *              of column lm_ids[row + 1] when that is < N; lm_logits (optional, [M, N] fp32) receives every logit of those rows.
+ *              Other rows are left untouched. lm_ids / lm_lens are device int32. */
+struct pg_gemm_form {  /* a struct tag only: the entry point below shares its name */
+  const int32_t* rot_pos; int32_t rot_half;
+  int32_t kchunk;
+  int32_t w_uniform;
+  float* lm_part; float* lm_tgt; float* lm_logits; const int32_t* lm_ids; const int32_t* lm_lens; int32_t lm_T;
+};
+int pg_gemm_form(const pg_gemm_args* args, const struct pg_gemm_form* form, pg_stream stream);
+
 /* fp32 weights [N, K] (nn.Linear layout) -> the operand format of pg_gemm's `w`: fmt 0 = nseg 1, fmt 1 = nseg 3,
  * fmt 2 = nseg 2 (writes w_inv[N]). out has N rows of K (fmt 0) or 2K (fmt 1, 2) fp16 elements. */
 int pg_pack_weight(const float* w, int32_t N, int32_t K, int32_t fmt, void* out, float* w_inv, pg_stream stream);
@@ -310,6 +329,26 @@ typedef struct {
   const void* base_o; const int32_t* mask_pos; void* cout; int64_t ldc; int64_t c_lo_off;
 } pg_attn_args;
 int pg_attention(const pg_attn_args* args, pg_stream stream);
+
+/* The attention forms the model stacks launch beyond pg_attention (impl 0 only; pg_attention is this call with form = NULL). An
+ * all-zero field keeps the plain behaviour, except head_dim, where 0 means 64.
+ *   prefix, prefix_len  causal shared prefix: the B sequences hold rows [prefix_len, prefix_len + T) of longer sequences whose first
+ *                       prefix_len rows (a multiple of 128) are shared; their K / V rows live in `prefix` (same pitch and planes as qkv).
+ *                       ALiBi is applied at the absolute key index.
+ *   prefix_mem          1: memory form of the prefix (64-wide heads): any prefix_len, every prefix row visible to every query, work
+ *                       items in head-major order and each key block's P V added to O in round-to-nearest fp32.
+ *   seg_start           segment-causal form (B == 1, causal, no prefix): seg_start[t] (device int32) = first row of row t's segment;
+ *                       row t sees keys seg_start[t] .. t.
+ *   perm_C              column form (64-wide heads, no prefix): sequence b is column (b / perm_C, b % perm_C) of an alignment of
+ *                       T rows; its row r goes to output row (b / perm_C, r, b % perm_C). B must be a multiple of perm_C.
+ *   head_dim            width of each head's q / k / v / output slot: 64, or 128 (d = heads * head_dim). */
+typedef struct pg_attn_form {
+  const void* prefix; int32_t prefix_len; int32_t prefix_mem;
+  const int32_t* seg_start;
+  int32_t perm_C;
+  int32_t head_dim;
+} pg_attn_form;
+int pg_attention_form(const pg_attn_args* args, const pg_attn_form* form, pg_stream stream);
 
 /* ---- MSA pre-processing for the Tranception retrieval prior (SURVEY.md §8f rank 2) ----
  * pg_msa_cluster_neighbors replaces calc_num_cluster_members_nogaps[_parallel] (proteingym/utils/weights.py:114-216):

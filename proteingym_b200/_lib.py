@@ -46,6 +46,17 @@ class PgAttnArgs(C.Structure):
                 ("base_o", C.c_void_p), ("mask_pos", C.c_void_p), ("cout", C.c_void_p), ("ldc", C.c_int64), ("c_lo_off", C.c_int64)]
 
 
+class PgAttnForm(C.Structure):
+    _fields_ = [("prefix", C.c_void_p), ("prefix_len", C.c_int32), ("prefix_mem", C.c_int32), ("seg_start", C.c_void_p),
+                ("perm_C", C.c_int32), ("head_dim", C.c_int32)]
+
+
+class PgGemmForm(C.Structure):
+    _fields_ = [("rot_pos", C.c_void_p), ("rot_half", C.c_int32), ("kchunk", C.c_int32), ("w_uniform", C.c_int32),
+                ("lm_part", C.c_void_p), ("lm_tgt", C.c_void_p), ("lm_logits", C.c_void_p), ("lm_ids", C.c_void_p),
+                ("lm_lens", C.c_void_p), ("lm_T", C.c_int32)]
+
+
 class PgArFusion(C.Structure):
     _fields_ = [("log_prior", C.c_void_p), ("prior_row", C.c_void_p), ("alpha", C.c_float),
                 ("log_prior2", C.c_void_p), ("prior_row2", C.c_void_p), ("beta", C.c_float),
@@ -78,10 +89,12 @@ SIGNATURES = {
     "pg_poet_loglik": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_poet_record": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "pg_gemm": (C.c_int, [C.POINTER(PgGemmArgs), C.c_void_p]),
+    "pg_gemm_form": (C.c_int, [C.POINTER(PgGemmArgs), C.POINTER(PgGemmForm), C.c_void_p]),
     "pg_layernorm_f16": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                    C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]),
     "pg_pack_weight": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_attention": (C.c_int, [C.POINTER(PgAttnArgs), C.c_void_p]),
+    "pg_attention_form": (C.c_int, [C.POINTER(PgAttnArgs), C.POINTER(PgAttnForm), C.c_void_p]),
     "pg_msa_cluster_neighbors": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_msa_prior": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p, C.c_void_p]),
     "pg_eve_output_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),

@@ -1750,7 +1750,9 @@ int pg_set_tuning(const char* key, int32_t value) {
   return set_error(PG_ERR_ARG, std::string("pg_set_tuning: unknown key ") + key);
 }
 
-int pg_gemm(const pg_gemm_args* a, pg_stream stream) {
+int pg_gemm(const pg_gemm_args* a, pg_stream stream) { return pg_gemm_form(a, nullptr, stream); }
+
+int pg_gemm_form(const pg_gemm_args* a, const struct pg_gemm_form* f, pg_stream stream) {
   if (!a) return set_error(PG_ERR_ARG, "pg_gemm: null args");
   GemmLaunch g{};
   g.a = a->a; g.lda = a->lda; g.w = a->w; g.ldw = a->ldw; g.bias = a->bias;
@@ -1762,6 +1764,12 @@ int pg_gemm(const pg_gemm_args* a, pg_stream stream) {
   g.out_fmt = a->out_fmt ? a->out_fmt : (a->out_lo_off > 0 ? 1 : 0);
   g.grp_rows_a = a->grp_rows_a; g.grp_rows_b = a->grp_rows_b;
   g.base_pre = a->base_pre; g.base_post = static_cast<const __half*>(a->base_post); g.base_T = a->base_T; g.mask_pos = a->mask_pos;
+  if (f) {
+    g.rot_pos = f->rot_pos; g.rot_half = f->rot_half ? f->rot_half : 32;
+    g.kchunk = f->kchunk; g.w_uniform = f->w_uniform;
+    g.lm_part = reinterpret_cast<float2*>(f->lm_part); g.lm_tgt = f->lm_tgt; g.lm_logits = f->lm_logits;
+    g.lm_ids = f->lm_ids; g.lm_lens = f->lm_lens; g.lm_T = f->lm_T;
+  }
   ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream));
   return launch_gemm(g, static_cast<cudaStream_t>(stream));
 }
@@ -1795,7 +1803,9 @@ int pg_pack_weight(const float* w, int32_t N, int32_t K, int32_t fmt, void* out,
   return PG_OK;
 }
 
-int pg_attention(const pg_attn_args* a, pg_stream stream) {
+int pg_attention(const pg_attn_args* a, pg_stream stream) { return pg_attention_form(a, nullptr, stream); }
+
+int pg_attention_form(const pg_attn_args* a, const pg_attn_form* f, pg_stream stream) {
   if (!a || !a->qkv || !a->out) return set_error(PG_ERR_ARG, "pg_attention: null args");
   AttnLaunch l{};
   l.qkv = static_cast<const __half*>(a->qkv); l.ld = a->ld; l.lo_off = a->lo_off;
@@ -1803,7 +1813,13 @@ int pg_attention(const pg_attn_args* a, pg_stream stream) {
   l.B = a->B; l.T = a->T; l.heads = a->heads; l.nseg = a->nseg; l.causal = a->causal; l.alibi_slopes = a->alibi_slopes;
   l.out_fmt = a->out_fmt ? a->out_fmt : -1; l.out_scale = a->out_scale;
   l.base_o = static_cast<const __half*>(a->base_o); l.mask_pos = a->mask_pos; l.cout = static_cast<__half*>(a->cout); l.ldc = a->ldc; l.c_lo_off = a->c_lo_off;
-  if ((l.base_o || l.mask_pos) && a->impl != 0) return set_error(PG_ERR_UNSUPPORTED, "pg_attention: the delta-operand form needs impl 0");
+  if (f) {
+    l.prefix = static_cast<const __half*>(f->prefix); l.prefix_len = f->prefix_len; l.prefix_mem = f->prefix_mem;
+    l.seg_start = f->seg_start; l.perm_C = f->perm_C; l.head_dim = f->head_dim ? f->head_dim : 64;
+  }
+  const bool form = l.prefix || l.prefix_len || l.prefix_mem || l.seg_start || l.perm_C || l.head_dim != 64;
+  if ((l.base_o || l.mask_pos || form) && a->impl != 0)
+    return set_error(PG_ERR_UNSUPPORTED, "pg_attention: the delta-operand form and the pg_attention_form forms need impl 0");
   ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream));
   if (a->impl == 0) return launch_attention_wgmma(l, static_cast<cudaStream_t>(stream));   // the model's kernel
   if (a->impl != 1) return set_error(PG_ERR_ARG, "pg_attention: impl must be 0 (the model's wgmma kernel) or 1 (mma.sync cross-check)");

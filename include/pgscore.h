@@ -314,6 +314,22 @@ int pg_pack_weight(const float* w, int32_t N, int32_t K, int32_t fmt, void* out,
 int pg_layernorm_f16(const float* x, int64_t ldx, const float* gamma, const float* beta, int32_t rows, int32_t d,
                      void* out, int64_t ldo, int64_t lo_off, int32_t fmt, float scale, pg_stream stream);
 
+/* The LayerNorm forms the model stacks launch beyond pg_layernorm_f16 (pg_layernorm_f16 is this call with form = NULL). An all-zero
+ * field keeps the plain behaviour.
+ *   dp              width of every output plane (>= d, a multiple of 4; 0 = d): columns [d, dp) of each plane are written as zeros
+ *                   (the K padding of the next GEMM, e.g. ESM2 35M's d = 480 in 512-wide rows); the e4m3 planes are dp bytes each
+ *   perm_R, perm_C  column layout of an alignment (MSA Transformer): input row (b, r, c) of [R, C] alignments goes to output row
+ *                   (b, c, r); rows must be a multiple of R * C
+ *   base, base_T    delta-operand form (PG_PREC_F16D, unpadded rows, no permutation): the output is LN(x[row]) - base[row % base_T],
+ *                   formed in fp32 before rounding; base is fp16 [base_T, d] (device) */
+typedef struct pg_ln_form {
+  int32_t dp;
+  int32_t perm_R; int32_t perm_C;
+  const void* base; int32_t base_T;
+} pg_ln_form;
+int pg_layernorm_form(const float* x, int64_t ldx, const float* gamma, const float* beta, int32_t rows, int32_t d,
+                      void* out, int64_t ldo, int64_t lo_off, int32_t fmt, float scale, const pg_ln_form* form, pg_stream stream);
+
 /* Multi-head self-attention over equal-length sequences (multihead_attention.py:357-394), head_dim 64, q pre-scaled.
  *   qkv [B*T, ld] fp16 with q at column 0, k at column d, v at 2d (d = heads*64); lo parts at +lo_off when nseg == 3.
  *   out [B*T, ldo] fp16 (lo at +out_lo_off). causal/alibi are for the Tranception path (model_pytorch.py:155-183). */
@@ -349,6 +365,74 @@ typedef struct pg_attn_form {
   int32_t head_dim;
 } pg_attn_form;
 int pg_attention_form(const pg_attn_args* args, const pg_attn_form* form, pg_stream stream);
+
+/* ---- the row kernels between the GEMMs and the attention, one entry point each (same kernels the model stacks launch) ---- */
+
+/* Attention for ONE query row per sequence (the pruned last layer of the ESM-family masked-marginal passes): row row_sel[b] (device
+ * int32) of sequence b attends to all T rows of b, written to output row b. Bidirectional, no bias, 64-wide heads; nseg 1 or 3
+ * (lo_off) and out_fmt 0 / 1 / 2 as pg_attention. causal, alibi_slopes, impl and the delta-operand fields must be zero. */
+int pg_attention_rows(const pg_attn_args* args, const int32_t* row_sel, pg_stream stream);
+
+/* ESM C's q/k LayerNorm + rotary, in place on rows [q | k] (q at column 0, k at heads * 64; fp16 hi, and lo at +lo_off when lo_off > 0):
+ * weight-only LayerNorm over the full width (eps 1e-5) with q_gamma / k_gamma [heads * 64], rotate-half rotary in every 64-wide head
+ * at position t = row % T (rot_cos / rot_sin [T, 32] fp32), and q scaled by exactly 1/8. heads 1..24; other columns are not touched. */
+int pg_qk_ln_rotary(void* qkv, int64_t ld, int64_t lo_off, int32_t rows, int32_t heads, const float* q_gamma, const float* k_gamma,
+                    const float* rot_cos, const float* rot_sin, int32_t T, pg_stream stream);
+
+/* ESM embedding of P masked copies of a window of T tokens (esm1.py:123-139, esm2.py:83-94): x [P * T, d] fp32, row (p, t) =
+ * embed[tok] (the <mask> row mask_idx at the copy's masked token, zeroed under token_dropout) * the token-dropout rescale
+ * 0.88 / (1 - n_mask / T) + pos_table[t + 2] (NULL for rotary models), then emb_layer_norm_before when lnb_gamma / lnb_beta are set.
+ * Copy p uses positions[p_offset + p] (masked token index into `tokens`, -1 = none; NULL = none) and win_start[p_offset + p] (NULL = 0);
+ * tokens past n_tokens read the last token. force_mask_scale = 1 applies the one-mask rescale to copies with no masked token in the
+ * window (the delta mode's shared base row). All pointers are device pointers. */
+typedef struct {
+  const int32_t* tokens; int32_t n_tokens;
+  const int32_t* positions; const int32_t* win_start;
+  int32_t P, T, d;
+  const float* embed; const float* pos_table;
+  const float* lnb_gamma; const float* lnb_beta;
+  int32_t token_dropout, mask_idx, p_offset, force_mask_scale;
+  float* x;
+} pg_esm_embed_args;
+int pg_esm_embed(const pg_esm_embed_args* args, pg_stream stream);
+
+/* The ESM-family LM head on P rows (esm/modules.py:322-328) + log_softmax: row p is x row p (all_rows = 1) or x row
+ * p * T + row_in_seq[p] (device int32); emb_layer_norm_after (lna_*) -> dense [d, d] + GELU -> LayerNorm (ln_*) -> out_w [vocab, d]
+ * (+ out_b, or NULL) -> out [P, vocab] log-probabilities. scratch_a / scratch_b: caller-owned [P, d] fp32 each. d + vocab <= 12288. */
+typedef struct {
+  const float* x; int32_t d; int32_t T;
+  const int32_t* row_in_seq; int32_t P; int32_t all_rows;
+  const float* lna_g; const float* lna_b;
+  const float* dense_w; const float* dense_b;
+  const float* ln_g; const float* ln_b;
+  const float* out_w; const float* out_b;
+  int32_t vocab;
+  float* scratch_a; float* scratch_b;
+  float* out;
+} pg_mlm_head_args;
+int pg_mlm_head(const pg_mlm_head_args* args, pg_stream stream);
+
+/* The autoregressive head on B right-padded sequences of T fp32 rows x [B * T, d]: ln_f (lnf_g / lnf_b, or both NULL for none) ->
+ * wte [vocab, d] (+ bias [vocab], or NULL) -> log_softmax -> the retrieval fusion of f (NULL = none; as pg_ar_loglik_fused, with
+ * first_col <= vocab) -> tok_logp[b * T + t] = log p(ids[b * T + t + 1]) for t < lens[b] - 1, the label of token id v being column
+ * v - label_off; 0 at t >= lens[b] - 1 and where the next token equals ignore_id (>= 0; -1 = none); NaN for a label outside
+ * [0, vocab). out_sum[b] = sum of tok_logp over t < lens[b] - 1. d + vocab <= 12288. */
+typedef struct {
+  const float* x; int32_t d; int32_t B; int32_t T; int32_t vocab;
+  const int32_t* ids; const int32_t* lens;
+  const float* lnf_g; const float* lnf_b;
+  const float* wte; const float* bias;
+  int32_t label_off; int32_t ignore_id;
+  float* tok_logp; float* out_sum;
+} pg_ar_head_args;
+int pg_ar_head(const pg_ar_head_args* args, const pg_ar_fusion* f, pg_stream stream);
+
+/* The combine that follows pg_gemm_form's epi 7 over B sequences of T rows: part [B * T, tiles] float pairs (max, sum exp) and tgt [B * T]
+ * as epi 7 writes them -> tok_logp[r] = tgt[r] - logsumexp of row r's partials (0 at t >= lens[b] - 1, NaN for a next token outside
+ * [0, vocab)); out_logprobs (NULL, or [B * T, vocab] holding the logits) becomes log-probabilities in place on those rows;
+ * out_sum[b] = the sum of tok_logp over t < lens[b] - 1. */
+int pg_lm_combine(const float* part, int32_t tiles, const float* tgt, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T,
+                  int32_t vocab, float* out_logprobs, float* tok_logp, float* out_sum, pg_stream stream);
 
 /* ---- MSA pre-processing for the Tranception retrieval prior (SURVEY.md §8f rank 2) ----
  * pg_msa_cluster_neighbors replaces calc_num_cluster_members_nogaps[_parallel] (proteingym/utils/weights.py:114-216):

@@ -63,6 +63,31 @@ class PgArFusion(C.Structure):
                 ("first_col", C.c_int32), ("out_logprobs", C.c_void_p)]
 
 
+class PgLnForm(C.Structure):
+    _fields_ = [("dp", C.c_int32), ("perm_R", C.c_int32), ("perm_C", C.c_int32), ("base", C.c_void_p), ("base_T", C.c_int32)]
+
+
+class PgEsmEmbedArgs(C.Structure):
+    _fields_ = [("tokens", C.c_void_p), ("n_tokens", C.c_int32), ("positions", C.c_void_p), ("win_start", C.c_void_p),
+                ("P", C.c_int32), ("T", C.c_int32), ("d", C.c_int32), ("embed", C.c_void_p), ("pos_table", C.c_void_p),
+                ("lnb_gamma", C.c_void_p), ("lnb_beta", C.c_void_p), ("token_dropout", C.c_int32), ("mask_idx", C.c_int32),
+                ("p_offset", C.c_int32), ("force_mask_scale", C.c_int32), ("x", C.c_void_p)]
+
+
+class PgMlmHeadArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("d", C.c_int32), ("T", C.c_int32), ("row_in_seq", C.c_void_p), ("P", C.c_int32),
+                ("all_rows", C.c_int32)] + [(n, C.c_void_p) for n in ("lna_g", "lna_b", "dense_w", "dense_b", "ln_g", "ln_b",
+                                                                      "out_w", "out_b")] + \
+        [("vocab", C.c_int32), ("scratch_a", C.c_void_p), ("scratch_b", C.c_void_p), ("out", C.c_void_p)]
+
+
+class PgArHeadArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("d", C.c_int32), ("B", C.c_int32), ("T", C.c_int32), ("vocab", C.c_int32),
+                ("ids", C.c_void_p), ("lens", C.c_void_p), ("lnf_g", C.c_void_p), ("lnf_b", C.c_void_p),
+                ("wte", C.c_void_p), ("bias", C.c_void_p), ("label_off", C.c_int32), ("ignore_id", C.c_int32),
+                ("tok_logp", C.c_void_p), ("out_sum", C.c_void_p)]
+
+
 # every symbol include/pgscore.h declares, with its ctypes signature
 SIGNATURES = {
     "pg_abi_version": (C.c_int, []),
@@ -92,9 +117,19 @@ SIGNATURES = {
     "pg_gemm_form": (C.c_int, [C.POINTER(PgGemmArgs), C.POINTER(PgGemmForm), C.c_void_p]),
     "pg_layernorm_f16": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                    C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]),
+    "pg_layernorm_form": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                    C.c_int64, C.c_int64, C.c_int32, C.c_float, C.POINTER(PgLnForm), C.c_void_p]),
     "pg_pack_weight": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_attention": (C.c_int, [C.POINTER(PgAttnArgs), C.c_void_p]),
     "pg_attention_form": (C.c_int, [C.POINTER(PgAttnArgs), C.POINTER(PgAttnForm), C.c_void_p]),
+    "pg_attention_rows": (C.c_int, [C.POINTER(PgAttnArgs), C.c_void_p, C.c_void_p]),
+    "pg_qk_ln_rotary": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_int32, C.c_void_p]),
+    "pg_esm_embed": (C.c_int, [C.POINTER(PgEsmEmbedArgs), C.c_void_p]),
+    "pg_mlm_head": (C.c_int, [C.POINTER(PgMlmHeadArgs), C.c_void_p]),
+    "pg_ar_head": (C.c_int, [C.POINTER(PgArHeadArgs), C.POINTER(PgArFusion), C.c_void_p]),
+    "pg_lm_combine": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_msa_cluster_neighbors": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_msa_prior": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p, C.c_void_p]),
     "pg_eve_output_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),

@@ -1776,9 +1776,17 @@ int pg_gemm_form(const pg_gemm_args* a, const struct pg_gemm_form* f, pg_stream 
 
 int pg_layernorm_f16(const float* x, int64_t ldx, const float* gamma, const float* beta, int32_t rows, int32_t d, void* out,
                      int64_t ldo, int64_t lo_off, int32_t fmt, float scale, pg_stream stream) {
+  return pg_layernorm_form(x, ldx, gamma, beta, rows, d, out, ldo, lo_off, fmt, scale, nullptr, stream);
+}
+
+int pg_layernorm_form(const float* x, int64_t ldx, const float* gamma, const float* beta, int32_t rows, int32_t d, void* out,
+                      int64_t ldo, int64_t lo_off, int32_t fmt, float scale, const pg_ln_form* f, pg_stream stream) {
   if (!x || !gamma || !beta || !out) return set_error(PG_ERR_ARG, "pg_layernorm_f16: null buffer");
+  if (rows < 0 || d <= 0) return set_error(PG_ERR_ARG, "pg_layernorm_f16: bad rows / d");
+  const pg_ln_form p = f ? *f : pg_ln_form{};
+  if (p.dp < 0 || p.perm_R < 0 || p.perm_C < 0 || p.base_T < 0) return set_error(PG_ERR_ARG, "pg_layernorm_form: negative form field");
   return launch_layernorm_f16(x, ldx, gamma, beta, rows, d, static_cast<__half*>(out), ldo, lo_off, static_cast<cudaStream_t>(stream),
-                              fmt ? fmt : -1, scale);
+                              fmt ? fmt : -1, scale, p.perm_R, p.perm_C, static_cast<const __half*>(p.base), p.base_T, p.dp);
 }
 
 int pg_pack_weight(const float* w, int32_t N, int32_t K, int32_t fmt, void* out, float* w_inv, pg_stream stream) {
@@ -1825,6 +1833,95 @@ int pg_attention_form(const pg_attn_args* a, const pg_attn_form* f, pg_stream st
   if (a->impl != 1) return set_error(PG_ERR_ARG, "pg_attention: impl must be 0 (the model's wgmma kernel) or 1 (mma.sync cross-check)");
   if (l.out_fmt == 2) return set_error(PG_ERR_UNSUPPORTED, "pg_attention: the mma.sync cross-check kernel writes fp16 planes only");
   return launch_attention(l, static_cast<cudaStream_t>(stream));
+}
+
+int pg_attention_rows(const pg_attn_args* a, const int32_t* row_sel, pg_stream stream) {
+  if (!a || !a->qkv || !a->out || !row_sel) return set_error(PG_ERR_ARG, "pg_attention_rows: null args");
+  if (a->B < 0 || a->T <= 0 || a->heads <= 0) return set_error(PG_ERR_ARG, "pg_attention_rows: bad B / T / heads");
+  if (a->nseg != 1 && a->nseg != 3) return set_error(PG_ERR_ARG, "pg_attention_rows: nseg must be 1 or 3");
+  const int64_t d = static_cast<int64_t>(a->heads) * 64, lo = a->nseg == 3 ? a->lo_off : 0;
+  if ((a->nseg == 3 && lo < 3 * d) || a->ld < lo + 3 * d || a->ld % 8 || lo % 8)
+    return set_error(PG_ERR_ARG, "pg_attention_rows: q/k/v rows need 3 * heads * 64 columns per plane and pitches that are multiples of 8");
+  if (a->causal || a->alibi_slopes || a->impl || a->base_o || a->mask_pos || a->cout)
+    return set_error(PG_ERR_UNSUPPORTED, "pg_attention_rows: bidirectional attention without bias or delta operands only");
+  int out_fmt = a->out_fmt ? a->out_fmt : -1;
+  if (int rc = resolve_out_fmt(out_fmt, a->out_lo_off, a->out_scale, "pg_attention_rows")) return rc;
+  if (a->ldo < d || (out_fmt > 0 && (a->out_lo_off < d || a->ldo < a->out_lo_off + d)))  // fmt 2: two e4m3 planes of d bytes
+    return set_error(PG_ERR_ARG, "pg_attention_rows: output rows too narrow for their planes");
+  ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream));
+  return launch_attn_single_query(static_cast<const __half*>(a->qkv), a->ld, lo, row_sel, a->B, a->T, a->heads, static_cast<__half*>(a->out),
+                                  a->ldo, a->out_lo_off, static_cast<cudaStream_t>(stream), out_fmt, a->out_scale);
+}
+
+int pg_qk_ln_rotary(void* qkv, int64_t ld, int64_t lo_off, int32_t rows, int32_t heads, const float* q_gamma, const float* k_gamma,
+                    const float* rot_cos, const float* rot_sin, int32_t T, pg_stream stream) {
+  if (!qkv) return set_error(PG_ERR_ARG, "pg_qk_ln_rotary: null buffer");
+  if (rows < 0 || lo_off < 0) return set_error(PG_ERR_ARG, "pg_qk_ln_rotary: bad rows / lo_off");
+  const int64_t d2 = 2 * static_cast<int64_t>(heads) * 64;
+  if ((lo_off > 0 && lo_off < d2) || ld < lo_off + d2) return set_error(PG_ERR_ARG, "pg_qk_ln_rotary: rows too narrow for [q | k] planes");
+  ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream));
+  return launch_qk_ln_rotary(static_cast<__half*>(qkv), ld, lo_off, rows, heads, q_gamma, k_gamma, rot_cos, rot_sin, T,
+                             static_cast<cudaStream_t>(stream));
+}
+
+int pg_esm_embed(const pg_esm_embed_args* a, pg_stream stream) {
+  if (!a || !a->tokens || !a->embed || !a->x) return set_error(PG_ERR_ARG, "pg_esm_embed: null args");
+  if (a->P < 0 || a->T <= 0 || a->d <= 0 || a->n_tokens <= 0 || a->p_offset < 0)
+    return set_error(PG_ERR_ARG, "pg_esm_embed: bad P / T / d / n_tokens / p_offset");
+  if ((a->lnb_gamma == nullptr) != (a->lnb_beta == nullptr)) return set_error(PG_ERR_ARG, "pg_esm_embed: lnb_gamma and lnb_beta go together");
+  EmbedLaunch e{};
+  e.tokens = a->tokens; e.n_tokens = a->n_tokens; e.positions = a->positions; e.win_start = a->win_start;
+  e.P = a->P; e.T = a->T; e.d = a->d; e.embed = a->embed; e.pos_table = a->pos_table;
+  e.lnb_gamma = a->lnb_gamma; e.lnb_beta = a->lnb_beta;
+  e.token_dropout = a->token_dropout; e.mask_idx = a->mask_idx; e.p_offset = a->p_offset; e.force_mask_scale = a->force_mask_scale;
+  e.x = a->x;
+  ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream));
+  return launch_embed(e, static_cast<cudaStream_t>(stream));
+}
+
+int pg_mlm_head(const pg_mlm_head_args* a, pg_stream stream) {
+  if (!a || !a->x || !a->lna_g || !a->lna_b || !a->dense_w || !a->dense_b || !a->ln_g || !a->ln_b || !a->out_w || !a->scratch_a ||
+      !a->scratch_b || !a->out)
+    return set_error(PG_ERR_ARG, "pg_mlm_head: null args");
+  if (a->P < 0 || a->d <= 0 || a->vocab <= 0) return set_error(PG_ERR_ARG, "pg_mlm_head: bad P / d / vocab");
+  if (!a->all_rows && (!a->row_in_seq || a->T <= 0)) return set_error(PG_ERR_ARG, "pg_mlm_head: row_in_seq needs T > 0 (or set all_rows)");
+  if (a->d + a->vocab > 12288) return set_error(PG_ERR_ARG, "pg_mlm_head: d + vocab floats exceed 48 KB of shared memory");
+  HeadLaunch h{};
+  h.x = a->x; h.d = a->d; h.T = a->T; h.row_in_seq = a->row_in_seq; h.P = a->P; h.all_rows = a->all_rows;
+  h.lna_g = a->lna_g; h.lna_b = a->lna_b; h.dense_w = a->dense_w; h.dense_b = a->dense_b;
+  h.ln_g = a->ln_g; h.ln_b = a->ln_b; h.out_w = a->out_w; h.out_b = a->out_b; h.vocab = a->vocab;
+  h.scratch_a = a->scratch_a; h.scratch_b = a->scratch_b; h.out = a->out;
+  ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream), 3);
+  return launch_head(h, static_cast<cudaStream_t>(stream));
+}
+
+int pg_ar_head(const pg_ar_head_args* a, const pg_ar_fusion* f, pg_stream stream) {
+  if (!a || !a->x || !a->ids || !a->lens || !a->wte || !a->tok_logp || !a->out_sum) return set_error(PG_ERR_ARG, "pg_ar_head: null args");
+  if (a->B < 0 || a->T <= 0 || a->d <= 0 || a->vocab <= 0) return set_error(PG_ERR_ARG, "pg_ar_head: bad B / T / d / vocab");
+  if ((a->lnf_g == nullptr) != (a->lnf_b == nullptr)) return set_error(PG_ERR_ARG, "pg_ar_head: lnf_g and lnf_b go together");
+  if (a->d + a->vocab > 12288) return set_error(PG_ERR_ARG, "pg_ar_head: d + vocab floats exceed 48 KB of shared memory");
+  ArFusion fu;
+  if (f) {
+    if ((f->log_prior == nullptr) != (f->prior_row == nullptr)) return set_error(PG_ERR_ARG, "pg_ar_head: log_prior and prior_row go together");
+    if ((f->log_prior2 == nullptr) != (f->prior_row2 == nullptr)) return set_error(PG_ERR_ARG, "pg_ar_head: log_prior2 and prior_row2 go together");
+    if (f->log_prior2 && !f->log_prior) return set_error(PG_ERR_ARG, "pg_ar_head: the second prior needs the first");
+    if (f->first_col < 0 || f->first_col > a->vocab) return set_error(PG_ERR_ARG, "pg_ar_head: first_col outside the vocabulary");
+    fu.log_prior = f->log_prior; fu.prior_row = f->prior_row; fu.alpha = f->alpha;
+    fu.log_prior2 = f->log_prior2; fu.prior_row2 = f->prior_row2; fu.beta = f->beta;
+    fu.first_col = f->first_col; fu.out_logprobs = f->out_logprobs;
+  }
+  ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream), 2);
+  return launch_ar_head(a->x, a->d, a->B, a->T, a->vocab, a->ids, a->lens, a->lnf_g, a->lnf_b, a->wte, a->bias, a->label_off, fu,
+                        a->tok_logp, a->out_sum, static_cast<cudaStream_t>(stream), a->ignore_id);
+}
+
+int pg_lm_combine(const float* part, int32_t tiles, const float* tgt, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T,
+                  int32_t vocab, float* out_logprobs, float* tok_logp, float* out_sum, pg_stream stream) {
+  if (!part || !tgt || !ids || !lens || !tok_logp || !out_sum) return set_error(PG_ERR_ARG, "pg_lm_combine: null buffer");
+  if (B < 0 || T <= 0 || tiles <= 0 || vocab <= 0) return set_error(PG_ERR_ARG, "pg_lm_combine: bad B / T / tiles / vocab");
+  ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream), 2);
+  return launch_lm_head_combine(reinterpret_cast<const float2*>(part), tiles, tgt, ids, lens, B, T, vocab, out_logprobs, tok_logp, out_sum,
+                                static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -125,7 +125,10 @@ typedef struct {
 /* Replaces pretrained.load_model_and_alphabet + model.cuda() (compute_fitness.py:349-353; esm/pretrained.py:24-218):
  * create a model instance, then hand it the (already key-normalised) fp32 state dict; the library repacks into its own
  * operand buffers (q scaling folded in, multihead_attention.py:261). pg_load_weights is SYNCHRONOUS: it runs on the default
- * stream and returns after the repack has finished, so the caller may free its tensors immediately.
+ * stream and returns after the repack has finished, so the caller may free its tensors immediately. pg_create allocates the
+ * workspace; pg_load_weights allocates every weight buffer, so an out-of-memory error can come from either. Call pg_load_weights
+ * once per handle: a second call returns PG_ERR_STATE, whether or not the first succeeded (after a failed load, destroy the
+ * handle and create a new one).
  * Limits of one handle: head_dim 64; a pass holds at most max_rows token rows and 8192 sequences (longer inputs are processed
  * in several passes inside the call; results do not depend on the split). */
 int pg_create(const pg_model_desc* desc, pg_handle* out);
@@ -142,7 +145,8 @@ const char* pg_last_error(pg_handle h); /* h may be NULL: returns the last creat
  *              sequence; NULL = positions[p]
  *   T          window length (<= 1024 for ESM-1b; tokens per row)
  *   out_logprobs [P, vocab] fp32 (device): log_softmax(logits)[out_row - win_start]
- * All rows share T (no padding exists on this path). */
+ * All rows share T (no padding exists on this path). PG_ARCH_ESM1B, PG_ARCH_ESM2 and PG_ARCH_ESMC handles only (others:
+ * PG_ERR_STATE); the same holds for pg_forward_logprobs. */
 int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, const int32_t* positions,
                         const int32_t* win_start, const int32_t* out_row, int32_t P, int32_t T, float* out_logprobs,
                         pg_stream stream);

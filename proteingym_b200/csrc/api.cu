@@ -263,6 +263,7 @@ __global__ void interleave_gate_up_kernel(const float* __restrict__ src, int f, 
 struct pg_handle_s {
   pg_model_desc desc{};
   pg::OpFmt op;
+  bool load_called = false;  // pg_load_weights runs once per handle
   bool loaded = false;
   std::string err;
   std::vector<void*> allocs;
@@ -290,8 +291,6 @@ struct pg_handle_s {
   float *tok_logp = nullptr, *slopes = nullptr;
   // exact wild-type-prefix reuse (pg_ar_prefix_begin / pg_ar_loglik_prefix): per layer, the wild type's raw q/k/v rows (conv
   // look-back) and conv'd q/k/v rows (keys / values of the shared prefix), [layers][prefix_T][3d*np] fp16 each
-  unsigned int* pack_scratch = nullptr;  // one word per packed matrix (absmax of the matrix), [layers * 6]
-  int pack_used = 0;
   __half *raw_cache = nullptr, *kv_cache = nullptr;
   int prefix_T = 0;        // rows recorded by the last pg_ar_prefix_begin (0 = none)
   int prefix_cap = 0;      // rows the caches can hold
@@ -312,12 +311,11 @@ struct pg_handle_s {
   __half* cq = nullptr;
   // PoET (pg_poet_context / pg_poet_loglik): the context record, per layer the multi-sequence attention's q/k/v rows of the context
   // ([layers][mem_T][3da*np] fp16; the rotated k and the v columns are read), regrown on demand (not in `allocs`); rotary positions and
-  // segment starts of the context rows [max_rows]; whether the head has its LayerNorm (norm=True)
+  // segment starts of the context rows [max_rows]
   __half* mem = nullptr;
   size_t mem_bytes = 0;
   int mem_T = -1;  // rows of the current record; -1 = none, 0 = an empty context
   int32_t *ctx_pos = nullptr, *ctx_seg = nullptr;
-  bool head_norm = false;
 };
 
 namespace pg {
@@ -325,6 +323,15 @@ namespace {
 
 bool is_ar(int arch) {
   return arch == PG_ARCH_TRANCEPTION || arch == PG_ARCH_RITA || arch == PG_ARCH_PROGEN2 || arch == PG_ARCH_PROTGPT2;
+}
+
+// Why a handle cannot run pg_masked_marginals / pg_forward_logprobs, or null: only ESM-1b, ESM2 and ESM C handles hold the ESM stack's
+// weights and its MLM head.
+const char* not_esm(int arch) {
+  if (arch == PG_ARCH_ESM1B || arch == PG_ARCH_ESM2 || arch == PG_ARCH_ESMC) return nullptr;
+  if (is_ar(arch)) return "handle is an autoregressive model (use pg_ar_loglik)";
+  if (arch == PG_ARCH_MSA) return "handle is an MSA Transformer (use pg_msa_masked_marginals)";
+  return "handle is not an ESM-1b, ESM2 or ESM C model";
 }
 
 int fail(pg_handle h, int code, const std::string& msg) {
@@ -1046,60 +1053,16 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   h->label_off = D.arch == PG_ARCH_PROGEN2 ? 5 : 0;
   const int d = D.embed_dim, f = D.ffn_dim, np = h->op.np, dk = h->op.dk, da = h->op.da;
   const int dw = dk > da ? dk : da;  // abuf / cabuf hold both LayerNorm outputs (dk) and attention outputs (da)
+  // the workspace only: pg_load_weights allocates every buffer a tensor fills
   int rc = PG_OK;
   auto A = [&](auto** p, size_t n) { if (!rc) rc = dev_alloc(h, p, n); };
-  h->layers.resize(D.layers);
-  const bool esmc = D.arch == PG_ARCH_ESMC;
-  const int f1 = esmc ? 2 * f : f;  // rows of fc1: ESM C holds the SwiGLU gate and up halves
-  for (auto& L : h->layers) {
-    A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
-    A(&L.w1, static_cast<size_t>(f1) * dk * np); A(&L.w2, static_cast<size_t>(d) * f * np);
-    if (!esmc && D.arch != PG_ARCH_PROGEN2) {  // ESM C and ProGen2 attention: no bias (null = none); PoET: out_proj only
-      if (D.arch != PG_ARCH_POET) A(&L.bqkv, 3 * da);
-      A(&L.bo, d);
-    }
-    if (!esmc) { A(&L.b1, f); A(&L.b2, d); }  // ESM C MLP: no bias
-    A(&L.ln1g, d); A(&L.ln1b, d); A(&L.ln2g, d); A(&L.ln2b, d);
-    if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); A(&L.i1, f1); A(&L.i2, d); }
-    if (D.arch == PG_ARCH_TRANCEPTION) A(&L.conv_taps, 3 * 4 * 64 * 8);
-    if (esmc) { A(&L.qlng, d); A(&L.klng, d); }
-  }
-  if (esmc || D.arch == PG_ARCH_RITA || D.arch == PG_ARCH_PROGEN2 || D.arch == PG_ARCH_POET) A(&h->outw, static_cast<size_t>(D.vocab) * d);
-  if (D.arch == PG_ARCH_POET) {  // multihead_attn blocks; context positions and segment starts
-    h->col_layers.resize(D.layers);
-    for (auto& L : h->col_layers) {
-      A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
-      A(&L.bo, d); A(&L.ln1g, d); A(&L.ln1b, d);
-      if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); }
-    }
-    A(&h->ctx_pos, static_cast<size_t>(h->max_rows)); A(&h->ctx_seg, static_cast<size_t>(h->max_rows));
-    A(&h->tok_logp, static_cast<size_t>(h->max_rows));
-  }
-  if (D.arch == PG_ARCH_MSA) {
-    h->col_layers.resize(D.layers);
-    for (auto& L : h->col_layers) {
-      A(&L.wqkv, static_cast<size_t>(3) * da * dk * np); A(&L.wo, static_cast<size_t>(d) * da * np);
-      A(&L.bqkv, 3 * da); A(&L.bo, d); A(&L.ln1g, d); A(&L.ln1b, d);
-      if (h->op.nseg == 2) { A(&L.iqkv, 3 * da); A(&L.io, d); }
-    }
-    A(&h->row_pos, static_cast<size_t>(1024) * d);
-  }
-  if (D.arch == PG_ARCH_TRANCEPTION) {
-    A(&h->qkv2, static_cast<size_t>(h->max_rows) * 3 * d * np);
-    A(&h->slopes, D.heads);
-  }
-  if (is_ar(D.arch)) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
+  if (D.arch == PG_ARCH_POET) { A(&h->ctx_pos, static_cast<size_t>(h->max_rows)); A(&h->ctx_seg, static_cast<size_t>(h->max_rows)); }
+  if (D.arch == PG_ARCH_TRANCEPTION) A(&h->qkv2, static_cast<size_t>(h->max_rows) * 3 * d * np);
+  if (is_ar(D.arch) || D.arch == PG_ARCH_POET) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
   if (D.arch == PG_ARCH_PROTGPT2) {  // 8 B per row and N tile: 412 MB at the default 131 072 rows and 50 257 columns
-    A(&h->lmw, static_cast<size_t>(D.vocab) * dk * np);
     A(&h->lm_part, static_cast<size_t>(h->max_rows) * ((D.vocab + GEMM_BN - 1) / GEMM_BN));
     A(&h->lm_tgt, static_cast<size_t>(h->max_rows));
-    A(&h->pos, static_cast<size_t>(D.max_positions) * d);
   }
-  if (h->op.nseg == 2) A(&h->pack_scratch, static_cast<size_t>(D.layers) * 6);
-  A(&h->embed, static_cast<size_t>(D.vocab) * d);
-  if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA) A(&h->pos, static_cast<size_t>(D.max_positions + 2) * d);
-  A(&h->lnbg, d); A(&h->lnbb, d); A(&h->lnag, d); A(&h->lnab, d);
-  A(&h->hdw, static_cast<size_t>(d) * d); A(&h->hdb, d); A(&h->hlng, d); A(&h->hlnb, d); A(&h->hbias, D.vocab);
   A(&h->x, static_cast<size_t>(h->max_rows) * d);
   A(&h->abuf, static_cast<size_t>(h->max_rows) * dw * np);
   A(&h->qkv, static_cast<size_t>(h->max_rows) * 3 * da * np);
@@ -1134,9 +1097,13 @@ int pg_destroy(pg_handle h) {
 
 int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
   if (!h || !tensors) return set_error(PG_ERR_ARG, "pg_load_weights: null argument");
+  if (h->load_called) return fail(h, PG_ERR_STATE, "pg_load_weights: called before on this handle (one load per handle)");
+  h->load_called = true;
   PG_CUDA_OK(cudaSetDevice(h->desc.device));
   const pg_model_desc& D = h->desc;
-  const int d = D.embed_dim, f = D.ffn_dim, np = h->op.np;
+  const int d = D.embed_dim, f = D.ffn_dim, V = D.vocab, np = h->op.np, hd = d / D.heads, dk = h->op.dk, da = h->op.da;
+  // head_dim^-1/2 (multihead_attention.py:103,261), folded into the fp32 q weights and bias: 0.125 (exact) for head_dim 64
+  const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(hd)));
   std::map<std::string, const pg_tensor*> by_name;
   for (int i = 0; i < n; ++i) by_name[tensors[i].name] = &tensors[i];
   std::string missing;
@@ -1146,81 +1113,126 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     if (it->second->shape[0] != r || it->second->shape[1] != c) { missing += name + "(shape) "; return nullptr; }
     return static_cast<const float*>(it->second->data);
   };
-  struct Scratch {  // weights expanded to the padded operand layout (ESM2 head slots); cudaFree waits for the packing kernels
-    std::vector<float*> p;
-    ~Scratch() { for (float* q : p) cudaFree(q); }
-  } expanded;
-  cudaError_t exp_err = cudaSuccess;
+  int rc = PG_OK;  // the first failed allocation of a handle buffer
+  auto alloc = [&](auto** p, size_t cnt) { if (!rc) rc = dev_alloc(h, p, cnt); return !rc; };
+  struct Scratch {  // buffers that live for the load only; cudaFree waits for the kernels that read them
+    std::vector<void*> p;
+    ~Scratch() { for (void* q : p) cudaFree(q); }
+  } scratch;
+  cudaError_t scratch_err = cudaSuccess;
+  auto tmp = [&](size_t bytes) -> void* {
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, bytes);
+    if (e != cudaSuccess) { if (!scratch_err) scratch_err = e; return nullptr; }
+    scratch.p.push_back(p);
+    return p;
+  };
   auto copy = [&](float* dst, const float* src, size_t cnt, float scale = 1.f) {
-    if (!src) return;
     scale_copy_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256>>>(src, dst, static_cast<int>(cnt), scale);
   };
-  // A group of [N, K] weights that form one GEMM operand, packed into dst (inv: where the per-row 1/t of PG_PREC_F16F8 go).
-  // Conv1D weights are stored [in = K, out = N]; conv_ld: their row pitch when the N columns are a slice of a wider matrix.
-  auto pack = [&](__half* dst, float* inv, std::initializer_list<PackSrc> group, int N, int K, bool conv1d = false, long long conv_ld = 0) {
+  // dst = src [cnt] * scale in a buffer allocated here (nothing when src is null: get() has reported it)
+  auto put = [&](float** dst, const float* src, size_t cnt, float scale = 1.f) {
+    if (src && alloc(dst, cnt)) copy(*dst, src, cnt, scale);
+  };
+  auto vec = [&](float** dst, const std::string& name, int64_t r, int64_t c = 1, float scale = 1.f) {
+    put(dst, get(name, r, c), static_cast<size_t>(r) * c, scale);
+  };
+  auto norm = [&](float** g, float** b, const std::string& p) { vec(g, p + "weight", d); vec(b, p + "bias", d); };
+  // q, k and v biases of n each into one [3n] buffer, q scaled by qs
+  auto bias3 = [&](float** dst, const float* q, const float* k, const float* v, int cnt, float qs) {
+    if (!q || !k || !v || !alloc(dst, 3 * static_cast<size_t>(cnt))) return;
+    copy(*dst, q, cnt, qs); copy(*dst + cnt, k, cnt); copy(*dst + 2 * cnt, v, cnt);
+  };
+  // A group of [N, K] weights that form one GEMM operand, packed into a buffer allocated here (inv: the per-row 1/t of
+  // PG_PREC_F16F8, one e4m3 scale for the group). Conv1D weights are stored [in = K, out]: conv_ld = their row pitch.
+  // Packing runs in order on stream 0, so one absmax word serves every group.
+  const bool f8 = h->op.nseg == 2;
+  unsigned int* f8_word = f8 ? static_cast<unsigned int*>(tmp(sizeof(unsigned int))) : nullptr;
+  auto pack = [&](__half** w, float** inv, std::initializer_list<PackSrc> group, int N, int K, long long conv_ld = 0) {
     for (const PackSrc& m : group)
       if (!m.w) return;
-    unsigned int* f8_scratch = h->op.nseg == 2 ? h->pack_scratch + (h->pack_used++ % (D.layers * 6)) : nullptr;
-    pack_weights(group, N, K, conv1d ? 1 : K, conv1d ? (conv_ld ? conv_ld : N) : 1, np, f8_scratch, dst, inv, 0);
+    const size_t g = group.size();
+    if ((f8 && !f8_word) || !alloc(w, g * N * K * np) || (f8 && !alloc(inv, g * N))) return;
+    pack_weights(group, N, K, conv_ld ? 1 : K, conv_ld ? conv_ld : 1, np, f8_word, *w, f8 ? *inv : nullptr, 0);
   };
-  // "rotary.cos" / "rotary.sin" [T, S/2] (ESM C, RITA: [T, 32]; ProGen2: half its slot width) -> the tables of the rotary GEMM epilogue
-  auto rotary32 = [&]() -> int {
-    const int hs = h->op.slot / 2;
-    auto it = by_name.find("rotary.cos");
-    auto is = by_name.find("rotary.sin");
-    if (it == by_name.end() || is == by_name.end() || it->second->shape[1] != hs || is->second->shape[1] != hs ||
-        is->second->shape[0] != it->second->shape[0]) {
-      missing += "rotary.cos/rotary.sin[T," + std::to_string(hs) + "] ";
-      return PG_OK;
-    }
-    h->rot_rows = static_cast<int>(it->second->shape[0]);
-    int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * hs);
-    if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * hs);
-    if (rc) return rc;
-    copy(h->rot_cos, static_cast<const float*>(it->second->data), static_cast<size_t>(h->rot_rows) * hs);
-    copy(h->rot_sin, static_cast<const float*>(is->second->data), static_cast<size_t>(h->rot_rows) * hs);
-    return PG_OK;
-  };
-  const int hd = d / D.heads;
-  // A [n_src, k_src] source weight placed in the padded operand layout [N, K] (OpFmt, slot maps rmap / cmap), in a scratch buffer
-  // freed on return; the source itself when the layout is unpadded. The ProGen2 maps read rows of the fused [3d, d] qkv_proj.
+  // A [n_src, k_src] source weight placed in the padded operand layout [N, K] (OpFmt, slot maps rmap / cmap), in a scratch buffer;
+  // the source itself when the layout is unpadded. The ProGen2 maps read rows of the fused [3d, d] qkv_proj.
   auto slots = [&](const float* w, int n_src, int k_src, int N, int K, int rmap, int cmap) -> const float* {
     if (!w || (N == n_src && K == k_src && rmap != SL_ILV)) return w;
-    float* p = nullptr;
-    const cudaError_t e = cudaMalloc(&p, static_cast<size_t>(N) * K * sizeof(float));
-    if (e != cudaSuccess) {
-      if (!exp_err) exp_err = e;
-      return nullptr;
-    }
-    expanded.p.push_back(p);
+    float* p = static_cast<float*>(tmp(static_cast<size_t>(N) * K * sizeof(float)));
+    if (!p) return nullptr;
     const long long tot = static_cast<long long>(N) * K;
     const int rn = rmap >= SL_PGQ ? n_src / 3 : n_src;
     expand_slots_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(w, rn, k_src, p, N, K, rmap, cmap, hd, h->op.slot, k_src);
     return p;
   };
+  // "rotary.cos" / "rotary.sin" [T, w] -> the rotary epilogue's tables [T, S/2], zero after column w. w is S/2, or `alt` (ESM2:
+  // checkpoint.rotary_tables writes [T, head_dim/2]). `full`: the tables must cover max_positions rows.
+  auto rotary = [&](int alt, bool full) {
+    const int hs = h->op.slot / 2;
+    auto it = by_name.find("rotary.cos"), is = by_name.find("rotary.sin");
+    const int64_t w = it == by_name.end() ? 0 : it->second->shape[1];
+    if (it == by_name.end() || is == by_name.end() || (w != hs && w != alt) || is->second->shape[1] != w ||
+        is->second->shape[0] != it->second->shape[0]) {
+      missing += "rotary.cos/rotary.sin[T," + std::to_string(alt) + "] ";
+      return;
+    }
+    h->rot_rows = static_cast<int>(it->second->shape[0]);
+    if (full && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
+    for (auto [dst, src] : {std::make_pair(&h->rot_cos, it->second->data), std::make_pair(&h->rot_sin, is->second->data)})
+      if (alloc(dst, static_cast<size_t>(h->rot_rows) * hs))
+        expand_slots_kernel<<<(h->rot_rows * hs + 255) / 256, 256>>>(static_cast<const float*>(src), h->rot_rows, static_cast<int>(w), *dst,
+                                                                     h->rot_rows, hs, SL_PAD, SL_PAD, hd, h->op.slot, static_cast<int>(w));
+  };
+  // One attention block: q/k/v/out projections at `pa`, its LayerNorm at `pl`. q, k and v form ONE GEMM operand (one common e4m3
+  // scale, q already scaled), the q / k rows placed by qk_map and the v rows by SL_HEAD into the head slots.
+  auto attn = [&](Layer& L, const std::string& pa, const std::string& pl, int qk_map, bool qkv_bias) {
+    const float* wq = slots(get(pa + "q_proj.weight", d, d), d, d, da, dk, qk_map, SL_PAD);
+    const float* wk = slots(get(pa + "k_proj.weight", d, d), d, d, da, dk, qk_map, SL_PAD);
+    const float* wv = slots(get(pa + "v_proj.weight", d, d), d, d, da, dk, SL_HEAD, SL_PAD);
+    pack(&L.wqkv, &L.iqkv, {{wq, qscale}, wk, wv}, da, dk);
+    if (qkv_bias)
+      bias3(&L.bqkv, slots(get(pa + "q_proj.bias", d, 1), d, 1, da, 1, qk_map, SL_PAD), slots(get(pa + "k_proj.bias", d, 1), d, 1, da, 1, qk_map, SL_PAD),
+            slots(get(pa + "v_proj.bias", d, 1), d, 1, da, 1, SL_HEAD, SL_PAD), da, qscale);
+    pack(&L.wo, &L.io, {slots(get(pa + "out_proj.weight", d, d), d, d, d, da, SL_PAD, SL_HEAD)}, d, da);
+    vec(&L.bo, pa + "out_proj.bias", d);
+    norm(&L.ln1g, &L.ln1b, pl);
+  };
+  // The MLP's fc1 [f, d] (its columns padded to dk) and fc2 [d, f] with their biases, at "<p1>weight" / "<p1>bias" and p2.
+  auto ffn = [&](Layer& L, const std::string& p1, const std::string& p2) {
+    pack(&L.w1, &L.i1, {slots(get(p1 + "weight", f, d), f, d, f, dk, SL_PAD, SL_PAD)}, f, dk);
+    vec(&L.b1, p1 + "bias", f);
+    pack(&L.w2, &L.i2, {get(p2 + "weight", d, f)}, d, f);
+    vec(&L.b2, p2 + "bias", d);
+  };
+  // A GPT-2 block at "h.{l}." (transformers modeling_gpt2.py GPT2Attention / GPT2MLP, Conv1D weights [in, out]): c_attn's q, k and v
+  // column blocks form one GEMM operand with qs folded into the q columns and bias.
+  auto gpt2_block = [&](Layer& L, const std::string& p, float qs) {
+    const float* wa = get(p + "attn.c_attn.weight", d, 3 * d);
+    pack(&L.wqkv, &L.iqkv, {{wa, qs}, wa ? wa + d : nullptr, wa ? wa + 2 * d : nullptr}, d, d, 3 * d);
+    const float* ba = get(p + "attn.c_attn.bias", 3 * d, 1);
+    bias3(&L.bqkv, ba, ba ? ba + d : nullptr, ba ? ba + 2 * d : nullptr, d, qs);
+    pack(&L.wo, &L.io, {get(p + "attn.c_proj.weight", d, d)}, d, d, d);
+    vec(&L.bo, p + "attn.c_proj.bias", d);
+    pack(&L.w1, &L.i1, {get(p + "mlp.c_fc.weight", d, f)}, f, d, f);
+    vec(&L.b1, p + "mlp.c_fc.bias", f);
+    pack(&L.w2, &L.i2, {get(p + "mlp.c_proj.weight", f, d)}, d, f, d);
+    vec(&L.b2, p + "mlp.c_proj.bias", d);
+    norm(&L.ln1g, &L.ln1b, p + "ln_1.");
+    norm(&L.ln2g, &L.ln2b, p + "ln_2.");
+  };
+  h->layers.resize(D.layers);
+  if (D.arch == PG_ARCH_MSA || D.arch == PG_ARCH_POET) h->col_layers.resize(D.layers);
   if (D.arch == PG_ARCH_TRANCEPTION) {
     // HF GPT2-style names with the "transformer." prefix stripped by the host
     for (int l = 0; l < D.layers; ++l) {
-      Layer& L = h->layers[l];
       const std::string p = "h." + std::to_string(l) + ".";
-      pack(L.wqkv, L.iqkv, {get(p + "attn.c_attn.weight", d, 3 * d)}, 3 * d, d, true);
-      copy(L.bqkv, get(p + "attn.c_attn.bias", 3 * d, 1), 3 * d);
-      pack(L.wo, L.io, {get(p + "attn.c_proj.weight", d, d)}, d, d, true);
-      copy(L.bo, get(p + "attn.c_proj.bias", d, 1), d);
-      pack(L.w1, L.i1, {get(p + "mlp.c_fc.weight", d, f)}, f, d, true);
-      copy(L.b1, get(p + "mlp.c_fc.bias", f, 1), f);
-      pack(L.w2, L.i2, {get(p + "mlp.c_proj.weight", f, d)}, d, f, true);
-      copy(L.b2, get(p + "mlp.c_proj.bias", d, 1), d);
-      copy(L.ln1g, get(p + "ln_1.weight", d, 1), d);
-      copy(L.ln1b, get(p + "ln_1.bias", d, 1), d);
-      copy(L.ln2g, get(p + "ln_2.weight", d, 1), d);
-      copy(L.ln2b, get(p + "ln_2.bias", d, 1), d);
-      copy(L.conv_taps, get(p + "attn.conv_taps", 3 * 4 * 64, 8), 3 * 4 * 64 * 8);
+      gpt2_block(h->layers[l], p, 1.f);
+      vec(&h->layers[l].conv_taps, p + "attn.conv_taps", 3 * 4 * 64, 8);
     }
-    copy(h->embed, get("wte.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    copy(h->lnag, get("ln_f.weight", d, 1), d);
-    copy(h->lnab, get("ln_f.bias", d, 1), d);
-    copy(h->slopes, get("alibi_slopes", D.heads, 1), D.heads);
+    vec(&h->embed, "wte.weight", V, d);
+    norm(&h->lnag, &h->lnab, "ln_f.");
+    vec(&h->slopes, "alibi_slopes", D.heads);
   } else if (D.arch == PG_ARCH_ESMC) {
     // evoscale key names (esm/models/esmc.py:63-76, layers/blocks.py:35-43,95-110, layers/attention.py:28-39). Residual branches are
     // divided by s = sqrt(layers / 36) (transformer_stack.py:48-50, blocks.py:150-160): 1/s is folded into out_proj and fc2 here.
@@ -1228,39 +1240,28 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     for (int l = 0; l < D.layers; ++l) {
       Layer& L = h->layers[l];
       const std::string p = "transformer.blocks." + std::to_string(l) + ".";
-      copy(L.ln1g, get(p + "attn.layernorm_qkv.0.weight", d, 1), d);
-      copy(L.ln1b, get(p + "attn.layernorm_qkv.0.bias", d, 1), d);
-      pack(L.wqkv, L.iqkv, {get(p + "attn.layernorm_qkv.1.weight", 3 * d, d)}, 3 * d, d);
-      copy(L.qlng, get(p + "attn.q_ln.weight", d, 1), d);
-      copy(L.klng, get(p + "attn.k_ln.weight", d, 1), d);
-      pack(L.wo, L.io, {{get(p + "attn.out_proj.weight", d, d), rs}}, d, d);
-      copy(L.ln2g, get(p + "ffn.0.weight", d, 1), d);
-      copy(L.ln2b, get(p + "ffn.0.bias", d, 1), d);
+      norm(&L.ln1g, &L.ln1b, p + "attn.layernorm_qkv.0.");
+      pack(&L.wqkv, &L.iqkv, {get(p + "attn.layernorm_qkv.1.weight", 3 * d, d)}, 3 * d, d);
+      vec(&L.qlng, p + "attn.q_ln.weight", d);
+      vec(&L.klng, p + "attn.k_ln.weight", d);
+      pack(&L.wo, &L.io, {{get(p + "attn.out_proj.weight", d, d), rs}}, d, d);
+      norm(&L.ln2g, &L.ln2b, p + "ffn.0.");
       const float* w1 = get(p + "ffn.1.weight", 2 * f, d);
-      if (w1) {  // gate / up rows interleaved in blocks of 8 for the SwiGLU epilogue
-        float* t = nullptr;
-        const cudaError_t e = cudaMalloc(&t, static_cast<size_t>(2) * f * d * sizeof(float));
-        if (e != cudaSuccess) {
-          if (!exp_err) exp_err = e;
-        } else {
-          expanded.p.push_back(t);
-          const long long tot = 2LL * f * d;
-          interleave_gate_up_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256>>>(w1, f, d, t);
-          pack(L.w1, L.i1, {t}, 2 * f, d);
-        }
-      }
-      pack(L.w2, L.i2, {{get(p + "ffn.3.weight", d, f), rs}}, d, f);
+      float* t = w1 ? static_cast<float*>(tmp(static_cast<size_t>(2) * f * d * sizeof(float))) : nullptr;
+      if (t)  // gate / up rows interleaved in blocks of 8 for the SwiGLU epilogue
+        interleave_gate_up_kernel<<<static_cast<unsigned>((2LL * f * d + 255) / 256), 256>>>(w1, f, d, t);
+      pack(&L.w1, &L.i1, {t}, 2 * f, d);
+      pack(&L.w2, &L.i2, {{get(p + "ffn.3.weight", d, f), rs}}, d, f);
     }
-    copy(h->embed, get("embed.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    copy(h->lnag, get("transformer.norm.weight", d, 1), d);
-    PG_CUDA_OK(cudaMemset(h->lnab, 0, static_cast<size_t>(d) * sizeof(float)));  // the final norm has no bias
-    copy(h->hdw, get("sequence_head.0.weight", d, d), static_cast<size_t>(d) * d);
-    copy(h->hdb, get("sequence_head.0.bias", d, 1), d);
-    copy(h->hlng, get("sequence_head.2.weight", d, 1), d);
-    copy(h->hlnb, get("sequence_head.2.bias", d, 1), d);
-    copy(h->outw, get("sequence_head.3.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    copy(h->hbias, get("sequence_head.3.bias", D.vocab, 1), D.vocab);
-    if (int rc = rotary32()) return rc;
+    vec(&h->embed, "embed.weight", V, d);
+    vec(&h->lnag, "transformer.norm.weight", d);
+    if (alloc(&h->lnab, d)) PG_CUDA_OK(cudaMemset(h->lnab, 0, static_cast<size_t>(d) * sizeof(float)));  // the final norm has no bias
+    vec(&h->hdw, "sequence_head.0.weight", d, d);
+    vec(&h->hdb, "sequence_head.0.bias", d);
+    norm(&h->hlng, &h->hlnb, "sequence_head.2.");
+    vec(&h->outw, "sequence_head.3.weight", V, d);
+    vec(&h->hbias, "sequence_head.3.bias", V);
+    rotary(h->op.slot / 2, false);
   } else if (D.arch == PG_ARCH_RITA) {
     // HF names without the "transformer." prefix (rita_modeling.py:113-121, 185-194, 222-224). q, k and v form one GEMM operand with
     // 1/sqrt(64) = 0.125 folded into the q rows and bias: exact (a power of two), and it commutes with the (linear) rotary.
@@ -1268,204 +1269,97 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
       Layer& L = h->layers[l];
       const std::string p = "layers." + std::to_string(l) + ".";
       const std::string a = p + "self_attention.";
-      pack(L.wqkv, L.iqkv, {{get(a + "query.weight", d, d), 0.125f}, get(a + "key.weight", d, d), get(a + "value.weight", d, d)}, d, d);
-      copy(L.bqkv, get(a + "query.bias", d, 1), d, 0.125f);
-      copy(L.bqkv + d, get(a + "key.bias", d, 1), d);
-      copy(L.bqkv + 2 * d, get(a + "value.bias", d, 1), d);
-      pack(L.wo, L.io, {get(a + "proj.weight", d, d)}, d, d);
-      copy(L.bo, get(a + "proj.bias", d, 1), d);
-      copy(L.ln1g, get(p + "attn_norm.weight", d, 1), d);
-      copy(L.ln1b, get(p + "attn_norm.bias", d, 1), d);
-      pack(L.w1, L.i1, {get(p + "mlp.0.weight", f, d)}, f, d);
-      copy(L.b1, get(p + "mlp.0.bias", f, 1), f);
-      pack(L.w2, L.i2, {get(p + "mlp.2.weight", d, f)}, d, f);
-      copy(L.b2, get(p + "mlp.2.bias", d, 1), d);
-      copy(L.ln2g, get(p + "mlp_norm.weight", d, 1), d);
-      copy(L.ln2b, get(p + "mlp_norm.bias", d, 1), d);
+      pack(&L.wqkv, &L.iqkv, {{get(a + "query.weight", d, d), 0.125f}, get(a + "key.weight", d, d), get(a + "value.weight", d, d)}, d, d);
+      bias3(&L.bqkv, get(a + "query.bias", d, 1), get(a + "key.bias", d, 1), get(a + "value.bias", d, 1), d, 0.125f);
+      pack(&L.wo, &L.io, {get(a + "proj.weight", d, d)}, d, d);
+      vec(&L.bo, a + "proj.bias", d);
+      norm(&L.ln1g, &L.ln1b, p + "attn_norm.");
+      ffn(L, p + "mlp.0.", p + "mlp.2.");
+      norm(&L.ln2g, &L.ln2b, p + "mlp_norm.");
     }
-    copy(h->embed, get("embedding.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    copy(h->lnag, get("final_norm.weight", d, 1), d);
-    copy(h->lnab, get("final_norm.bias", d, 1), d);
+    vec(&h->embed, "embedding.weight", V, d);
+    norm(&h->lnag, &h->lnab, "final_norm.");
     // the output head: "lm_head.weight" when the caller passes it (an untied checkpoint), else the embedding matrix
-    if (by_name.count("lm_head.weight")) copy(h->outw, get("lm_head.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    else copy(h->outw, get("embedding.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    if (int rc = rotary32()) return rc;
-    if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
+    vec(&h->outw, by_name.count("lm_head.weight") ? "lm_head.weight" : "embedding.weight", V, d);
+    rotary(h->op.slot / 2, true);
   } else if (D.arch == PG_ARCH_PROTGPT2) {
-    // GPT-2 names without the "transformer." prefix (transformers modeling_gpt2.py GPT2Attention / GPT2MLP / GPT2Model), Conv1D weights
-    // [in, out]. c_attn's q, k and v column blocks form one GEMM operand with 1/sqrt(64) = 0.125 folded into the q columns and bias
-    // (exact: a power of two). The head is wte itself (tied), packed once more as a [vocab, d] operand for K16.
-    for (int l = 0; l < D.layers; ++l) {
-      Layer& L = h->layers[l];
-      const std::string p = "h." + std::to_string(l) + ".";
-      const float* wa = get(p + "attn.c_attn.weight", d, 3 * d);
-      pack(L.wqkv, L.iqkv, {{wa, 0.125f}, wa ? wa + d : nullptr, wa ? wa + 2 * d : nullptr}, d, d, true, 3 * d);
-      const float* ba = get(p + "attn.c_attn.bias", 3 * d, 1);
-      copy(L.bqkv, ba, d, 0.125f);
-      copy(L.bqkv + d, ba ? ba + d : nullptr, 2 * d);
-      pack(L.wo, L.io, {get(p + "attn.c_proj.weight", d, d)}, d, d, true);
-      copy(L.bo, get(p + "attn.c_proj.bias", d, 1), d);
-      pack(L.w1, L.i1, {get(p + "mlp.c_fc.weight", d, f)}, f, d, true);
-      copy(L.b1, get(p + "mlp.c_fc.bias", f, 1), f);
-      pack(L.w2, L.i2, {get(p + "mlp.c_proj.weight", f, d)}, d, f, true);
-      copy(L.b2, get(p + "mlp.c_proj.bias", d, 1), d);
-      copy(L.ln1g, get(p + "ln_1.weight", d, 1), d);
-      copy(L.ln1b, get(p + "ln_1.bias", d, 1), d);
-      copy(L.ln2g, get(p + "ln_2.weight", d, 1), d);
-      copy(L.ln2b, get(p + "ln_2.bias", d, 1), d);
-    }
-    const float* wte = get("wte.weight", D.vocab, d);
-    copy(h->embed, wte, static_cast<size_t>(D.vocab) * d);
-    if (wte) pack_weights({wte}, D.vocab, d, d, 1, np, nullptr, h->lmw, nullptr, 0);  // fp16 hi [| lo] in every mode
-    copy(h->pos, get("wpe.weight", D.max_positions, d), static_cast<size_t>(D.max_positions) * d);
-    copy(h->lnag, get("ln_f.weight", d, 1), d);
-    copy(h->lnab, get("ln_f.bias", d, 1), d);
+    // GPT-2 names without the "transformer." prefix, 1/sqrt(64) = 0.125 folded into q (exact: a power of two). The head is wte itself
+    // (tied), packed once more as a [vocab, d] operand for K16.
+    for (int l = 0; l < D.layers; ++l) gpt2_block(h->layers[l], "h." + std::to_string(l) + ".", 0.125f);
+    const float* wte = get("wte.weight", V, d);
+    put(&h->embed, wte, static_cast<size_t>(V) * d);
+    if (wte && alloc(&h->lmw, static_cast<size_t>(V) * h->op.dk * np))
+      pack_weights({wte}, V, d, d, 1, np, nullptr, h->lmw, nullptr, 0);  // fp16 hi [| lo] in every mode
+    vec(&h->pos, "wpe.weight", D.max_positions, d);
+    norm(&h->lnag, &h->lnab, "ln_f.");
   } else if (D.arch == PG_ARCH_POET) {
-    // PoET names (poet/models/poet.py without the checkpoint's "model." prefix). q, k and v of each attention form one GEMM operand
-    // without bias, the q rows scaled by 1/sqrt(64) = 0.125 (flash-attn's default softmax scale; exact), the q and k rows permuted by
-    // SL_ILV. norm=False checkpoints carry no "norm.*": the head then reads the residual stream directly.
-    auto attn = [&](Layer& L, const std::string& pa, const std::string& pn) {
-      const float* wq = slots(get(pa + "q_proj.weight", d, d), d, d, d, d, SL_ILV, SL_PAD);
-      const float* wk = slots(get(pa + "k_proj.weight", d, d), d, d, d, d, SL_ILV, SL_PAD);
-      pack(L.wqkv, L.iqkv, {{wq, 0.125f}, wk, get(pa + "v_proj.weight", d, d)}, d, d);
-      pack(L.wo, L.io, {get(pa + "out_proj.weight", d, d)}, d, d);
-      copy(L.bo, get(pa + "out_proj.bias", d, 1), d);
-      copy(L.ln1g, get(pn + ".weight", d, 1), d);
-      copy(L.ln1b, get(pn + ".bias", d, 1), d);
-    };
+    // PoET names (poet/models/poet.py without the checkpoint's "model." prefix). The attentions have no q/k/v bias; q is scaled by
+    // 1/sqrt(64) = 0.125 (flash-attn's default softmax scale; exact), the q and k rows permuted by SL_ILV. norm=False checkpoints
+    // carry no "norm.*": the head then reads the residual stream directly (h->lnag stays null).
     for (int l = 0; l < D.layers; ++l) {
       Layer& L = h->layers[l];
       const std::string p = "decoder.layers." + std::to_string(l) + ".";
-      attn(L, p + "self_attn.", p + "norm1");
-      attn(h->col_layers[l], p + "multihead_attn.", p + "norm2");
-      pack(L.w1, L.i1, {get(p + "linear1.weight", f, d)}, f, d);
-      copy(L.b1, get(p + "linear1.bias", f, 1), f);
-      pack(L.w2, L.i2, {get(p + "linear2.weight", d, f)}, d, f);
-      copy(L.b2, get(p + "linear2.bias", d, 1), d);
-      copy(L.ln2g, get(p + "norm3.weight", d, 1), d);
-      copy(L.ln2b, get(p + "norm3.bias", d, 1), d);
+      attn(L, p + "self_attn.", p + "norm1.", SL_ILV, false);
+      attn(h->col_layers[l], p + "multihead_attn.", p + "norm2.", SL_ILV, false);
+      ffn(L, p + "linear1.", p + "linear2.");
+      norm(&L.ln2g, &L.ln2b, p + "norm3.");
     }
-    copy(h->embed, get("token_embed.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    copy(h->outw, get("linear.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    copy(h->hbias, get("linear.bias", D.vocab, 1), D.vocab);
-    h->head_norm = by_name.count("norm.weight") > 0;
-    if (h->head_norm) {
-      copy(h->lnag, get("norm.weight", d, 1), d);
-      copy(h->lnab, get("norm.bias", d, 1), d);
-    }
-    if (int rc = rotary32()) return rc;
-    if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
+    vec(&h->embed, "token_embed.weight", V, d);
+    vec(&h->outw, "linear.weight", V, d);
+    vec(&h->hbias, "linear.bias", V);
+    if (by_name.count("norm.weight")) norm(&h->lnag, &h->lnab, "norm.");
+    rotary(h->op.slot / 2, true);
   } else if (D.arch == PG_ARCH_PROGEN2) {
     // HF names without the "transformer." prefix (modeling_progen.py:84-95, 209-226, 389-401, 541-548). qkv_proj [3d, d] is placed
     // into the head slots by SL_PGQ / SL_PGK / SL_PGV (one GEMM operand, no bias) with head_dim^-1/2 folded into the q rows: exact
     // for head_dim 64, one fp32 rounding for 80 and 96. out_proj's columns take the SL_HEAD slots. The head is rows 5..29 of
     // lm_head (weight and bias): the reference's log-softmax runs over exactly those columns (compute_fitness.py:71-77).
-    const int da = h->op.da;
-    const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(hd)));
     for (int l = 0; l < D.layers; ++l) {
       Layer& L = h->layers[l];
       const std::string p = "h." + std::to_string(l) + ".";
       const float* wqkv = get(p + "attn.qkv_proj.weight", 3 * d, d);
-      pack(L.wqkv, L.iqkv, {{slots(wqkv, 3 * d, d, da, d, SL_PGQ, SL_PAD), qscale}, slots(wqkv, 3 * d, d, da, d, SL_PGK, SL_PAD),
-                            slots(wqkv, 3 * d, d, da, d, SL_PGV, SL_PAD)}, da, d);
-      pack(L.wo, L.io, {slots(get(p + "attn.out_proj.weight", d, d), d, d, d, da, SL_PAD, SL_HEAD)}, d, da);
-      copy(L.ln1g, get(p + "ln_1.weight", d, 1), d);
-      copy(L.ln1b, get(p + "ln_1.bias", d, 1), d);
-      pack(L.w1, L.i1, {get(p + "mlp.fc_in.weight", f, d)}, f, d);
-      copy(L.b1, get(p + "mlp.fc_in.bias", f, 1), f);
-      pack(L.w2, L.i2, {get(p + "mlp.fc_out.weight", d, f)}, d, f);
-      copy(L.b2, get(p + "mlp.fc_out.bias", d, 1), d);
+      pack(&L.wqkv, &L.iqkv, {{slots(wqkv, 3 * d, d, da, d, SL_PGQ, SL_PAD), qscale}, slots(wqkv, 3 * d, d, da, d, SL_PGK, SL_PAD),
+                              slots(wqkv, 3 * d, d, da, d, SL_PGV, SL_PAD)}, da, d);
+      pack(&L.wo, &L.io, {slots(get(p + "attn.out_proj.weight", d, d), d, d, d, da, SL_PAD, SL_HEAD)}, d, da);
+      norm(&L.ln1g, &L.ln1b, p + "ln_1.");
+      ffn(L, p + "mlp.fc_in.", p + "mlp.fc_out.");
     }
-    copy(h->embed, get("wte.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    copy(h->lnag, get("ln_f.weight", d, 1), d);
-    copy(h->lnab, get("ln_f.bias", d, 1), d);
-    const float* hw = get("lm_head.weight", D.vocab, d);
-    const float* hb = get("lm_head.bias", D.vocab, 1);
-    copy(h->outw, hw ? hw + static_cast<size_t>(h->label_off) * d : nullptr, static_cast<size_t>(h->head_vocab) * d);
-    copy(h->hbias, hb ? hb + h->label_off : nullptr, h->head_vocab);
-    if (int rc = rotary32()) return rc;
-    if (h->rot_rows && h->rot_rows < D.max_positions) missing += "rotary.cos/rotary.sin(fewer than max_positions rows) ";
+    vec(&h->embed, "wte.weight", V, d);
+    norm(&h->lnag, &h->lnab, "ln_f.");
+    const float* hw = get("lm_head.weight", V, d);
+    const float* hb = get("lm_head.bias", V, 1);
+    put(&h->outw, hw ? hw + static_cast<size_t>(h->label_off) * d : nullptr, static_cast<size_t>(h->head_vocab) * d);
+    put(&h->hbias, hb ? hb + h->label_off : nullptr, h->head_vocab);
+    rotary(h->op.slot / 2, true);
   } else {
-    const int dk = h->op.dk, da = h->op.da;
-    // head_dim^-1/2 (multihead_attention.py:103,261), folded into the fp32 q weights and bias: 0.125 (exact) for head_dim 64
-    const float qscale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(hd)));
-    // one attention block: q/k/v/out projections at `pa` ("...self_attn." / "...row_self_attention.layer."), its LayerNorm at `pl`
-    auto load_attn = [&](Layer& L, const std::string& pa, const std::string& pl) {
-      // q, k, v form ONE GEMM operand: one common e4m3 scale (matrix maximum over the three, q already scaled)
-      const float* wq = slots(get(pa + "q_proj.weight", d, d), d, d, da, dk, SL_ROT, SL_PAD);
-      const float* wk = slots(get(pa + "k_proj.weight", d, d), d, d, da, dk, SL_ROT, SL_PAD);
-      const float* wv = slots(get(pa + "v_proj.weight", d, d), d, d, da, dk, SL_HEAD, SL_PAD);
-      pack(L.wqkv, L.iqkv, {{wq, qscale}, wk, wv}, da, dk);
-      copy(L.bqkv, slots(get(pa + "q_proj.bias", d, 1), d, 1, da, 1, SL_ROT, SL_PAD), da, qscale);
-      copy(L.bqkv + da, slots(get(pa + "k_proj.bias", d, 1), d, 1, da, 1, SL_ROT, SL_PAD), da);
-      copy(L.bqkv + 2 * da, slots(get(pa + "v_proj.bias", d, 1), d, 1, da, 1, SL_HEAD, SL_PAD), da);
-      pack(L.wo, L.io, {slots(get(pa + "out_proj.weight", d, d), d, d, d, da, SL_PAD, SL_HEAD)}, d, da);
-      copy(L.bo, get(pa + "out_proj.bias", d, 1), d);
-      copy(L.ln1g, get(pl + "weight", d, 1), d);
-      copy(L.ln1b, get(pl + "bias", d, 1), d);
-    };
-    auto load_ffn = [&](Layer& L, const std::string& pf, const std::string& pl) {
-      pack(L.w1, L.i1, {slots(get(pf + "fc1.weight", f, d), f, d, f, dk, SL_PAD, SL_PAD)}, f, dk);
-      copy(L.b1, get(pf + "fc1.bias", f, 1), f);
-      pack(L.w2, L.i2, {get(pf + "fc2.weight", d, f)}, d, f);
-      copy(L.b2, get(pf + "fc2.bias", d, 1), d);
-      copy(L.ln2g, get(pl + "weight", d, 1), d);
-      copy(L.ln2b, get(pl + "bias", d, 1), d);
-    };
     for (int l = 0; l < D.layers; ++l) {
+      Layer& L = h->layers[l];
       const std::string p = "layers." + std::to_string(l) + ".";
       if (D.arch == PG_ARCH_MSA) {  // AxialTransformerLayer (modules.py:194-196): three NormalizedResidualBlocks {layer, layer_norm}
-        load_attn(h->layers[l], p + "row_self_attention.layer.", p + "row_self_attention.layer_norm.");
-        load_attn(h->col_layers[l], p + "column_self_attention.layer.", p + "column_self_attention.layer_norm.");
-        load_ffn(h->layers[l], p + "feed_forward_layer.layer.", p + "feed_forward_layer.layer_norm.");
+        attn(L, p + "row_self_attention.layer.", p + "row_self_attention.layer_norm.", SL_ROT, true);
+        attn(h->col_layers[l], p + "column_self_attention.layer.", p + "column_self_attention.layer_norm.", SL_ROT, true);
+        ffn(L, p + "feed_forward_layer.layer.fc1.", p + "feed_forward_layer.layer.fc2.");
+        norm(&L.ln2g, &L.ln2b, p + "feed_forward_layer.layer_norm.");
       } else {
-        load_attn(h->layers[l], p + "self_attn.", p + "self_attn_layer_norm.");
-        load_ffn(h->layers[l], p, p + "final_layer_norm.");
+        attn(L, p + "self_attn.", p + "self_attn_layer_norm.", SL_ROT, true);
+        ffn(L, p + "fc1.", p + "fc2.");
+        norm(&L.ln2g, &L.ln2b, p + "final_layer_norm.");
       }
     }
-    if (D.arch == PG_ARCH_MSA) {
-      auto it = by_name.find("msa_position_embedding");  // host-expanded to [1024, d] (the first release stores a 1-wide table)
-      if (it != by_name.end()) {
-        if (it->second->shape[0] != 1024 || it->second->shape[1] != d) missing += "msa_position_embedding(shape) ";
-        else copy(h->row_pos, static_cast<const float*>(it->second->data), static_cast<size_t>(1024) * d);
-      } else {
-        h->row_pos = nullptr;  // embed_positions_msa off (msa_transformer.py:106-114)
-      }
-    }
-    copy(h->embed, get("embed_tokens.weight", D.vocab, d), static_cast<size_t>(D.vocab) * d);
-    if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA)
-      copy(h->pos, get("embed_positions.weight", D.max_positions + 2, d), static_cast<size_t>(D.max_positions + 2) * d);
-    if (D.emb_ln_before || D.arch == PG_ARCH_MSA) {
-      copy(h->lnbg, get("emb_layer_norm_before.weight", d, 1), d);
-      copy(h->lnbb, get("emb_layer_norm_before.bias", d, 1), d);
-    }
-    copy(h->lnag, get("emb_layer_norm_after.weight", d, 1), d);
-    copy(h->lnab, get("emb_layer_norm_after.bias", d, 1), d);
-    copy(h->hdw, get("lm_head.dense.weight", d, d), static_cast<size_t>(d) * d);
-    copy(h->hdb, get("lm_head.dense.bias", d, 1), d);
-    copy(h->hlng, get("lm_head.layer_norm.weight", d, 1), d);
-    copy(h->hlnb, get("lm_head.layer_norm.bias", d, 1), d);
-    copy(h->hbias, get("lm_head.bias", D.vocab, 1), D.vocab);
-    if (D.arch == PG_ARCH_ESM2) {
-      // cos / sin [T, hd/2] (checkpoint.rotary_tables) or [T, 32] -> device tables [T, 32], zero after column hd/2
-      auto it = by_name.find("rotary.cos");
-      auto is = by_name.find("rotary.sin");
-      const int64_t rw = it == by_name.end() ? 0 : it->second->shape[1];
-      if (it == by_name.end() || is == by_name.end() || (rw != 32 && rw != hd / 2) || is->second->shape[1] != rw ||
-          is->second->shape[0] != it->second->shape[0]) {
-        missing += "rotary.cos/rotary.sin[T,head_dim/2] ";
-      } else {
-        h->rot_rows = static_cast<int>(it->second->shape[0]);
-        int rc = dev_alloc(h, &h->rot_cos, static_cast<size_t>(h->rot_rows) * 32);
-        if (!rc) rc = dev_alloc(h, &h->rot_sin, static_cast<size_t>(h->rot_rows) * 32);
-        if (rc) return rc;
-        for (auto [dst, src] : {std::make_pair(h->rot_cos, it->second->data), std::make_pair(h->rot_sin, is->second->data)})
-          expand_slots_kernel<<<(h->rot_rows * 32 + 255) / 256, 256>>>(static_cast<const float*>(src), h->rot_rows, static_cast<int>(rw), dst,
-                                                                       h->rot_rows, 32, SL_PAD, SL_PAD, hd, 64, static_cast<int>(rw));
-      }
-    }
+    // host-expanded to [1024, d] (the first release stores a 1-wide table); absent: embed_positions_msa off (msa_transformer.py:106-114)
+    if (D.arch == PG_ARCH_MSA && by_name.count("msa_position_embedding")) vec(&h->row_pos, "msa_position_embedding", 1024, d);
+    vec(&h->embed, "embed_tokens.weight", V, d);
+    if (D.arch == PG_ARCH_ESM1B || D.arch == PG_ARCH_MSA) vec(&h->pos, "embed_positions.weight", D.max_positions + 2, d);
+    if (D.emb_ln_before || D.arch == PG_ARCH_MSA) norm(&h->lnbg, &h->lnbb, "emb_layer_norm_before.");
+    norm(&h->lnag, &h->lnab, "emb_layer_norm_after.");
+    vec(&h->hdw, "lm_head.dense.weight", d, d);
+    vec(&h->hdb, "lm_head.dense.bias", d);
+    norm(&h->hlng, &h->hlnb, "lm_head.layer_norm.");
+    vec(&h->hbias, "lm_head.bias", V);
+    if (D.arch == PG_ARCH_ESM2) rotary(hd / 2, false);
   }
-  if (exp_err != cudaSuccess) return fail(h, PG_ERR_CUDA, std::string("pg_load_weights: cudaMalloc: ") + cudaGetErrorString(exp_err));
+  if (rc) return rc;
+  if (scratch_err != cudaSuccess) return fail(h, PG_ERR_CUDA, std::string("pg_load_weights: cudaMalloc: ") + cudaGetErrorString(scratch_err));
   if (!missing.empty()) return fail(h, PG_ERR_ARG, "pg_load_weights: missing or mis-shaped tensors: " + missing);
   PG_CUDA_OK(cudaGetLastError());
   PG_CUDA_OK(cudaDeviceSynchronize());  // caller may free its tensors on return
@@ -1477,8 +1371,7 @@ int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, co
                         const int32_t* out_row, int32_t P, int32_t T, float* out_logprobs, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_masked_marginals: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_masked_marginals: weights not loaded");
-  if (is_ar(h->desc.arch)) return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is an autoregressive model (use pg_ar_loglik)");
-  if (h->desc.arch == PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_masked_marginals: handle is an MSA Transformer (use pg_msa_masked_marginals)");
+  if (const char* why = not_esm(h->desc.arch)) return fail(h, PG_ERR_STATE, std::string("pg_masked_marginals: ") + why);
   if (!tokens || !positions || !out_logprobs) return fail(h, PG_ERR_ARG, "pg_masked_marginals: null buffer");
   if (P < 0 || T <= 0 || T > n_tokens) return fail(h, PG_ERR_ARG, "pg_masked_marginals: bad P/T");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions)
@@ -1541,8 +1434,7 @@ int pg_forward_logprobs(pg_handle h, const int32_t* tokens, int32_t n_tokens, in
                         float* out_logprobs, pg_stream stream) {
   if (!h) return set_error(PG_ERR_ARG, "pg_forward_logprobs: null handle");
   if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: weights not loaded");
-  if (is_ar(h->desc.arch)) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an autoregressive model (use pg_ar_loglik)");
-  if (h->desc.arch == PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: handle is an MSA Transformer (use pg_msa_masked_marginals)");
+  if (const char* why = not_esm(h->desc.arch)) return fail(h, PG_ERR_STATE, std::string("pg_forward_logprobs: ") + why);
   if (!tokens || !out_logprobs || T <= 0 || win_start < 0 || win_start + T > n_tokens) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: bad arguments");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than the learned position table");
   if ((h->desc.arch == PG_ARCH_ESM2 || h->desc.arch == PG_ARCH_ESMC) && T > h->rot_rows)
@@ -1726,7 +1618,7 @@ int pg_poet_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t
     int rc = forward_poet_rows(h, ids + off, Bc, T, s);
     if (rc) return fail(h, rc, tls_error());
     ProfScope ps(CAT_HEAD, s, 2);
-    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->head_norm ? h->lnag : nullptr, h->lnab,
+    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->lnag, h->lnab,
                         h->outw, h->hbias, 0, ArFusion{}, out_tok_logp ? out_tok_logp + off : h->tok_logp, out_sum_logp + b0, s, 23);
     if (rc) return fail(h, rc, tls_error());
   }

@@ -8,7 +8,9 @@ ESM-1v scores in f16x3 / f16f8 / f16d / f16, an ESM2 of the 35M release's shape 
 f16f8, Tranception mutant scores with and without prefix reuse and rows with a three-way retrieval fusion in f16x3 / f16f8, a
 two-layer MSA Transformer table (a full and a pruned last layer) in f16x3 / f16f8, and RITA, ProGen2 and ProtGPT2 scores of a 900-residue
 wild type's substitutions and indels with and without prefix reuse in f16f8. Every run with prefix reuse also records its token-row
-counts (reuse_rows)."""
+counts (reuse_rows). The load paths the runs above leave out have a run each (loads()): ESM C in f16f8 / f16x3, an ESM-1b with
+emb_layer_norm_before, an MSA Transformer without msa_position_embedding, ProGen2 with 80-wide heads (128-wide slots), RITA with an
+untied head, and PoET with and without its final norm in f16x3 / f16f8 (per-token log p and layer 0 of the context record)."""
 import os
 import sys
 
@@ -66,6 +68,7 @@ def collect():
         out[f"msa.{mode}"] = sc.masked_marginal_rows(toks, pos).cpu().numpy()
         sc.close()
     out.update(decoders())
+    out.update(loads())
     return out
 
 
@@ -111,6 +114,72 @@ def decoders():
             out[f"{name}.f16f8.reuse{int(reuse)}"] = sc.score(prots, wt=wt)
             out[f"{name}.f16f8.reuse{int(reuse)}.rows"] = np.asarray(sc.reuse_rows)
         sc.close()
+    return out
+
+
+def loads():
+    """One run per weight-load path that collect() and decoders() do not reach."""
+    from proteingym_b200 import checkpoint, msa_engine, synth
+    from proteingym_b200 import poet_engine as E
+    from proteingym_b200.esm_engine import EsmScorer
+    from proteingym_b200.progen2_engine import Progen2Scorer
+    from proteingym_b200.rita_engine import RitaScorer, RitaTokenizer
+    golden = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
+    out = {}
+    seq = synth.random_protein(150, 21)
+    muts = synth.sample_mutants(seq, 200, 22, multi_frac=0.2)
+    st = synth.make_esmc_state(synth.EsmcArch(2, 256, 512), seed=23)
+    for mode in ("f16f8", "f16x3"):
+        sc = EsmScorer(checkpoint.esmc_config_from_state(st), st, precision=mode)
+        out[f"esmc.{mode}"] = np.asarray(sc.score_assay(seq, muts))
+        sc.close()
+    arch = synth.EsmArch("esm1v", 2, 256, 4, 1024, emb_layer_norm_before=True)
+    sc = EsmScorer(checkpoint.config_from_synth(arch), checkpoint.normalise_synth_state(arch, synth.make_esm_state(arch, seed=24)),
+                   precision="f16f8")
+    out["esm1b_ln_before.f16f8"] = np.asarray(sc.score_assay(seq, muts))
+    sc.close()
+    arch = synth.MsaArch(2, 256, 4, 1024, embed_positions_msa=False)
+    cfg = checkpoint.config_from_msa_synth(arch)
+    st = checkpoint.normalise_msa_synth_state(arch, synth.make_msa_state(arch, 25))
+    toks = msa_engine.tokenize_alignment(synth.random_alignment(synth.random_protein(90, 26), 24, seed=27))
+    R, Cc = toks.shape
+    sc = msa_engine.MsaScorer(cfg, st, precision="f16f8", max_rows=msa_engine.default_max_rows(cfg, R, Cc, want=4))
+    out["msa_no_row_pos.f16f8"] = sc.masked_marginal_rows(toks, np.arange(1, Cc, 7).astype(np.int32)).cpu().numpy()
+    sc.close()
+    wt = synth.random_protein(300, 28)
+    prots = [synth.apply_mutant(wt, m) for m in synth.sample_mutants(wt, 24, 29)] + synth.random_indels(wt, 8, 30)
+    a = synth.Progen2Arch(2, 640, 8, 32)
+    st = synth.make_progen2_state(a, 31, buffers=False)
+    ws = {k[len("transformer."):] if k.startswith("transformer.") else k: v for k, v in st.items()}
+    sc = Progen2Scorer(checkpoint.Progen2Config(a.layers, a.embed_dim, a.heads, a.ffn_dim, a.vocab, a.rotary_dim, a.n_positions), ws,
+                       precision="f16f8")
+    out["progen2_hd80.f16f8"] = sc.score(prots, wt=wt)
+    sc.close()
+    arch = synth.RitaArch(2, 256, 4)
+    st = synth.make_rita_state(arch, 32, untied=True)
+    ws = {k[len("transformer."):] if k.startswith("transformer.") else k: v for k, v in st.items() if "inv_freq" not in k}
+    sc = RitaScorer(checkpoint.RitaConfig(arch.layers, arch.embed_dim, arch.heads, arch.ffn_dim, arch.vocab, False), ws,
+                    st["transformer.layers.0.self_attention.rotary_embedding.inv_freq"],
+                    RitaTokenizer(os.path.join(golden, "rita_tokenizer_plain")), precision="f16f8")
+    out["rita_untied.f16f8"] = sc.score(prots, wt=wt)
+    sc.close()
+    rng = np.random.default_rng(33)
+
+    def row(n):
+        return np.concatenate([[E.START], rng.integers(0, 20, size=n - 2), [E.STOP]]).astype(np.int64)
+    ctx = [row(n) for n in (40, 130, 7, 90)]
+    variants = [row(n) for n in (20, 65, 128, 129)]
+    for norm in (False, True):
+        arch = synth.PoetArch(2, 256, 4, norm=norm)
+        st = synth.make_poet_state(arch, seed=34)
+        conf = checkpoint.PoetConfig(arch.layers, arch.hidden_dim, arch.heads, 4 * arch.hidden_dim, norm)
+        for mode in ("f16x3", "f16f8"):
+            sc = E.PoetScorer(conf, st, 256, precision=mode)
+            sc.set_context(ctx)
+            k, v = sc.record(0)
+            out[f"poet.norm{int(norm)}.{mode}.tok"] = sc.loglik(variants, tok_logp=True)[1]
+            out[f"poet.norm{int(norm)}.{mode}.record0"] = np.concatenate([k.cpu().numpy(), v.cpu().numpy()], axis=1)
+            sc.close()
     return out
 
 

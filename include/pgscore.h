@@ -74,7 +74,7 @@ enum pg_arch {
                               "h.{i}.mlp.c_fc.{weight [d, ffn], bias}", "h.{i}.mlp.c_proj.{weight [ffn, d], bias}", "wte.weight" [vocab, d],
                               "wpe.weight" [max_positions, d], "ln_f.*"): Conv1D weights are [in, out] as for PG_ARCH_TRANCEPTION, and
                               no "lm_head.weight" (tied). LayerNorms use eps 1e-5. */
-  PG_ARCH_POET = 8         /* PoET (proteingym/baselines/PoET/poet/models/poet.py:687-730, modules/transformer.py TieredTransformerEncoderLayer):
+  PG_ARCH_POET = 8,        /* PoET (proteingym/baselines/PoET/poet/models/poet.py:687-730, modules/transformer.py TieredTransformerEncoderLayer):
                               token embedding without positions; per layer x += self_attn(norm1 x) causal within each sequence, x +=
                               multihead_attn(norm2 x) causal over the whole sequence of sequences, x += linear2(erf-GELU(linear1(norm3 x)));
                               q/k/v without bias, out_proj with bias, interleaved rotary over 64-wide heads (positions restart at 0 in
@@ -85,6 +85,25 @@ enum pg_arch {
                               "decoder.layers.{i}.{self_attn,multihead_attn}.{q,k,v}_proj.weight", "...out_proj.{weight,bias}",
                               "decoder.layers.{i}.linear{1,2}.*", "decoder.layers.{i}.norm{1,2,3}.*", "token_embed.weight", "linear.*",
                               optional "norm.*") plus "rotary.cos" / "rotary.sin" [T, 32] = cos / sin(t * inv_freq[2c]) in fp32. */
+  PG_ARCH_PROGEN3 = 9      /* ProGen3 sparse mixture-of-experts causal decoder (proteingym/baselines/progen3/progen3/modeling.py:193-290,
+                              369-495, model/attention.py, model/moe.py:33-134): x = embed_tokens + embed_seq_id[0]; per layer x +=
+                              o_proj(attn(RMSNorm(x))) with bias-free q/k/v projections, kv_heads key / value heads (grouped-query
+                              attention), rotate-half rotary over the whole head (base rope_theta) and causal attention at scale
+                              head_dim^-1/2; then x += moe(RMSNorm(x)): router softmax in fp32, top-k (descending probability, equal
+                              probabilities by lower expert index first), weights renormalised to sum 1, each selected expert's SiLU MLP
+                              (or, gated_mlp, silu(x w1^T) * (x w3^T)) times its weight, added in increasing expert index; final RMSNorm
+                              and the untied head without bias, log-softmax over all `vocab` columns. RMSNorm = x * rsqrt(mean(x^2) +
+                              rms_eps) * weight in fp32. head_dim 64 or 128; PG_PREC_F16D refused; max_positions = the rotary table rows.
+                              Scored through pg_ar_loglik / pg_ar_loglik_fused without retrieval fusion or prefix reuse. Weights
+                              (canonical names; the host maps the eager, fused-norm and megablocks layouts onto them):
+                              "layers.{i}.input_layernorm.weight", "layers.{i}.post_attention_layernorm.weight" [d],
+                              "layers.{i}.self_attn.{q,k,v,o}_proj.weight" ([d, d], [kv_heads*hd, d] x2, [d, d]),
+                              "layers.{i}.block_sparse_moe.gate.weight" [E, d] (not when E == 1), "layers.{i}.block_sparse_moe.w1"
+                              [E*f, d] and (gated_mlp) ".w3" [E*f, d] = the experts' w1 / w3 Linear weights stacked in expert order,
+                              "layers.{i}.block_sparse_moe.w2" [E*d, f] = the experts' w2 Linear weights [d, f] stacked,
+                              "embed_tokens.weight" [vocab, d], "embed_seq_id.weight" [S, d] (row 0 is used), "norm.weight",
+                              "lm_head.weight" [vocab, d], plus "rotary.cos" / "rotary.sin" [T, head_dim/2] = cos / sin(t * rope_theta^(-2c /
+                              head_dim)) in fp32. */
 };
 
 /* Tensor-core operand precision. The reference is strict fp32 (SURVEY.md §0.4). Every operand is an fp16 pair hi + lo.
@@ -114,6 +133,12 @@ typedef struct {
   int32_t precision;       /* pg_precision */
   int32_t device;          /* CUDA device ordinal */
   int32_t max_rows;        /* workspace capacity in token rows (sequences x window length) per pass; 0 = default */
+  /* PG_ARCH_PROGEN3 only (zero elsewhere) */
+  int32_t kv_heads;        /* num_key_value_heads (divides heads) */
+  int32_t n_experts;       /* num_experts, 1..64 */
+  int32_t top_k;           /* num_experts_per_tok, 1..min(n_experts, 8) */
+  int32_t gated_mlp;       /* 1: GLU experts (w1, w3, w2) */
+  float rms_eps;           /* rms_norm_eps */
 } pg_model_desc;
 
 typedef struct {
@@ -134,6 +159,11 @@ typedef struct {
 int pg_create(const pg_model_desc* desc, pg_handle* out);
 int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n);
 int pg_destroy(pg_handle h);
+
+/* PG_ARCH_PROGEN3, for tests: the routing of layer `layer` in the last pass of the last pg_ar_loglik* call (one pass: B * T <= max_rows),
+ * token row r = b * T + t: out_expert[r * top_k + j] / out_weight[r * top_k + j] (device, int32 / fp32) = the j-th selected expert and
+ * its renormalised weight; *out_rows (host) = B * T of that pass. */
+int pg_progen3_routing(pg_handle h, int32_t layer, int32_t* out_expert, float* out_weight, int32_t* out_rows, pg_stream stream);
 const char* pg_last_error(pg_handle h); /* h may be NULL: returns the last creation error */
 
 /* Replaces the masked-marginals loop (compute_fitness.py:486-504) — L+2 batch-1 forwards of
@@ -268,7 +298,10 @@ int pg_score_mutants(const float* table, int32_t n_rows, int32_t vocab, const in
  *   epi 4: as 0 with squared ReLU relu(x)^2 (tranception/activations.py:79-84). bias may be NULL (no bias).
  *   epi 5: SwiGLU silu(g) * v (esm/layers/blocks.py:21-43): w rows interleaved in blocks of 8 (rows 16i..16i+7 = gate rows 8i..8i+7,
  *          rows 16i+8..16i+15 = up rows 8i..8i+7; N % 16 == 0); the output is N/2 columns wide (planes of N/2 columns at out_lo_off,
- *          out_fmt 2 needs N/2 % 64 == 0), column 8i + c = silu(acc[16i + c]) * acc[16i + 8 + c]. */
+ *          out_fmt 2 needs N/2 % 64 == 0), column 8i + c = silu(acc[16i + c]) * acc[16i + 8 + c].
+ *   epi 8: as 0 with SiLU x * sigmoid(x) (ProGen3's experts, progen3/model/moe.py:33-43).
+ *   epi 9: resid[M, ldr] (fp32) = acc + bias (stored, not added: ProGen3's expert outputs per slot).
+ *   The first 2*rot_dim columns of epi 3 must be whole slots (rot_dim a multiple of 32, or of 64 with 128-wide slots). */
 typedef struct {
   const void* a; int64_t lda;
   const void* w; int64_t ldw;
@@ -306,6 +339,11 @@ struct pg_gemm_form {  /* a struct tag only: the entry point below shares its na
   int32_t kchunk;
   int32_t w_uniform;
   float* lm_part; float* lm_tgt; float* lm_logits; const int32_t* lm_ids; const int32_t* lm_lens; int32_t lm_T;
+  /* ragged grouped form (ProGen3's experts): a holds expert segments, each padded to rg_pad rows (128, or 256 for two-CTA clusters that
+   * share the W tile; M a multiple of rg_pad); rg_tiles[0] (device int32) = the rg_pad-row tiles in use, rg_expert[m] (device int32) = the
+   * expert of tile m, whose W rows are [e * grp_rows_b, e * grp_rows_b + N) of a stacked [rg_experts * grp_rows_b, K] w. Tiles past
+   * rg_tiles[0] are not computed (their rows are left untouched). No bias, rotary, LM-head or delta form; nseg 2 needs w_uniform. */
+  const int32_t* rg_expert; const int32_t* rg_tiles; int32_t rg_pad; int32_t rg_experts;
 };
 int pg_gemm_form(const pg_gemm_args* args, const struct pg_gemm_form* form, pg_stream stream);
 
@@ -472,7 +510,9 @@ int pg_profile_end(float* ms, int32_t* counts, int32_t ncat);
  *   "gemm_cta2"    1 (default): the GEMM runs as clusters of two CTAs that share the W tile (each loads half and multicasts it
  *                  to both); 0: one CTA per 128 x 128 tile. PG_GEMM_CTA2.
  *   "gemm_prefetch" k-blocks of L2 look-ahead the GEMM's TMA producer issues for the streamed A operand (default 0 = off: measured
- *                  neutral-to-negative in the model; PG_GEMM_PREFETCH). */
+ *                  neutral-to-negative in the model; PG_GEMM_PREFETCH).
+ *   "moe_pad"      128 (default) or 256: the row multiple each ProGen3 expert segment is padded to; 256 lets the experts' ragged grouped
+ *                  GEMMs run as two-CTA clusters sharing the W tile (when "gemm_cta2" is on), 128 runs them single-CTA with less padding. */
 int pg_set_tuning(const char* key, int32_t value);
 
 

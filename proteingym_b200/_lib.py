@@ -13,13 +13,15 @@ LIB_PATH = os.path.join(_HERE, "libpgscore.so")
 PG_ARCH_ESM1B, PG_ARCH_ESM2, PG_ARCH_TRANCEPTION, PG_ARCH_MSA, PG_ARCH_ESMC, PG_ARCH_RITA, PG_ARCH_PROGEN2 = 0, 1, 2, 3, 4, 5, 6
 PG_ARCH_PROTGPT2 = 7
 PG_ARCH_POET = 8
+PG_ARCH_PROGEN3 = 9
 PG_PREC_F16, PG_PREC_F16X3, PG_PREC_F16F8, PG_PREC_F16D = 0, 1, 2, 3
 PRECISIONS = {"f16": PG_PREC_F16, "f16x3": PG_PREC_F16X3, "f16f8": PG_PREC_F16F8, "f16d": PG_PREC_F16D}
 
 
 class PgModelDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("arch", "layers", "embed_dim", "heads", "ffn_dim", "vocab", "max_positions",
-                                         "token_dropout", "emb_ln_before", "precision", "device", "max_rows")]
+                                         "token_dropout", "emb_ln_before", "precision", "device", "max_rows",
+                                         "kv_heads", "n_experts", "top_k", "gated_mlp")] + [("rms_eps", C.c_float)]
 
 
 class PgTensor(C.Structure):
@@ -54,7 +56,8 @@ class PgAttnForm(C.Structure):
 class PgGemmForm(C.Structure):
     _fields_ = [("rot_pos", C.c_void_p), ("rot_half", C.c_int32), ("kchunk", C.c_int32), ("w_uniform", C.c_int32),
                 ("lm_part", C.c_void_p), ("lm_tgt", C.c_void_p), ("lm_logits", C.c_void_p), ("lm_ids", C.c_void_p),
-                ("lm_lens", C.c_void_p), ("lm_T", C.c_int32)]
+                ("lm_lens", C.c_void_p), ("lm_T", C.c_int32), ("rg_expert", C.c_void_p), ("rg_tiles", C.c_void_p),
+                ("rg_pad", C.c_int32), ("rg_experts", C.c_int32)]
 
 
 class PgArFusion(C.Structure):
@@ -133,6 +136,7 @@ SIGNATURES = {
     "pg_msa_cluster_neighbors": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_msa_prior": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p, C.c_void_p]),
     "pg_eve_output_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "pg_progen3_routing": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
     "pg_set_tuning": (C.c_int, [C.c_char_p, C.c_int32]),
     "pg_launch_count": (C.c_longlong, []),
     "pg_profile_begin": (C.c_int, []),

@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpgscore.so")
-SOURCES = ["api.cu", "gemm_tc.cu", "attention_mma.cu", "attention_wgmma.cu", "elementwise.cu", "tranception.cu", "msa.cu", "msa_transformer.cu"]
+SOURCES = ["api.cu", "gemm_tc.cu", "attention_mma.cu", "attention_wgmma.cu", "elementwise.cu", "tranception.cu", "msa.cu", "msa_transformer.cu", "moe.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC,-O3,-Wall", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 

@@ -494,3 +494,114 @@ def load_poet_checkpoint(path: str):
         raise NotImplementedError("PoET use_multi_rotary=False: the multi-sequence attention is built with rotary positions")
     state = {k.split(".", 1)[1]: v.float() for k, v in ckpt["state_dict"].items()}
     return conf, state
+
+
+@dataclass
+class Progen3Config:
+    layers: int
+    embed_dim: int
+    heads: int
+    kv_heads: int
+    ffn_dim: int
+    vocab: int
+    n_experts: int
+    top_k: int
+    gated_mlp: bool
+    rms_eps: float
+    rope_theta: float
+
+    @property
+    def head_dim(self) -> int:
+        return self.embed_dim // self.heads
+
+
+PROGEN3_VOCAB = 134          # tokenizer.json's 34 entries plus the 100 <span_i> tokens added on top (ids 34..133)
+PROGEN3_MAX_PARAM_BYTES = 64e9  # fp32 weights the loader stages on one 80 GB device next to their packed copies
+
+
+def progen3_config(cfg: dict) -> Progen3Config:
+    """ProGen3Config (progen3/config.py:289-382) from a config.json dict, with its defaults for absent keys, refusing what the kernels do
+    not implement: an activation other than silu, clip_qkv, head_dim other than 64 / 128, heads not a multiple of kv_heads, and models
+    whose fp32 weights alone exceed PROGEN3_MAX_PARAM_BYTES (the 46B defaults: ~184 GB)."""
+    d = int(cfg.get("hidden_size", 4096))
+    gated = bool(cfg.get("gated_mlp", False))
+    f = cfg.get("intermediate_size", 16384)
+    f = int(f) if f is not None else (3 * d if gated else 4 * d)
+    heads = int(cfg.get("num_attention_heads", 32))
+    kv = cfg.get("num_key_value_heads", 8)
+    kv = heads if kv is None else int(kv)
+    layers = int(cfg.get("num_hidden_layers", 40))
+    E = int(cfg.get("num_experts", 8))
+    k = min(int(cfg.get("num_experts_per_tok", 2)), E)
+    vocab = cfg.get("vocab_size")
+    vocab = PROGEN3_VOCAB if vocab is None else int(vocab)
+    if cfg.get("hidden_act", "silu") != "silu":
+        raise NotImplementedError(f"ProGen3: hidden_act {cfg.get('hidden_act')!r}: the expert kernels implement silu only")
+    if cfg.get("clip_qkv") is not None:
+        raise NotImplementedError(f"ProGen3: clip_qkv {cfg.get('clip_qkv')}: q/k/v clipping is not implemented")
+    if d % heads or d // heads not in (64, 128):
+        raise NotImplementedError(f"ProGen3: head_dim = hidden_size / num_attention_heads = {d} / {heads} must be 64 or 128")
+    if kv <= 0 or heads % kv:
+        raise ValueError(f"ProGen3: num_attention_heads {heads} is not a multiple of num_key_value_heads {kv}")
+    hd = d // heads
+    per_layer = d * (d + 2 * kv * hd) + d * d + (E * d if E > 1 else 0) + E * f * d * (3 if gated else 2) + 2 * d
+    params = layers * per_layer + 2 * vocab * d + int(cfg.get("max_num_sequences", 512)) * d + d
+    if 4 * params > PROGEN3_MAX_PARAM_BYTES:
+        raise NotImplementedError(f"ProGen3: {params / 1e9:.1f}B parameters = {4 * params / 1e9:.0f} GB in fp32: the parity modes stage fp32 "
+                                  f"weights on one device (limit {PROGEN3_MAX_PARAM_BYTES / 1e9:.0f} GB)")
+    return Progen3Config(layers=layers, embed_dim=d, heads=heads, kv_heads=kv, ffn_dim=f, vocab=vocab, n_experts=E, top_k=k,
+                         gated_mlp=gated, rms_eps=float(cfg.get("rms_norm_eps", 1e-5)), rope_theta=float(cfg.get("rope_theta", 100000.0)))
+
+
+def normalise_progen3_state(conf: Progen3Config, raw: dict) -> dict:
+    """A ProGen3ForCausalLM state dict in any of its layouts -> the canonical names of include/pgscore.h's PG_ARCH_PROGEN3 (fp32).
+
+    - eager: ``layers.{i}.self_attn.*``, ``input_layernorm`` / ``post_attention_layernorm``, ``block_sparse_moe.gate.weight`` and
+      ``block_sparse_moe.experts.{e}.w{1,2,3}.weight`` (nn.Linear weights);
+    - fused attention norm (``fused_attention_norm``): the same under ``layers.{i}.norm_attn_norm.``;
+    - megablocks (the released checkpoints, ``moe_implementation`` "megablocks"; an assumption about megablocks' dMoE layout, whose
+      source is not part of the reference): ``block_sparse_moe.router.layer.weight`` [E, d], ``block_sparse_moe.experts.mlp.w1`` [E*f, d]
+      applied as x w1^T, ``experts.mlp.v1`` [E*f, d] (gated, the up projection) and ``experts.mlp.w2`` [E*f, d] applied as h w2.
+    The ``model.`` prefix is dropped."""
+    st = {}
+    for k, v in raw.items():
+        k = k[len("model."):] if k.startswith("model.") else k
+        k = re.sub(r"^layers\.(\d+)\.norm_attn_norm\.", r"layers.\1.", k)
+        st[k] = v.float()
+    E, f, d = conf.n_experts, conf.ffn_dim, conf.embed_dim
+    out = {}
+    for k, v in st.items():
+        if ".block_sparse_moe." not in k:
+            out[k] = v
+    for i in range(conf.layers):
+        p = f"layers.{i}.block_sparse_moe."
+        if p + "experts.mlp.w1" in st:
+            if E > 1:
+                out[p + "gate.weight"] = st[p + "router.layer.weight"]
+            out[p + "w1"] = st[p + "experts.mlp.w1"].reshape(E * f, d)
+            if conf.gated_mlp:
+                out[p + "w3"] = st[p + "experts.mlp.v1"].reshape(E * f, d)
+            out[p + "w2"] = st[p + "experts.mlp.w2"].reshape(E, f, d).transpose(1, 2).reshape(E * d, f)
+        else:
+            if E > 1:
+                out[p + "gate.weight"] = st[p + "gate.weight"]
+            out[p + "w1"] = torch.cat([st[f"{p}experts.{e}.w1.weight"] for e in range(E)])
+            if conf.gated_mlp:
+                out[p + "w3"] = torch.cat([st[f"{p}experts.{e}.w3.weight"] for e in range(E)])
+            out[p + "w2"] = torch.cat([st[f"{p}experts.{e}.w2.weight"] for e in range(E)])
+    return {k: v.contiguous() for k, v in out.items()}
+
+
+def load_progen3_checkpoint(folder: str):
+    """ProGen3 model directory (config.json + *.safetensors or pytorch_model.bin) -> (Progen3Config, canonical state)."""
+    import json
+    conf = progen3_config(json.load(open(os.path.join(folder, "config.json"))))
+    return conf, normalise_progen3_state(conf, _read_hf_weights(folder))
+
+
+def progen3_rotary_tables(head_dim: int, theta: float, T: int):
+    """cos / sin [T, head_dim/2] fp32 as RotaryPositionalEmbedding builds them (progen3/model/attention.py:38-63): inv_freq =
+    theta^-(arange(0, hd, 2) / hd) in fp32, angles = outer(t, inv_freq) in fp32 (both halves of the reference's table are equal)."""
+    inv_freq = theta ** -(torch.arange(0, head_dim, 2, dtype=torch.float32) / head_dim)
+    ang = torch.outer(torch.arange(T, dtype=torch.float32), inv_freq)
+    return ang.cos().contiguous(), ang.sin().contiguous()

@@ -151,6 +151,11 @@ __global__ void scale_copy_kernel(const float* __restrict__ src, float* __restri
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = src[i] * scale;
 }
+// dst [V, d] = src [V, d] + row [d] (ProGen3: embed_tokens + embed_seq_id[0], the fp32 sum modeling.py:441 forms per token)
+__global__ void add_row_kernel(const float* __restrict__ src, const float* __restrict__ row, int V, int d, float* __restrict__ dst) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < V * d) dst[i] = src[i] + row[i % d];
+}
 
 struct Layer {
   __half *wqkv = nullptr, *wo = nullptr, *w1 = nullptr, *w2 = nullptr;
@@ -159,6 +164,7 @@ struct Layer {
   float *iqkv = nullptr, *io = nullptr, *i1 = nullptr, *i2 = nullptr;  // PG_PREC_F16F8: 1 / t_n per weight row
   float* conv_taps = nullptr;  // Tranception: [3][4][64][8]
   float *qlng = nullptr, *klng = nullptr;  // ESM C: q_ln / k_ln weights [d]
+  float* gate = nullptr;  // ProGen3: router [E, d] fp32 (null for one expert); w1 / w2 hold the stacked experts
 };
 
 // Power-of-two scales the producers of A operands apply to their e4m3 planes (PG_PREC_F16F8; gemm_tc.cu header). e4m3 keeps
@@ -183,6 +189,7 @@ struct OpFmt {
   int pseg = 1;  // nseg of the operands that are fp16 hi [| lo] in every mode (attention, the MSA tied GEMMs): 3 when np == 2
   int slot = 64;                               // head slot width S
   int dk = 0, da = 0;                          // plane widths of GEMM-input rows of width d, and of attention rows (see above)
+  int dkv = 0, nq = 0;                         // k / v widths (ProGen3's kv_heads slots; da elsewhere) and q/k/v row width da + 2 dkv
   int64_t ldd = 0, ldf = 0, ldat = 0, ldq = 0;  // pitches of dk-, ffn-, da- and 3da-wide rows
   int64_t lo_d = 0, lo_at = 0, lo_q = 0;        // offset of the planes after the hi plane in dk-, da- and 3da-wide rows (0: none)
 };
@@ -194,15 +201,17 @@ OpFmt op_fmt(const pg_model_desc& D) {
   o.qfmt = o.np - 1;
   o.pseg = o.np == 2 ? 3 : 1;
   o.dk = (D.embed_dim + 63) / 64 * 64;
-  o.slot = D.arch == PG_ARCH_PROGEN2 && D.embed_dim / D.heads > 64 ? 128 : 64;
+  o.slot = (D.arch == PG_ARCH_PROGEN2 || D.arch == PG_ARCH_PROGEN3) && D.embed_dim / D.heads > 64 ? 128 : 64;
   o.da = D.heads * o.slot;
+  o.dkv = D.arch == PG_ARCH_PROGEN3 ? D.kv_heads * o.slot : o.da;
+  o.nq = o.da + 2 * o.dkv;
   o.ldd = static_cast<int64_t>(o.dk) * o.np;
   o.ldf = static_cast<int64_t>(D.ffn_dim) * o.np;
   o.ldat = static_cast<int64_t>(o.da) * o.np;
-  o.ldq = 3 * o.ldat;
+  o.ldq = static_cast<int64_t>(o.nq) * o.np;
   o.lo_d = o.np == 2 ? o.dk : 0;
   o.lo_at = o.np == 2 ? o.da : 0;
-  o.lo_q = 3 * o.lo_at;
+  o.lo_q = o.np == 2 ? o.nq : 0;
   return o;
 }
 
@@ -316,13 +325,20 @@ struct pg_handle_s {
   size_t mem_bytes = 0;
   int mem_T = -1;  // rows of the current record; -1 = none, 0 = an empty context
   int32_t *ctx_pos = nullptr, *ctx_seg = nullptr;
+  // ProGen3 mixture of experts (moe.cu): per layer the routing of the last pass ([layers][max_rows][top_k] expert ids and weights), the
+  // dispatch scratch, the expert-grouped operand rows gA, hidden rows gH and fp32 outputs gY of moe_rows slots
+  int32_t* route_e = nullptr; float* route_w = nullptr;
+  int32_t *moe_rank = nullptr, *moe_hist = nullptr, *moe_seg = nullptr, *moe_tiles = nullptr, *moe_ntiles = nullptr, *moe_slot = nullptr;
+  __half *gA = nullptr, *gH = nullptr; float* gY = nullptr;
+  long long moe_rows = 0;
+  int route_rows = 0;  // token rows of the last pass (pg_progen3_routing)
 };
 
 namespace pg {
 namespace {
 
 bool is_ar(int arch) {
-  return arch == PG_ARCH_TRANCEPTION || arch == PG_ARCH_RITA || arch == PG_ARCH_PROGEN2 || arch == PG_ARCH_PROTGPT2;
+  return arch == PG_ARCH_TRANCEPTION || arch == PG_ARCH_RITA || arch == PG_ARCH_PROGEN2 || arch == PG_ARCH_PROTGPT2 || arch == PG_ARCH_PROGEN3;
 }
 
 // Why a handle cannot run pg_masked_marginals / pg_forward_logprobs, or null: only ESM-1b, ESM2 and ESM C handles hold the ESM stack's
@@ -387,7 +403,7 @@ GemmLaunch proj_gemm(pg_handle h, const Layer& L, Proj p, const __half* a, float
   const int d = h->desc.embed_dim, f = h->desc.ffn_dim, dk = h->op.dk, da = h->op.da;
   GemmLaunch g{};
   switch (p) {
-    case QKV: g.w = L.wqkv; g.w_inv = L.iqkv; g.bias = L.bqkv; g.N = 3 * da; g.K = dk; break;
+    case QKV: g.w = L.wqkv; g.w_inv = L.iqkv; g.bias = L.bqkv; g.N = h->op.nq; g.K = dk; break;
     case OUT: g.w = L.wo; g.w_inv = L.io; g.bias = L.bo; g.N = d; g.K = da; break;
     case FC1: g.w = L.w1; g.w_inv = L.i1; g.bias = L.b1; g.N = h->desc.arch == PG_ARCH_ESMC ? 2 * f : f; g.K = dk; break;  // ESM C: gate|up
     case FC2: g.w = L.w2; g.w_inv = L.i2; g.bias = L.b2; g.N = d; g.K = f; break;
@@ -412,7 +428,7 @@ int lin(pg_handle h, const Layer& L, Proj p, const __half* a, float a_scale, int
   if (epi == 3) {  // q and k slots; tables [T, S/2]
     const int hs = h->op.slot / 2;
     g.rot_cos = h->rot_cos + static_cast<int64_t>(rot_start) * hs; g.rot_sin = h->rot_sin + static_cast<int64_t>(rot_start) * hs;
-    g.rot_T = rot_T; g.rot_dim = h->op.da; g.rot_half = hs; g.rot_pos = rot_pos;
+    g.rot_T = rot_T; g.rot_dim = (h->op.da + h->op.dkv) / 2; g.rot_half = hs; g.rot_pos = rot_pos;  // q and k: [0, da + dkv)
   }
   ProfScope ps(p, s);
   return launch_gemm(g, s);
@@ -659,8 +675,80 @@ int forward_rows_delta(pg_handle h, const int32_t* tokens, int n_tokens, const i
 // mode 2: the B sequences are rows [start, start + T) of sequences whose first `start` rows (multiple of 128) equal the recorded
 // wild type's: the keys / values of the prefix (and Tranception's conv look-back) come from the caches, and the rotary or learned
 // positions are the absolute positions start + t.
+// Segment height of the expert-grouped rows: 128 (single-CTA GEMM tiles, the default) or 256 (two-CTA tiles sharing the W tile).
+static int g_moe_pad = 128;
+
+// ProGen3 (progen3/modeling.py:193-290, 369-495; model/attention.py; model/moe.py) over B right-padded sequences of T tokens:
+// x = embed_tokens + embed_seq_id[0] (folded at load); per layer x += o_proj(attn(RMSNorm(x))) with bias-free q/k/v (kv_heads key / value
+// heads), rotate-half rotary over the whole head at positions 0..T-1 (GEMM epilogue 3, head_dim^-1/2 folded into q) and causal
+// grouped-query attention; then x += moe(RMSNorm(x)): router + dispatch (moe.cu), the experts' w1 as one ragged grouped GEMM with SiLU
+// (epilogue 8) or SwiGLU (epilogue 5, w1 / w3 interleaved at load), w2 as one ragged grouped GEMM storing fp32 rows per slot (epilogue 9),
+// and the combine into x in expert order. Layer l's routing stays in route_e / route_w.
+int forward_progen3(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s) {
+  const pg_model_desc& D = h->desc;
+  const OpFmt& o = h->op;
+  const int d = D.embed_dim, f = D.ffn_dim, E = D.n_experts, K = D.top_k;
+  const long long rows = static_cast<long long>(B) * T;
+  const int pad = g_moe_pad;
+  const long long R = (rows * K + static_cast<long long>(E) * (pad - 1) + pad - 1) / pad * pad;  // slots this pass can fill
+  const Act act = D.gated_mlp ? Act{5, S_SWIGLU} : Act{8, S_GELU};
+  int rc;
+  { ProfScope ps(CAT_EMBED, s);
+    rc = launch_gather_embed(ids, h->embed, rows, d, D.vocab, h->x, s); }
+  if (rc) return rc;
+  auto rms = [&](const float* g, float* rt_w, int32_t* rt_e, const float* gate) {
+    MoeRouteLaunch r{};
+    r.x = h->x; r.d = d; r.rows = rows; r.gamma = g; r.eps = D.rms_eps;
+    r.out = h->abuf; r.ldo = o.ldd; r.lo_off = o.lo_d; r.fmt = o.afmt; r.scale = S_LN;
+    r.gate = gate; r.E = E; r.K = K; r.route_e = rt_e; r.route_w = rt_w;
+    ProfScope ps(rt_e ? CAT_OTHER : CAT_LN, s);
+    return launch_moe_route(r, s);
+  };
+  for (int l = 0; l < D.layers; ++l) {
+    const Layer& L = h->layers[l];
+    if ((rc = rms(L.ln1g, nullptr, nullptr, nullptr))) return rc;
+    if ((rc = lin(h, L, QKV, h->abuf, S_LN, static_cast<int>(rows), h->qkv, s, 3, 0.f, T))) return rc;
+    AttnLaunch a = attn_args(h, h->qkv, h->abuf, B, T);
+    a.causal = 1; a.kv_heads = D.kv_heads;
+    { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
+    if (rc) return rc;
+    if ((rc = lin_add(h, L, OUT, h->abuf, S_ATT, static_cast<int>(rows), h->x, s))) return rc;
+    int32_t* re = h->route_e + static_cast<long long>(l) * h->max_rows * K;
+    float* rw = h->route_w + static_cast<long long>(l) * h->max_rows * K;
+    if ((rc = rms(L.ln2g, rw, re, L.gate))) return rc;
+    MoeDispatchLaunch m{};
+    m.route_e = re; m.rows = rows; m.E = E; m.K = K; m.pad = pad;
+    m.src = h->abuf; m.dst = h->gA; m.pitch_bytes = o.ldd * 2; m.row_bytes = static_cast<int>(o.ldd * 2);
+    m.rank = h->moe_rank; m.hist = h->moe_hist; m.seg_start = h->moe_seg; m.tile_expert = h->moe_tiles; m.n_tiles = h->moe_ntiles;
+    m.slot_of = h->moe_slot;
+    { ProfScope ps(CAT_REGROUP, s, 3); rc = launch_moe_dispatch(m, s); }
+    if (rc) return rc;
+    GemmLaunch g{};
+    g.a = h->gA; g.lda = o.ldd; g.w = L.w1; g.w_inv = L.i1; g.M = static_cast<int>(R); g.K = o.dk; g.N = D.gated_mlp ? 2 * f : f;
+    g.ldw = static_cast<int64_t>(o.dk) * o.np; g.nseg = o.nseg; g.a_scale = S_LN; g.w_uniform = 1; g.epi = act.epi;
+    g.out = h->gH; g.ldo = o.ldf; g.out_fmt = o.afmt; g.out_lo_off = o.afmt ? f : 0; g.out_scale = act.scale;
+    g.rg_expert = h->moe_tiles; g.rg_tiles = h->moe_ntiles; g.rg_pad = pad; g.rg_experts = E; g.grp_rows_b = g.N;
+    { ProfScope ps(CAT_GEMM_FC1, s); rc = launch_gemm(g, s); }
+    if (rc) return rc;
+    GemmLaunch g2{};
+    g2.a = h->gH; g2.lda = o.ldf; g2.w = L.w2; g2.w_inv = L.i2; g2.M = static_cast<int>(R); g2.K = f; g2.N = d; g2.ldw = o.ldf;
+    g2.nseg = o.nseg; g2.a_scale = act.scale; g2.w_uniform = 1; g2.epi = 9; g2.resid = h->gY; g2.ldr = d;
+    g2.rg_expert = h->moe_tiles; g2.rg_tiles = h->moe_ntiles; g2.rg_pad = pad; g2.rg_experts = E; g2.grp_rows_b = d;
+    { ProfScope ps(CAT_GEMM_FC2, s); rc = launch_gemm(g2, s); }
+    if (rc) return rc;
+    { ProfScope ps(CAT_OTHER, s); rc = launch_moe_combine(h->gY, d, re, rw, h->moe_slot, rows, K, h->x, s); }
+    if (rc) return rc;
+  }
+  h->route_rows = static_cast<int>(rows);
+  return PG_OK;
+}
+
 int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, int mode = 0, int start = 0) {
   const pg_model_desc& D = h->desc;
+  if (D.arch == PG_ARCH_PROGEN3) {
+    if (mode != 0) return set_error(PG_ERR_UNSUPPORTED, "ProGen3: wild-type prefix reuse is not implemented");
+    return forward_progen3(h, ids, B, T, s);
+  }
   const bool progen2 = D.arch == PG_ARCH_PROGEN2;
   const bool tranception = D.arch == PG_ARCH_TRANCEPTION;  // conv'd q/k/v, grouped ALiBi, relu^2; the others: tanh-GELU, no attention bias
   const bool rotary = D.arch == PG_ARCH_RITA || progen2;
@@ -863,7 +951,8 @@ int ar_head(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, 
             cudaStream_t s) {
   if (h->desc.arch == PG_ARCH_PROTGPT2) return lm_head_fused(h, ids, lens, B, T, f, tok_logp, out_sum, s);
   return launch_ar_head(h->x, h->desc.embed_dim, B, T, h->head_vocab, ids, lens, h->lnag, h->lnab, h->outw ? h->outw : h->embed,
-                        h->desc.arch == PG_ARCH_PROGEN2 ? h->hbias : nullptr, h->label_off, f, tok_logp, out_sum, s);
+                        h->desc.arch == PG_ARCH_PROGEN2 ? h->hbias : nullptr, h->label_off, f, tok_logp, out_sum, s, -1,
+                        h->desc.arch == PG_ARCH_PROGEN3 ? h->desc.rms_eps : 0.f);
 }
 
 // The decoder passes over B sequences of T rows (forward_ar mode 0, or mode 2 after the recorded prefix at `start`), as many sequences
@@ -1010,6 +1099,19 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     if (D.heads % 8) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen2 needs heads % 8 == 0 (qkv_proj is 8 shards, modeling_progen.py:157-168)");
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
     if (D.vocab < 30) return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen2 scores vocabulary columns 5..29 (vocab >= 30)");
+  } else if (D.arch == PG_ARCH_PROGEN3) {
+    const int hd = D.embed_dim % D.heads ? 0 : D.embed_dim / D.heads;
+    if (hd != 64 && hd != 128)
+      return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen3 head_dim (hidden_size / num_attention_heads) must be 64 or 128, got " +
+                                               std::to_string(D.embed_dim) + " / " + std::to_string(D.heads));
+    if (D.kv_heads <= 0 || D.heads % D.kv_heads)
+      return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen3 num_attention_heads % num_key_value_heads must be 0");
+    if (D.n_experts < 1 || D.n_experts > 64 || D.top_k < 1 || D.top_k > 8 || D.top_k > D.n_experts)
+      return set_error(PG_ERR_UNSUPPORTED, "pg_create: ProGen3 needs 1 <= num_experts <= 64 and 1 <= num_experts_per_tok <= min(num_experts, 8)");
+    if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: hidden_size and intermediate_size must be multiples of 64");
+    if (!(D.rms_eps > 0.f)) return set_error(PG_ERR_ARG, "pg_create: ProGen3 needs rms_norm_eps > 0");
+    if (D.max_positions <= 0) return set_error(PG_ERR_ARG, "pg_create: ProGen3 needs max_positions = the rotary table rows");
+    if (D.precision == PG_PREC_F16D) return set_error(PG_ERR_UNSUPPORTED, "pg_create: PG_PREC_F16D is built for the ESM-1b masked marginals");
   } else if (D.arch == PG_ARCH_ESM2) {  // narrow heads in 64-wide slots, widths padded to 64 (OpFmt)
     if (D.embed_dim % D.heads || (D.embed_dim / D.heads) % 2 || D.embed_dim / D.heads > 64)
       return set_error(PG_ERR_UNSUPPORTED, "pg_create: ESM2 head_dim must be even and at most 64");
@@ -1025,7 +1127,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
   }
   if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC &&
-      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2 && D.arch != PG_ARCH_PROTGPT2 && D.arch != PG_ARCH_POET)
+      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2 && D.arch != PG_ARCH_PROTGPT2 && D.arch != PG_ARCH_POET && D.arch != PG_ARCH_PROGEN3)
     return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
   if (D.arch == PG_ARCH_POET && D.vocab != 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: PoET needs the 24-token Uniprot21 vocabulary");
   if (D.arch == PG_ARCH_POET && D.max_positions <= 0)
@@ -1074,6 +1176,16 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   A(&h->cabuf, static_cast<size_t>(h->head_cap) * dw * np);
   A(&h->cfbuf, static_cast<size_t>(h->head_cap) * f * np);
   if (h->delta) A(&h->cq, static_cast<size_t>(h->head_cap) * 3 * d * np);
+  if (D.arch == PG_ARCH_PROGEN3) {  // slots for every (token, k) plus each segment's padding to 256 rows (either segment height fits)
+    const long long ent = h->max_rows * D.top_k;
+    h->moe_rows = (ent + 255LL * D.n_experts + 255) / 256 * 256;
+    A(&h->route_e, static_cast<size_t>(D.layers) * ent); A(&h->route_w, static_cast<size_t>(D.layers) * ent);
+    A(&h->moe_rank, static_cast<size_t>(ent)); A(&h->moe_slot, static_cast<size_t>(ent));
+    A(&h->moe_hist, static_cast<size_t>(moe_ws_blocks(ent)) * D.n_experts);
+    A(&h->moe_seg, static_cast<size_t>(D.n_experts)); A(&h->moe_tiles, static_cast<size_t>(h->moe_rows / 128)); A(&h->moe_ntiles, 1);
+    A(&h->gA, static_cast<size_t>(h->moe_rows) * h->op.ldd); A(&h->gH, static_cast<size_t>(h->moe_rows) * h->op.ldf);
+    A(&h->gY, static_cast<size_t>(h->moe_rows) * d);
+  }
   if (rc) {
     std::string m = h->err;
     pg_destroy(h);
@@ -1107,10 +1219,10 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
   std::map<std::string, const pg_tensor*> by_name;
   for (int i = 0; i < n; ++i) by_name[tensors[i].name] = &tensors[i];
   std::string missing;
-  auto get = [&](const std::string& name, int64_t r, int64_t c) -> const float* {
+  auto get = [&](const std::string& name, int64_t r, int64_t c) -> const float* {  // r < 0: any number of rows (at least one)
     auto it = by_name.find(name);
     if (it == by_name.end()) { missing += name + " "; return nullptr; }
-    if (it->second->shape[0] != r || it->second->shape[1] != c) { missing += name + "(shape) "; return nullptr; }
+    if ((r >= 0 ? it->second->shape[0] != r : it->second->shape[0] < 1) || it->second->shape[1] != c) { missing += name + "(shape) "; return nullptr; }
     return static_cast<const float*>(it->second->data);
   };
   int rc = PG_OK;  // the first failed allocation of a handle buffer
@@ -1308,6 +1420,52 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
     vec(&h->outw, "linear.weight", V, d);
     vec(&h->hbias, "linear.bias", V);
     if (by_name.count("norm.weight")) norm(&h->lnag, &h->lnab, "norm.");
+    rotary(h->op.slot / 2, true);
+  } else if (D.arch == PG_ARCH_PROGEN3) {
+    // Canonical names (include/pgscore.h; checkpoint.load_progen3 maps the eager, fused-norm and megablocks layouts onto them). q, k
+    // and v are stacked into one [da + 2 dkv, d] operand with head_dim^-1/2 folded into the q rows (exact at 64, one rounding at 128);
+    // the experts' w1 (and w3, interleaved with w1 per expert for the SwiGLU epilogue) and w2 are one stacked operand each.
+    const int kvw = D.kv_heads * hd, E = D.n_experts;
+    const int n1 = D.gated_mlp ? 2 * f : f;
+    for (int l = 0; l < D.layers; ++l) {
+      Layer& L = h->layers[l];
+      const std::string p = "layers." + std::to_string(l) + ".";
+      const float* wq = get(p + "self_attn.q_proj.weight", d, d);
+      const float* wk = get(p + "self_attn.k_proj.weight", kvw, d);
+      const float* wv = get(p + "self_attn.v_proj.weight", kvw, d);
+      float* qkv = (wq && wk && wv) ? static_cast<float*>(tmp(static_cast<size_t>(d + 2 * kvw) * d * sizeof(float))) : nullptr;
+      if (qkv) {
+        copy(qkv, wq, static_cast<size_t>(d) * d, qscale);
+        copy(qkv + static_cast<size_t>(d) * d, wk, static_cast<size_t>(kvw) * d);
+        copy(qkv + static_cast<size_t>(d + kvw) * d, wv, static_cast<size_t>(kvw) * d);
+      }
+      pack(&L.wqkv, &L.iqkv, {qkv}, d + 2 * kvw, d);
+      pack(&L.wo, &L.io, {get(p + "self_attn.o_proj.weight", d, d)}, d, d);
+      vec(&L.ln1g, p + "input_layernorm.weight", d);
+      vec(&L.ln2g, p + "post_attention_layernorm.weight", d);
+      if (E > 1) vec(&L.gate, p + "block_sparse_moe.gate.weight", E, d);
+      const float* w1 = get(p + "block_sparse_moe.w1", static_cast<int64_t>(E) * f, d);
+      const float* w3 = D.gated_mlp ? get(p + "block_sparse_moe.w3", static_cast<int64_t>(E) * f, d) : nullptr;
+      const float* w1p = w1;
+      if (D.gated_mlp) {  // per expert [w1_e ; w3_e] -> rows interleaved in blocks of 8
+        float* pair = (w1 && w3) ? static_cast<float*>(tmp(static_cast<size_t>(2) * f * d * sizeof(float))) : nullptr;
+        float* st = pair ? static_cast<float*>(tmp(static_cast<size_t>(E) * n1 * d * sizeof(float))) : nullptr;
+        for (int e = 0; st && e < E; ++e) {
+          const size_t fd = static_cast<size_t>(f) * d;
+          copy(pair, w1 + e * fd, fd);
+          copy(pair + fd, w3 + e * fd, fd);
+          interleave_gate_up_kernel<<<static_cast<unsigned>((2LL * f * d + 255) / 256), 256>>>(pair, f, d, st + 2 * e * fd);
+        }
+        w1p = st;
+      }
+      pack(&L.w1, &L.i1, {w1p}, E * n1, d);
+      pack(&L.w2, &L.i2, {get(p + "block_sparse_moe.w2", static_cast<int64_t>(E) * d, f)}, E * d, f);
+    }
+    const float* et = get("embed_tokens.weight", V, d);
+    const float* es = get("embed_seq_id.weight", -1, d);
+    if (et && es && alloc(&h->embed, static_cast<size_t>(V) * d)) add_row_kernel<<<(V * d + 255) / 256, 256>>>(et, es, V, d, h->embed);
+    vec(&h->lnag, "norm.weight", d);
+    vec(&h->outw, "lm_head.weight", V, d);
     rotary(h->op.slot / 2, true);
   } else if (D.arch == PG_ARCH_PROGEN2) {
     // HF names without the "transformer." prefix (modeling_progen.py:84-95, 209-226, 389-401, 541-548). qkv_proj [3d, d] is placed
@@ -1545,6 +1703,19 @@ int pg_ar_loglik_prefix(pg_handle h, const int32_t* ids, const int32_t* lens, in
   return ar_passes(h, ids, lens, B, T, 2, start, base, out_sum_logp, static_cast<cudaStream_t>(stream));
 }
 
+int pg_progen3_routing(pg_handle h, int32_t layer, int32_t* out_expert, float* out_weight, int32_t* out_rows, pg_stream stream) {
+  if (!h) return set_error(PG_ERR_ARG, "pg_progen3_routing: null handle");
+  if (h->desc.arch != PG_ARCH_PROGEN3) return fail(h, PG_ERR_STATE, "pg_progen3_routing: handle is not a ProGen3 model");
+  if (layer < 0 || layer >= h->desc.layers || !out_expert || !out_weight || !out_rows) return fail(h, PG_ERR_ARG, "pg_progen3_routing: bad arguments");
+  const size_t n = static_cast<size_t>(h->route_rows) * h->desc.top_k, off = static_cast<size_t>(layer) * h->max_rows * h->desc.top_k;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  PG_CUDA_OK(cudaSetDevice(h->desc.device));
+  PG_CUDA_OK(cudaMemcpyAsync(out_expert, h->route_e + off, n * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_weight, h->route_w + off, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  *out_rows = h->route_rows;
+  return PG_OK;
+}
+
 int pg_ar_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, const float* log_prior,
                  const int32_t* prior_row, float alpha, float* out_sum_logp, pg_stream stream) {
   pg_ar_fusion f = {};
@@ -1639,6 +1810,11 @@ int pg_set_tuning(const char* key, int32_t value) {
   if (std::string(key) == "gemm_kchunk") { set_gemm_kchunk(value); return PG_OK; }
   if (std::string(key) == "gemm_prefetch") { set_gemm_prefetch(value); return PG_OK; }
   if (std::string(key) == "gemm_cta2") { set_gemm_cta2(value); return PG_OK; }
+  if (std::string(key) == "moe_pad") {
+    if (value != 128 && value != 256) return set_error(PG_ERR_ARG, "pg_set_tuning: moe_pad must be 128 or 256");
+    pg::g_moe_pad = value;
+    return PG_OK;
+  }
   return set_error(PG_ERR_ARG, std::string("pg_set_tuning: unknown key ") + key);
 }
 
@@ -1661,6 +1837,7 @@ int pg_gemm_form(const pg_gemm_args* a, const struct pg_gemm_form* f, pg_stream 
     g.kchunk = f->kchunk; g.w_uniform = f->w_uniform;
     g.lm_part = reinterpret_cast<float2*>(f->lm_part); g.lm_tgt = f->lm_tgt; g.lm_logits = f->lm_logits;
     g.lm_ids = f->lm_ids; g.lm_lens = f->lm_lens; g.lm_T = f->lm_T;
+    g.rg_expert = f->rg_expert; g.rg_tiles = f->rg_tiles; g.rg_pad = f->rg_pad; g.rg_experts = f->rg_experts;
   }
   ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream));
   return launch_gemm(g, static_cast<cudaStream_t>(stream));

@@ -36,6 +36,7 @@ struct AttnWParams {
   int B, T, heads, nqt, nkb;   // T = full sequence length (prefix + own rows); nqt = query tiles of the own rows; nkb = key blocks of T
   int Tq, s_blocks;            // own rows per sequence; shared-prefix length / 64 (0 = no prefix: Tq == T)
   int d;
+  int dkv, grp;                // k / v width (kv_heads slots) and query heads per key / value head (grouped-query attention)
   long long lo_off;
   __half* out; long long ldo; long long out_lo_off;
   int causal;
@@ -80,7 +81,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_wgmma_kernel(const __grid_co
   const int nb = p.B;
   const int h = p.head_major ? bh / nb : bh % p.heads, b = p.head_major ? bh % nb : bh / p.heads;
   const int row0 = b * p.Tq;
-  const int cq = h * HD, ck = p.d + h * HD, cv = 2 * p.d + h * HD;
+  const int hk = h / p.grp;
+  const int cq = h * HD, ck = p.d + hk * HD, cv = p.d + p.dkv + hk * HD;
   // segment-causal: the tile's first row has the smallest segment start; blocks before it hold no visible key
   const int j0 = p.seg_start ? __ldg(p.seg_start + qt_l * QT) / KT : 0;
   const int nkb = (p.causal ? min(qt + 1, p.nkb) : p.nkb) - j0;  // causal: query tile qt needs key blocks 0 .. qt
@@ -302,7 +304,11 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
   if (HDw == 128 && (a.base_o || a.mask_pos || a.perm_C))
     return set_error(PG_ERR_UNSUPPORTED, "attention_wgmma: the delta-operand and column-attention forms run on 64-wide heads only");
   AttnWParams p{};
+  const int kvh = a.kv_heads ? a.kv_heads : a.heads;
+  if (kvh <= 0 || a.heads % kvh || (kvh != a.heads && (a.prefix || a.perm_C || a.base_o || a.mask_pos || a.seg_start)))
+    return set_error(PG_ERR_ARG, "attention_wgmma: kv_heads must divide heads; grouped-query attention runs the plain and causal forms");
   p.B = a.B; p.heads = a.heads; p.d = a.heads * HDw;
+  p.dkv = kvh * HDw; p.grp = a.heads / kvh;
   p.Tq = a.T; p.s_blocks = a.prefix ? (a.prefix_len + KT - 1) / KT : 0;
   p.p_valid = a.prefix_mem ? a.prefix_len : p.s_blocks * KT;
   p.head_major = a.prefix_mem; p.seg_start = a.seg_start;
@@ -319,8 +325,9 @@ int launch_attention_wgmma(const AttnLaunch& a, cudaStream_t s) {
     return set_error(PG_ERR_ARG, "attention_wgmma: delta-operand mode needs plain sequences and, with mask_pos, a compact hi/lo output");
   if (a.perm_C < 0 || (a.perm_C > 0 && (a.prefix || a.B % a.perm_C))) return set_error(PG_ERR_ARG, "attention_wgmma: bad column-attention arguments");
   const int np = a.nseg == 3 ? 2 : 1;
-  const uint64_t width = static_cast<uint64_t>(3) * p.d * np;
-  if (np == 2 && a.lo_off != 3ll * p.d) return set_error(PG_ERR_ARG, "attention_wgmma: lo planes must follow the hi planes (lo_off == 3*d)");
+  const uint64_t width = static_cast<uint64_t>(p.d + 2 * p.dkv) * np;
+  if (np == 2 && a.lo_off != p.d + 2ll * p.dkv)
+    return set_error(PG_ERR_ARG, "attention_wgmma: lo planes must follow the hi planes (lo_off == q + k + v width)");
   CUtensorMap tmQ, tm, tmP;
   int rc = make_tmap_f16_2d(&tmQ, a.qkv, static_cast<uint64_t>(a.B) * a.T, width, a.ld, QT, 64);
   if (rc) return rc;

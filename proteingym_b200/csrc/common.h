@@ -80,6 +80,10 @@ struct GemmLaunch {
   // lm_ids[row + 1] to lm_tgt[row]; lm_logits (optional, [M, N] fp32) receives every logit of those rows.
   float2* lm_part = nullptr; float* lm_tgt = nullptr; float* lm_logits = nullptr;
   const int32_t* lm_ids = nullptr; const int32_t* lm_lens = nullptr; int lm_T = 0;
+  // Ragged grouped form (ProGen3's experts): the A rows are expert segments, each padded to rg_pad rows (128, or 256 for the
+  // two-CTA form); rg_tiles[0] (device) = the rg_pad-row tiles in use, rg_expert[m] (device) = the expert of tile m, whose W rows are
+  // [e * grp_rows_b, e * grp_rows_b + N) of a stacked [E * grp_rows_b, K] w. M = the rows the buffers hold; tiles past rg_tiles[0] exit.
+  const int32_t* rg_expert = nullptr; const int32_t* rg_tiles = nullptr; int rg_pad = 0; int rg_experts = 0;
 };
 int launch_gemm(const GemmLaunch& g, cudaStream_t s);
 constexpr int GEMM_BN = 128;  // N tile of launch_gemm (the granularity of the epi 7 partials)
@@ -124,6 +128,9 @@ struct AttnLaunch {
   // Segment-causal form (wgmma kernel, B == 1): seg_start[t] (device) = first row of row t's segment; row t sees keys seg_start[t] .. t.
   // Key blocks before the query tile's first segment start are skipped.
   const int32_t* seg_start = nullptr;
+  // Grouped-query attention (wgmma kernel): the q/k/v rows are [q (heads slots) | k (kv_heads slots) | v (kv_heads slots)] and query
+  // head h reads key / value head h / (heads / kv_heads). 0 = kv_heads == heads.
+  int kv_heads = 0;
 };
 int launch_attention(const AttnLaunch& a, cudaStream_t s);
 
@@ -196,9 +203,10 @@ struct ArFusion {
 // wte: the head [vocab, d]; bias: [vocab] or null; the label of token id v is head column v - label_off.
 // lnf_g null: no LayerNorm before the head (PoET's norm=False). ignore_id >= 0: a next token equal to it contributes 0 (cross entropy's
 // ignore_index).
+// rms_eps > 0: lnf is an RMSNorm (x * rsqrt(mean(x^2) + rms_eps) * lnf_g, lnf_b unused) instead of a LayerNorm.
 int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t* ids, const int32_t* lens, const float* lnf_g,
                    const float* lnf_b, const float* wte, const float* bias, int label_off, const ArFusion& fusion, float* tok_logp,
-                   float* out_sum, cudaStream_t s, int ignore_id = -1);
+                   float* out_sum, cudaStream_t s, int ignore_id = -1, float rms_eps = 0.f);
 // After a GEMM epi 7 pass over B sequences of T rows: tok_logp[r] = lm_tgt[r] - logsumexp of the row's `tiles` partials combined in
 // tile order (0 for t >= lens[b] - 1, NaN for a next token outside [0, vocab)); out_logprobs (optional, [B*T, vocab], holding the logits
 // epi 7 wrote) becomes the log-softmax rows in place; out_sum[b] = the sequence sums (seq_sum_kernel).
@@ -232,4 +240,28 @@ int launch_tied_scatter_out(const __half* ot, int64_t ldo_t, __half* out, int64_
 int launch_tied_col_attention(const __half* qkv, int64_t ldq, int64_t lo_off, const int32_t* sel, int B, int R, int C, int H, float scale,
                               float* S1, __half* out, int64_t ldo, int64_t out_lo_off, int out_fmt, float out_scale, cudaStream_t s);
 int launch_msa_gather_col(const float* x, const int32_t* sel, int B, int R, int C, int d, float* xr, cudaStream_t s);
+}  // namespace pg
+
+namespace pg {
+// ProGen3 mixture of experts (moe.cu). RMSNorm of `rows` fp32 rows x [rows, d] into operand rows `out` (fmt / scale as above, planes
+// d wide); with route_e: also the router (gate [E, d] fp32, null when E == 1) -> route_e / route_w [rows, K].
+struct MoeRouteLaunch {
+  const float* x; int d; long long rows; const float* gamma; float eps;
+  __half* out; int64_t ldo; int64_t lo_off; int fmt; float scale;
+  const float* gate = nullptr; int E = 1, K = 1;
+  int32_t* route_e = nullptr; float* route_w = nullptr;
+};
+int launch_moe_route(const MoeRouteLaunch& r, cudaStream_t s);
+// Expert-grouped operand rows from the routing of `rows` tokens: rank / hist are scratch ([rows*K], [moe_ws_blocks(rows*K) * E]);
+// seg_start [E], tile_expert [rows*K / pad + E], n_tiles [1] feed the ragged GEMM; slot_of [rows*K] the combine.
+struct MoeDispatchLaunch {
+  const int32_t* route_e; long long rows; int E, K, pad;
+  const void* src; void* dst; int64_t pitch_bytes; int row_bytes;  // token operand rows -> slot rows, same pitch
+  int32_t *rank, *hist, *seg_start, *tile_expert, *n_tiles, *slot_of;
+};
+int moe_ws_blocks(long long entries);
+int launch_moe_dispatch(const MoeDispatchLaunch& m, cudaStream_t s);
+// x[t] += sum over the token's experts in increasing index order of route_w * y[slot] (fp32 rows y [slots, d]).
+int launch_moe_combine(const float* y, int d, const int32_t* route_e, const float* route_w, const int32_t* slot_of, long long rows, int K,
+                       float* x, cudaStream_t s);
 }  // namespace pg

@@ -23,8 +23,9 @@
 //   warpgroup 0   TMA producer (one elected thread of warp 0): cp.async.bulk.tensor 2D tiles (128 rows x 128 B of A, 128 rows
 //                 x 128 B of W, 128B swizzle; a row of 128 B is 64 fp16 or 128 e4m3 along K) into a 6-stage ring; 40 registers
 //   warpgroups 1-2 consumers, rows [0, 64) and [64, 128) of the tile: wgmma m64n128 (K = 16 fp16 / 32 e4m3: 32 B of each row) x4
-//                 per stage, then bias / erf-GELU / relu^2 / rotary / SwiGLU / tanh-GELU and fp16 hi [+ fp16 lo | + e4m3 planes for the next GEMM]
-//                 stored straight from the accumulator fragments, or added into the fp32 residual stream (one owner per element), or
+//                 per stage, then bias / erf-GELU / relu^2 / rotary / SwiGLU / tanh-GELU / SiLU and fp16 hi [+ fp16 lo | + e4m3 planes for the next GEMM]
+//                 stored straight from the accumulator fragments, or added into the fp32 residual stream (one owner per element) or
+//                 stored as fp32 rows (epi 9), or
 //                 (epi 7, K16) reduced to per-tile log-softmax partials of an LM head without storing the logits
 // Roofline: tensor bound. Algorithmic FLOPs = 2*M*N*K; issued tensor-pipe work = x1 / x2 / x3 by mode.
 #include <cstdlib>
@@ -78,6 +79,8 @@ struct GemmKParams {
   int grp_rows_a, grp_rows_b;  // grouped (block-diagonal) mode: A rows [g*grp_rows_a, (g+1)*grp_rows_a) pair with W rows g*grp_rows_b + n
   // LM-head log-softmax partials (epi 7; common.h GemmLaunch)
   float2* lm_part; float* lm_tgt; float* lm_logits; const int32_t* lm_ids; const int32_t* lm_lens; int lm_T;
+  const int32_t* rg_expert; const int32_t* rg_tiles;  // ragged grouped form (common.h GemmLaunch), or null
+  int rg_pad;                                          // ragged: rows per table entry (a multiple of the CTA (pair)'s tile rows)
 };
 
 // Exact-erf GELU (esm/modules.py:17-24): 0.5*x*(1+erf(x/sqrt2)) = 0.5*x + 0.5*|x|*erf(|x|/sqrt2).
@@ -150,6 +153,9 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
       } else if (EPI == 6) {
         v0 = gelu_tanh(v0);
         v1 = gelu_tanh(v1);
+      } else if (EPI == 8) {  // SiLU (ProGen3's ungated experts, progen3/model/moe.py:33-43)
+        v0 = silu(v0);
+        v1 = silu(v1);
       }
     }
     if (EPI == 3 && p.rot_half == 64) {
@@ -234,15 +240,19 @@ __device__ __forceinline__ void epilogue(float (&acc)[64], const GemmKParams& p,
           if (col + 1 < p.N) lr[col + 1] = acc[4 * j + 2 * h + 1];
         }
       }
-    } else if (EPI == 2) {
+    } else if (EPI == 2 || EPI == 9) {
+      // EPI 9 stores the fp32 accumulator instead of adding it (the experts' outputs per slot)
       // the masked row of each copy is updated by the compact exact path instead (delta-operand mode)
-      if (p.mask_pos != nullptr && trow == __ldg(p.mask_pos + row / p.base_T)) continue;
+      if (EPI == 2 && p.mask_pos != nullptr && trow == __ldg(p.mask_pos + row / p.base_T)) continue;
       float* r = p.resid + row * p.ldr;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int col = col0 + 8 * j;
         if (col >= p.N) continue;
-        if (col + 1 < p.N && !(reinterpret_cast<uintptr_t>(r + col) & 7)) {
+        if (EPI == 9) {
+          r[col] = acc[4 * j + 2 * h];
+          if (col + 1 < p.N) r[col + 1] = acc[4 * j + 2 * h + 1];
+        } else if (col + 1 < p.N && !(reinterpret_cast<uintptr_t>(r + col) & 7)) {
           float2 x = *reinterpret_cast<float2*>(r + col);
           x.x += acc[4 * j + 2 * h];
           x.y += acc[4 * j + 2 * h + 1];
@@ -340,7 +350,8 @@ __device__ __forceinline__ void consume_seg(float (&cacc)[64], int nkb, uint32_t
   }
 }
 
-template <int EPI, int CTA2>
+// RG: the ragged grouped form (a separate instance, so that the plain instances keep their code)
+template <int EPI, int CTA2, int RG>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmA8, const __grid_constant__ CUtensorMap tmB8, const __grid_constant__ GemmKParams p) {
@@ -360,6 +371,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int tile0 = CTA2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
   const int tstep = CTA2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
   constexpr int ROWS = CTA2 ? 2 * BM : BM;                          // rows of the output tile per (pair of) CTA(s)
+  // ragged form: the output tiles the routing filled (a prefix of tiles_m; one table entry covers rg_pad / ROWS of them)
+  const int m_used = RG ? __ldg(p.rg_tiles) * (p.rg_pad / ROWS) : p.tiles_m;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -392,9 +405,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int i = 0; i < p.prefetch; ++i) pf_step();
       for (int tile = tile0; tile < ntiles; tile += tstep) {
         const int m_blk = tile / p.tiles_n, n_blk = tile % p.tiles_n;
+        if (RG && m_blk >= m_used) break;
         const int a_row = m_blk * ROWS + static_cast<int>(rank) * BM;
         int b_row = n_blk * BN + (CTA2 ? static_cast<int>(rank) * (BN / 2) : 0);  // pair: this CTA's half of the W tile
         if (p.grp_rows_a) b_row += (m_blk * ROWS / p.grp_rows_a) * p.grp_rows_b;  // grouped: this group's block of W rows
+        if (RG) b_row += __ldg(p.rg_expert + m_blk * ROWS / p.rg_pad) * p.grp_rows_b;  // ragged: this tile's expert
         for (int s = 0; s < p.nsegs; ++s) {
           const GemmSeg sg = p.seg[s];
           const CUtensorMap* ma = sg.kind ? &tmA8 : &tmA;
@@ -423,6 +438,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint32_t phase = 0;
     for (int tile = tile0; tile < ntiles; tile += tstep) {
       const int m_blk = tile / p.tiles_n, n_blk = tile % p.tiles_n;
+      if (RG && m_blk >= m_used) break;
       const long long row0 = static_cast<long long>(m_blk) * ROWS + rank * BM + cw * 64 + (warp & 3) * 16 + g;
       const int col0 = n_blk * BN + 2 * t;
       float acc[64], cacc[64];
@@ -578,56 +594,67 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return set_error(PG_ERR_ARG, "gemm: empty problem");
   if (g.K % BK) return set_error(PG_ERR_ARG, "gemm: K must be a multiple of 64");
   if (g.nseg < 1 || g.nseg > 3) return set_error(PG_ERR_ARG, "gemm: nseg must be 1, 2 (fp16 + e4m3 cross terms) or 3");
-  if (g.epi < 0 || g.epi > 7) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
+  if (g.epi < 0 || g.epi > 9) return set_error(PG_ERR_ARG, "gemm: bad epilogue");
+  const bool f32out = g.epi == 2 || g.epi == 9;  // fp32 rows `resid`: added into (2) or stored (9)
   if (g.epi == 7 && (!g.lm_part || !g.lm_tgt || !g.lm_ids || !g.lm_lens || g.lm_T <= 0 || g.M % g.lm_T || g.grp_rows_a || g.bias))
     return set_error(PG_ERR_ARG, "gemm: the LM-head epilogue needs partial, target, ids and lens buffers, rows a multiple of lm_T, no groups or bias");
   if (g.epi == 5 && (g.N % 16 || (g.out_fmt == 2 && (g.N / 2) % 64) || g.grp_rows_a || (g.out_fmt >= 1 && g.out_lo_off < g.N / 2)))
     return set_error(PG_ERR_ARG, "gemm: the SwiGLU epilogue needs N % 16 == 0 (N/2 % 64 == 0 for out_fmt 2), no groups, planes >= N/2 apart");
-  if (g.epi != 7 && (g.epi == 2 ? !g.resid : !g.out)) return set_error(PG_ERR_ARG, "gemm: missing output");
-  if (g.epi == 3 && (!g.rot_cos || !g.rot_sin || g.rot_T <= 0 || g.rot_dim % 64)) return set_error(PG_ERR_ARG, "gemm: bad rotary args");
-  if (g.epi == 3 && ((g.rot_half != 32 && g.rot_half != 64) || g.rot_dim % (2 * g.rot_half)))
-    return set_error(PG_ERR_ARG, "gemm: rotary slots must be 64 or 128 wide and divide rot_dim");
+  if (g.epi != 7 && (f32out ? !g.resid : !g.out)) return set_error(PG_ERR_ARG, "gemm: missing output");
+  if (g.epi == 3 && (!g.rot_cos || !g.rot_sin || g.rot_T <= 0)) return set_error(PG_ERR_ARG, "gemm: bad rotary args");
+  // columns [0, 2 rot_dim) are rotated, whole slots of 2 rot_half columns each
+  if (g.epi == 3 && ((g.rot_half != 32 && g.rot_half != 64) || g.rot_dim <= 0 || g.rot_dim % g.rot_half))
+    return set_error(PG_ERR_ARG, "gemm: rotary slots must be 64 or 128 wide and 2 rot_dim a whole number of slots");
   if (g.nseg == 2 && (!g.w_inv || !(g.a_scale > 0.f))) return set_error(PG_ERR_ARG, "gemm: nseg 2 needs w_inv[N] and a_scale > 0");
   if (g.out_fmt < 0 || g.out_fmt > 2) return set_error(PG_ERR_ARG, "gemm: bad out_fmt");
   if ((g.base_pre || g.base_post || g.mask_pos) && (!g.base_pre || g.base_T <= 0 || g.N % 64 || g.M % g.base_T || g.grp_rows_a ||
                                                        (g.mask_pos && g.epi != 2) || (g.base_post && g.epi == 2)))
     return set_error(PG_ERR_ARG, "gemm: delta-operand mode needs base_pre, base_T > 0 dividing M, N % 64 == 0, no groups; mask_pos only with the residual epilogue");
-  if (g.epi != 2 && g.out_fmt == 2 && (g.N % 64 || !(g.out_scale > 0.f)))
+  if (!f32out && g.out_fmt == 2 && (g.N % 64 || !(g.out_scale > 0.f)))
     return set_error(PG_ERR_ARG, "gemm: out_fmt 2 needs N % 64 == 0 and out_scale > 0");
-  if (g.epi != 2 && g.out_fmt >= 1 && g.out_lo_off <= 0) return set_error(PG_ERR_ARG, "gemm: out_fmt 1/2 need out_lo_off > 0");
+  if (!f32out && g.out_fmt >= 1 && g.out_lo_off <= 0) return set_error(PG_ERR_ARG, "gemm: out_fmt 1/2 need out_lo_off > 0");
   if ((g.base_pre || g.base_post || g.mask_pos) && g.epi > 2)
     return set_error(PG_ERR_UNSUPPORTED, "gemm: the delta-operand form runs with epilogues 0, 1, 2");
-  if (g.epi != 7 && (g.epi == 2 ? (g.ldr % 2 || (reinterpret_cast<uintptr_t>(g.resid) & 7)) : (g.ldo % 2 || (reinterpret_cast<uintptr_t>(g.out) & 3) || g.out_lo_off % 2)))
+  if (g.epi != 7 && (f32out ? (g.ldr % 2 || (reinterpret_cast<uintptr_t>(g.resid) & 7)) : (g.ldo % 2 || (reinterpret_cast<uintptr_t>(g.out) & 3) || g.out_lo_off % 2)))
     return set_error(PG_ERR_ARG, "gemm: output pitches must be even and the output 8-byte (fp32) / 4-byte (fp16) aligned");
   int dev = 0;
   PG_CUDA_OK(cudaGetDevice(&dev));
   static bool attr_set[64] = {};
   if (dev < 64 && !attr_set[dev]) {
-#define PG_SET_SMEM(E)                                                                                           \
-  PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM)); \
-  PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM))
-    PG_SET_SMEM(0); PG_SET_SMEM(1); PG_SET_SMEM(2); PG_SET_SMEM(3); PG_SET_SMEM(4); PG_SET_SMEM(5); PG_SET_SMEM(6); PG_SET_SMEM(7);
+#define PG_SET_SMEM(E, R)                                                                                           \
+  PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 0, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM)); \
+  PG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<E, 1, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM))
+    PG_SET_SMEM(0, 0); PG_SET_SMEM(1, 0); PG_SET_SMEM(2, 0); PG_SET_SMEM(3, 0); PG_SET_SMEM(4, 0); PG_SET_SMEM(5, 0); PG_SET_SMEM(6, 0);
+    PG_SET_SMEM(7, 0); PG_SET_SMEM(0, 1); PG_SET_SMEM(5, 1); PG_SET_SMEM(8, 1); PG_SET_SMEM(9, 1);
 #undef PG_SET_SMEM
     attr_set[dev] = true;
   }
   const uint64_t K = static_cast<uint64_t>(g.K);
   const uint64_t width = K * (g.nseg == 3 ? 2 : 1);
-  const bool grouped = g.grp_rows_a > 0;
-  // pairs work on 256-row tiles; a grouped problem whose groups are only a multiple of 128 rows runs the single-CTA form
-  const int cta2 = gemm_cta2() && !(grouped && g.grp_rows_a % (2 * BM));
+  const bool grouped = g.grp_rows_a > 0, ragged = g.rg_expert != nullptr;
+  if (!ragged && g.epi >= 8) return set_error(PG_ERR_ARG, "gemm: epilogues 8 and 9 run in the ragged form only");
+  if (ragged && ((g.epi != 0 && g.epi != 5 && g.epi != 8 && g.epi != 9) || grouped || !g.rg_tiles || (g.rg_pad != BM && g.rg_pad != 2 * BM) || g.M % g.rg_pad || g.rg_experts <= 0 ||
+                 g.grp_rows_b < g.N || g.bias || (g.nseg == 2 && !g.w_uniform) ||
+                 g.base_pre || g.base_post || g.mask_pos))
+    return set_error(PG_ERR_ARG, "gemm: the ragged form runs epilogues 0, 5, 8 and 9 and needs a tile table, segments padded to 128 or 256 rows "
+                                 "(M a multiple), W blocks of >= N rows, no bias or delta form, one e4m3 scale per matrix");
+  // pairs work on 256-row tiles; a grouped problem whose groups are only a multiple of 128 rows, or a ragged one padded to 128 rows,
+  // runs the single-CTA form
+  const int cta2 = gemm_cta2() && !(grouped && g.grp_rows_a % (2 * BM)) && !(ragged && g.rg_pad != 2 * BM);
   const uint32_t wbox = cta2 ? BN / 2 : BN;  // rows of W one CTA loads per k-block
   CUtensorMap tmA, tmB, tmA8{}, tmB8{};
   int rc = make_tmap_2d(&tmA, g.a, g.M, width, g.lda, BM, BK, 2, 128);
   if (rc) return rc;
   if (grouped && (g.nseg == 2 || g.grp_rows_a % BM || g.grp_rows_b < g.N || g.M % g.grp_rows_a || g.bias || g.epi == 3))
     return set_error(PG_ERR_ARG, "gemm: grouped mode needs fp16 operands, A groups of a multiple of 128 rows, W groups of >= N rows, no bias");
-  const uint64_t w_rows = grouped ? static_cast<uint64_t>(g.M / g.grp_rows_a) * g.grp_rows_b : static_cast<uint64_t>(g.N);
+  const uint64_t w_rows = grouped ? static_cast<uint64_t>(g.M / g.grp_rows_a) * g.grp_rows_b
+                         : ragged ? static_cast<uint64_t>(g.rg_experts) * g.grp_rows_b : static_cast<uint64_t>(g.N);
   rc = make_tmap_2d(&tmB, g.w, w_rows, width, g.ldw, wbox, BK, 2, 128);
   if (rc) return rc;
   if (g.nseg == 2) {  // e4m3 planes follow the fp16 hi plane of each row: bytes [2K, 4K) = K-concatenated [lo8 | hi8] / [hi8 | lo8]
     rc = make_tmap_2d(&tmA8, static_cast<const uint8_t*>(g.a) + 2 * K, g.M, 2 * K, static_cast<uint64_t>(g.lda) * 2, BM, 2 * BK, 1, 128);
     if (rc) return rc;
-    rc = make_tmap_2d(&tmB8, static_cast<const uint8_t*>(g.w) + 2 * K, g.N, 2 * K, static_cast<uint64_t>(g.ldw) * 2, wbox, 2 * BK, 1, 128);
+    rc = make_tmap_2d(&tmB8, static_cast<const uint8_t*>(g.w) + 2 * K, w_rows, 2 * K, static_cast<uint64_t>(g.ldw) * 2, wbox, 2 * BK, 1, 128);
     if (rc) return rc;
   }
   GemmKParams p{};
@@ -663,13 +690,14 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   p.bias = g.bias;
   p.out = g.out; p.ldo = g.ldo; p.out_lo_off = g.out_lo_off;
   p.resid = g.resid; p.ldr = g.ldr;
-  p.out_fmt = (g.epi == 2) ? 0 : g.out_fmt;
+  p.out_fmt = f32out ? 0 : g.out_fmt;
   p.out_scale = g.out_scale;
   p.rot_cos = g.rot_cos; p.rot_sin = g.rot_sin; p.rot_T = g.rot_T; p.rot_dim = g.rot_dim; p.rot_half = g.rot_half; p.rot_pos = g.rot_pos;
   p.tiles_m = cta2 ? (g.M + 2 * BM - 1) / (2 * BM) : (g.M + BM - 1) / BM;
   p.tiles_n = (g.N + BN - 1) / BN;
-  p.prefetch = grouped ? 0 : gemm_prefetch();
+  p.prefetch = grouped || ragged ? 0 : gemm_prefetch();
   p.grp_rows_a = g.grp_rows_a; p.grp_rows_b = g.grp_rows_b;
+  p.rg_expert = g.rg_expert; p.rg_tiles = g.rg_tiles; p.rg_pad = g.rg_pad;
   p.base_pre = g.base_pre; p.base_post = g.base_post; p.base_T = g.base_T; p.mask_pos = g.mask_pos;
   p.lm_part = g.lm_part; p.lm_tgt = g.lm_tgt; p.lm_logits = g.lm_logits; p.lm_ids = g.lm_ids; p.lm_lens = g.lm_lens; p.lm_T = g.lm_T;
   const int ntiles = p.tiles_m * p.tiles_n;
@@ -688,18 +716,26 @@ int launch_gemm(const GemmLaunch& g, cudaStream_t s) {
   cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = GEMM_SMEM;
   cfg.stream = s;
-#define PG_LAUNCH(E) (cta2 ? cudaLaunchKernelEx(&cfg, gemm_tc_kernel<E, 1>, tmA, tmB, tmA8, tmB8, p) \
-                           : cudaLaunchKernelEx(&cfg, gemm_tc_kernel<E, 0>, tmA, tmB, tmA8, tmB8, p))
+#define PG_LAUNCH(E, R) (cta2 ? cudaLaunchKernelEx(&cfg, gemm_tc_kernel<E, 1, R>, tmA, tmB, tmA8, tmB8, p) \
+                              : cudaLaunchKernelEx(&cfg, gemm_tc_kernel<E, 0, R>, tmA, tmB, tmA8, tmB8, p))
   cudaError_t e;
-  switch (g.epi) {
-    case 0: e = PG_LAUNCH(0); break;
-    case 1: e = PG_LAUNCH(1); break;
-    case 2: e = PG_LAUNCH(2); break;
-    case 3: e = PG_LAUNCH(3); break;
-    case 4: e = PG_LAUNCH(4); break;
-    case 5: e = PG_LAUNCH(5); break;
-    case 6: e = PG_LAUNCH(6); break;
-    default: e = PG_LAUNCH(7); break;
+  if (ragged) {
+    switch (g.epi) {
+      case 0: e = PG_LAUNCH(0, 1); break;
+      case 5: e = PG_LAUNCH(5, 1); break;
+      case 8: e = PG_LAUNCH(8, 1); break;
+      default: e = PG_LAUNCH(9, 1); break;
+    }
+  } else switch (g.epi) {
+    case 0: e = PG_LAUNCH(0, 0); break;
+    case 1: e = PG_LAUNCH(1, 0); break;
+    case 2: e = PG_LAUNCH(2, 0); break;
+    case 3: e = PG_LAUNCH(3, 0); break;
+    case 4: e = PG_LAUNCH(4, 0); break;
+    case 5: e = PG_LAUNCH(5, 0); break;
+    case 6: e = PG_LAUNCH(6, 0); break;
+    case 7: e = PG_LAUNCH(7, 0); break;
+    default: return set_error(PG_ERR_ARG, "gemm: epilogues 8 and 9 run in the ragged form only");
   }
 #undef PG_LAUNCH
   PG_CUDA_OK(e);

@@ -125,6 +125,7 @@ struct ArHeadParams {
   ArFusion f;
   float* tok_logp;  // [B*T]
   int ignore_id;    // >= 0: a next token equal to it scores 0
+  float rms_eps;    // > 0: lnf is an RMSNorm with this eps (ProGen3's norm), lnf_b unused
 };
 
 // Retrieval fusion of one log-probability (Tranception model_pytorch.py:806-830; TranceptEVE model_pytorch.py:1100-1116, and the
@@ -159,7 +160,12 @@ __global__ void ar_head_kernel(ArHeadParams p) {
     return;
   }
   const float* xr = p.x + r * p.d;
-  if (p.lnf_g) {
+  if (p.lnf_g && p.rms_eps > 0.f) {
+    float ss = 0.f;
+    for (int j = threadIdx.x; j < p.d; j += blockDim.x) ss += xr[j] * xr[j];
+    const float rstd = rsqrtf(block_sum(ss, sh) / p.d + p.rms_eps);
+    for (int j = threadIdx.x; j < p.d; j += blockDim.x) y[j] = __fmul_rn(__fmul_rn(xr[j], rstd), p.lnf_g[j]);
+  } else if (p.lnf_g) {
     float mean, rstd;
     block_ln_stats(xr, p.d, sh, mean, rstd);
     for (int j = threadIdx.x; j < p.d; j += blockDim.x) y[j] = (xr[j] - mean) * rstd * p.lnf_g[j] + p.lnf_b[j];
@@ -266,9 +272,9 @@ int launch_qkv_conv(const __half* in, __half* out, int64_t ld, int64_t lo_off, i
 
 int launch_ar_head(const float* x, int d, int B, int T, int vocab, const int32_t* ids, const int32_t* lens, const float* lnf_g,
                    const float* lnf_b, const float* wte, const float* bias, int label_off, const ArFusion& fusion, float* tok_logp,
-                   float* out_sum, cudaStream_t s, int ignore_id) {
+                   float* out_sum, cudaStream_t s, int ignore_id, float rms_eps) {
   if (B <= 0 || T <= 0) return PG_OK;
-  ArHeadParams p{x, d, T, vocab, ids, lens, lnf_g, lnf_b, wte, bias, label_off, fusion, tok_logp, ignore_id};
+  ArHeadParams p{x, d, T, vocab, ids, lens, lnf_g, lnf_b, wte, bias, label_off, fusion, tok_logp, ignore_id, rms_eps};
   ar_head_kernel<<<static_cast<unsigned>(static_cast<long long>(B) * T), 128, (d + vocab) * sizeof(float), s>>>(p);
   seq_sum_kernel<<<(B + 3) / 4, 128, 0, s>>>(tok_logp, lens, B, T, out_sum);
   PG_CUDA_OK(cudaGetLastError());

@@ -839,3 +839,86 @@ def poet_a3m(target_seq: str, n: int, seed: int, sub_rate=(0.05, 0.9), gap_rate=
                 out.append("".join(AA20[i] for i in rng.randint(0, 20, size=rng.randint(1, 4))).lower())
         rows.append("".join(out))
     return rows
+
+
+# ---- ProGen3 (proteingym/baselines/progen3/progen3/modeling.py, model/moe.py) ----------------------------------------------------------
+@dataclass(frozen=True)
+class Progen3Arch:
+    layers: int
+    embed_dim: int
+    heads: int
+    kv_heads: int
+    ffn_dim: int
+    n_experts: int = 8
+    top_k: int = 2
+    gated_mlp: bool = False
+    vocab: int = 134
+    gate_std: float = 1.0  # router logit spread: larger separates the top-k from the rest by more
+
+    def config(self) -> dict:
+        """config.json of this shape (ProGen3Config's keys), eager MoE."""
+        return dict(model_type="progen3", vocab_size=self.vocab, hidden_size=self.embed_dim, intermediate_size=self.ffn_dim,
+                    gated_mlp=self.gated_mlp, num_hidden_layers=self.layers, num_attention_heads=self.heads,
+                    num_key_value_heads=self.kv_heads, hidden_act="silu", rms_norm_eps=1e-5, max_num_sequences=4,
+                    max_position_embeddings=4096, rope_theta=100000.0, clip_qkv=None, moe_implementation="eager",
+                    num_experts=self.n_experts, num_experts_per_tok=self.top_k, torch_dtype="float32")
+
+
+def make_progen3_state(arch: Progen3Arch, seed: int = 0) -> dict:
+    """Seeded fp32 ProGen3ForCausalLM state in the eager layout (reference key names with the ``model.`` prefix)."""
+    g = torch.Generator().manual_seed(seed)
+    d, f, E, hd = arch.embed_dim, arch.ffn_dim, arch.n_experts, arch.embed_dim // arch.heads
+    lin = lambda n, k, s=1.0: (s / math.sqrt(k)) * torch.randn((n, k), generator=g)
+    nw = lambda: 1 + 0.1 * torch.randn(d, generator=g)
+    st = {"model.embed_tokens.weight": torch.randn((arch.vocab, d), generator=g),
+          "model.embed_seq_id.weight": 0.1 * torch.randn((4, d), generator=g)}
+    for i in range(arch.layers):
+        p = f"model.layers.{i}."
+        st[p + "input_layernorm.weight"] = nw()
+        st[p + "post_attention_layernorm.weight"] = nw()
+        st[p + "self_attn.q_proj.weight"] = lin(d, d)
+        st[p + "self_attn.k_proj.weight"] = lin(arch.kv_heads * hd, d)
+        st[p + "self_attn.v_proj.weight"] = lin(arch.kv_heads * hd, d)
+        st[p + "self_attn.o_proj.weight"] = lin(d, d, 0.5)
+        if E > 1:
+            st[p + "block_sparse_moe.gate.weight"] = lin(E, d, arch.gate_std)
+        for e in range(E):
+            q = f"{p}block_sparse_moe.experts.{e}."
+            st[q + "w1.weight"] = lin(f, d)
+            if arch.gated_mlp:
+                st[q + "w3.weight"] = lin(f, d)
+            st[q + "w2.weight"] = lin(d, f, 0.5)
+    st["model.norm.weight"] = nw()
+    st["lm_head.weight"] = (2 / math.sqrt(d)) * torch.randn((arch.vocab, d), generator=g)
+    return st
+
+
+def progen3_megablocks_state(arch: Progen3Arch, st: dict) -> dict:
+    """The same weights in the megablocks dMoE layout (router.layer.weight; experts.mlp.w1 / v1 [E*f, d]; experts.mlp.w2 [E*f, d] applied
+    as h w2, i.e. each expert's w2 Linear weight transposed)."""
+    out = {k: v for k, v in st.items() if ".block_sparse_moe." not in k}
+    E = arch.n_experts
+    for i in range(arch.layers):
+        p = f"model.layers.{i}.block_sparse_moe."
+        out[p + "router.layer.weight"] = st[p + "gate.weight"]
+        out[p + "experts.mlp.w1"] = torch.cat([st[f"{p}experts.{e}.w1.weight"] for e in range(E)])
+        if arch.gated_mlp:
+            out[p + "experts.mlp.v1"] = torch.cat([st[f"{p}experts.{e}.w3.weight"] for e in range(E)])
+        out[p + "experts.mlp.w2"] = torch.cat([st[f"{p}experts.{e}.w2.weight"].t() for e in range(E)]).contiguous()
+    return out
+
+
+def write_progen3_checkpoint(folder: str, arch: Progen3Arch, seed: int = 0, layout: str = "eager", state: dict | None = None) -> dict:
+    """A ProGen3 model directory: config.json and model.safetensors in the eager or the megablocks layout (returns the eager state)."""
+    os.makedirs(folder, exist_ok=True)
+    st = make_progen3_state(arch, seed) if state is None else state
+    cfg = arch.config()
+    out = st
+    if layout == "megablocks":
+        cfg["moe_implementation"] = "megablocks"
+        out = progen3_megablocks_state(arch, st)
+    with open(os.path.join(folder, "config.json"), "w") as fh:
+        json.dump(cfg, fh, indent=1)
+    from safetensors.torch import save_file
+    save_file({k: v.contiguous() for k, v in out.items()}, os.path.join(folder, "model.safetensors"))
+    return st

@@ -1,4 +1,5 @@
 // C-ABI of libpgscore.so (include/pgscore.h): model handle, weight repacking, and the batched masked-marginal forward.
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <map>
@@ -266,6 +267,26 @@ __global__ void interleave_gate_up_kernel(const float* __restrict__ src, int f, 
   dst[i] = src[static_cast<long long>(sr) * K + k];
 }
 
+// A device buffer regrown on demand (not in `allocs`): grow() keeps it when it holds `bytes`, else waits for the work queued on s, which
+// may still read it, and replaces it.
+template <typename T>
+struct DevBuf {
+  T* p = nullptr;
+  size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  ~DevBuf() { cudaFree(p); }
+  int grow(size_t need, cudaStream_t s) {
+    if (need <= bytes) return PG_OK;
+    PG_CUDA_OK(cudaStreamSynchronize(s));
+    cudaFree(p);
+    p = nullptr; bytes = 0;
+    PG_CUDA_OK(cudaMalloc(&p, need));
+    bytes = need;
+    return PG_OK;
+  }
+};
+
 }  // namespace
 }  // namespace pg
 
@@ -306,23 +327,20 @@ struct pg_handle_s {
   // MSA Transformer: column-attention blocks (ln1*, wqkv, wo of a Layer), row-position table, tied-attention workspace
   std::vector<pg::Layer> col_layers;
   float* row_pos = nullptr;         // [1024, d] or null
-  void* tied_ws = nullptr;          // one allocation, regrown on demand (not in `allocs`)
-  size_t tied_bytes = 0;
+  pg::DevBuf<uint8_t> tied_ws;
   // compact buffers for the pruned last layer (one row per sequence)
   float* xc = nullptr;
   __half *cabuf = nullptr, *cfbuf = nullptr;
-  // delta-operand mode (PG_PREC_F16D): per-layer base rows of the unmasked window (one allocation, regrown on demand, not in
-  // `allocs`) and the compact exact q/k/v rows of the masked positions
+  // delta-operand mode (PG_PREC_F16D): per-layer base rows of the unmasked window and the compact exact q/k/v rows of the masked
+  // positions
   bool delta = false;
-  float* base = nullptr;
-  size_t base_alloc_bytes = 0;  // allocated for `base`
+  pg::DevBuf<float> base;
   int base_T = 0;
   __half* cq = nullptr;
   // PoET (pg_poet_context / pg_poet_loglik): the context record, per layer the multi-sequence attention's q/k/v rows of the context
-  // ([layers][mem_T][3da*np] fp16; the rotated k and the v columns are read), regrown on demand (not in `allocs`); rotary positions and
-  // segment starts of the context rows [max_rows]
-  __half* mem = nullptr;
-  size_t mem_bytes = 0;
+  // ([layers][mem_T][3da*np] fp16; the rotated k and the v columns are read); rotary positions and segment starts of the context rows
+  // [max_rows]
+  pg::DevBuf<__half> mem;
   int mem_T = -1;  // rows of the current record; -1 = none, 0 = an empty context
   int32_t *ctx_pos = nullptr, *ctx_seg = nullptr;
   // ProGen3 mixture of experts (moe.cu): per layer the routing of the last pass ([layers][max_rows][top_k] expert ids and weights), the
@@ -337,22 +355,79 @@ struct pg_handle_s {
 namespace pg {
 namespace {
 
-bool is_ar(int arch) {
-  return arch == PG_ARCH_TRANCEPTION || arch == PG_ARCH_RITA || arch == PG_ARCH_PROGEN2 || arch == PG_ARCH_PROTGPT2 || arch == PG_ARCH_PROGEN3;
+// The scoring entry points an architecture runs: the ESM masked marginals (pg_masked_marginals, pg_forward_logprobs), the MSA
+// Transformer's, the decoders' (pg_ar_*) or PoET's (pg_poet_*). Of the decoders, only Tranception takes a retrieval prior, and every one
+// but ProGen3 takes wild-type prefix reuse.
+enum Family { FAM_ESM, FAM_MSA, FAM_DECODER, FAM_POET };
+struct ArchInfo {
+  int arch;
+  const char* name;
+  Family family;
+  bool fusion, prefix;
+};
+constexpr ArchInfo ARCHS[] = {
+    // arch                name               family       fusion prefix
+    {PG_ARCH_ESM1B,        "ESM-1b",          FAM_ESM,     false, false},
+    {PG_ARCH_ESM2,         "ESM2",            FAM_ESM,     false, false},
+    {PG_ARCH_ESMC,         "ESM C",           FAM_ESM,     false, false},
+    {PG_ARCH_MSA,          "MSA Transformer", FAM_MSA,     false, false},
+    {PG_ARCH_TRANCEPTION,  "Tranception",     FAM_DECODER, true,  true},
+    {PG_ARCH_RITA,         "RITA",            FAM_DECODER, false, true},
+    {PG_ARCH_PROGEN2,      "ProGen2",         FAM_DECODER, false, true},
+    {PG_ARCH_PROTGPT2,     "ProtGPT2",        FAM_DECODER, false, true},
+    {PG_ARCH_PROGEN3,      "ProGen3",         FAM_DECODER, false, false},
+    {PG_ARCH_POET,         "PoET",            FAM_POET,    false, false},
+};
+// null: not an architecture of this library
+const ArchInfo* arch_info(int arch) {
+  for (const ArchInfo& a : ARCHS)
+    if (a.arch == arch) return &a;
+  return nullptr;
 }
-
-// Why a handle cannot run pg_masked_marginals / pg_forward_logprobs, or null: only ESM-1b, ESM2 and ESM C handles hold the ESM stack's
-// weights and its MLM head.
-const char* not_esm(int arch) {
-  if (arch == PG_ARCH_ESM1B || arch == PG_ARCH_ESM2 || arch == PG_ARCH_ESMC) return nullptr;
-  if (is_ar(arch)) return "handle is an autoregressive model (use pg_ar_loglik)";
-  if (arch == PG_ARCH_MSA) return "handle is an MSA Transformer (use pg_msa_masked_marginals)";
-  return "handle is not an ESM-1b, ESM2 or ESM C model";
+// "ESM-1b, ESM2 or ESM C"
+std::string family_names(Family f) {
+  std::string s, last;
+  for (const ArchInfo& a : ARCHS) {
+    if (a.family != f) continue;
+    if (!last.empty()) s += (s.empty() ? "" : ", ") + last;
+    last = a.name;
+  }
+  return s.empty() ? last : s + " or " + last;
 }
 
 int fail(pg_handle h, int code, const std::string& msg) {
   if (h) h->err = msg;
   return set_error(code, msg);
+}
+
+// The first step of every scoring entry point `who`: h is a handle (PG_ERR_ARG) whose weights are loaded (PG_ERR_STATE; with
+// `loaded` false, not asked), of an architecture of family `fam` (PG_ERR_STATE) that, with `prefix`, takes wild-type prefix reuse
+// (PG_ERR_UNSUPPORTED). Then h's device is made current.
+int enter(pg_handle h, const char* who, Family fam, bool loaded = true, bool prefix = false) {
+  const std::string w = who;
+  if (!h) return set_error(PG_ERR_ARG, w + ": null handle");
+  if (loaded && !h->loaded) return fail(h, PG_ERR_STATE, w + ": weights not loaded");
+  const ArchInfo& a = *arch_info(h->desc.arch);  // pg_create admits no other
+  if (a.family != fam) return fail(h, PG_ERR_STATE, w + ": handle is " + a.name + ", not " + family_names(fam));
+  if (prefix && !a.prefix) return fail(h, PG_ERR_UNSUPPORTED, w + ": " + a.name + " has no wild-type prefix reuse");
+  PG_CUDA_OK(cudaSetDevice(h->desc.device));
+  return PG_OK;
+}
+
+// The retrieval fusion block f (null: none) of a call on a head of `vocab` columns into *out. `arch`: the handle's architecture, which
+// must take a prior when f holds one (null: any).
+int fusion_args(const pg_ar_fusion* f, int vocab, const ArchInfo* arch, const std::string& who, ArFusion* out) {
+  if (!f) return PG_OK;
+  if ((f->log_prior == nullptr) != (f->prior_row == nullptr)) return set_error(PG_ERR_ARG, who + ": log_prior and prior_row go together");
+  if ((f->log_prior2 == nullptr) != (f->prior_row2 == nullptr)) return set_error(PG_ERR_ARG, who + ": log_prior2 and prior_row2 go together");
+  if (f->log_prior2 && !f->log_prior) return set_error(PG_ERR_ARG, who + ": the second prior needs the first (it is fused inside the MSA overlap)");
+  if (f->first_col < 0 || f->first_col > vocab) return set_error(PG_ERR_ARG, who + ": first_col outside the vocabulary");
+  if (arch && !arch->fusion && f->log_prior)
+    return set_error(PG_ERR_ARG, who + ": " + arch->name + " has no retrieval fusion (pass no log_prior / log_prior2)");
+  out->log_prior = f->log_prior; out->prior_row = f->prior_row; out->alpha = f->alpha;
+  out->log_prior2 = f->log_prior2; out->prior_row2 = f->prior_row2; out->beta = f->beta;
+  out->first_col = f->first_col; out->out_logprobs = f->out_logprobs;
+  return PG_OK;
 }
 
 template <typename T>
@@ -529,8 +604,8 @@ size_t base_bytes(const pg_model_desc& D, int T) {
 }
 BaseRows base_rows(pg_handle h, int l) {
   const long long T = h->base_T, d = h->desc.embed_dim, f = h->desc.ffn_dim;
-  float* p = h->base + static_cast<long long>(l) * T * (5 * d + f);
-  __half* q = reinterpret_cast<__half*>(h->base + static_cast<long long>(h->desc.layers) * T * (5 * d + f)) +
+  float* p = h->base.p + static_cast<long long>(l) * T * (5 * d + f);
+  __half* q = reinterpret_cast<__half*>(h->base.p + static_cast<long long>(h->desc.layers) * T * (5 * d + f)) +
               static_cast<long long>(l) * T * (3 * d + f);
   BaseRows b;
   b.bqkv = p; b.bout = p + T * 3 * d; b.bfc1 = p + T * 4 * d; b.bfc2 = p + T * (4 * d + f);
@@ -545,16 +620,11 @@ int forward_base(pg_handle h, const int32_t* tokens, int n_tokens, int T, cudaSt
   const OpFmt& o = h->op;
   const int d = D.embed_dim, f = D.ffn_dim;
   const size_t need = base_bytes(D, T);
-  if (need > h->base_alloc_bytes) {
-    if (h->base) cudaFree(h->base);
-    h->base = nullptr; h->base_alloc_bytes = 0;
-    cudaError_t e = cudaMalloc(&h->base, need);
-    if (e != cudaSuccess) return set_error(PG_ERR_CUDA, std::string("forward_base: cudaMalloc: ") + cudaGetErrorString(e));
-    h->base_alloc_bytes = need;
-  }
+  int rc = h->base.grow(need, s);
+  if (rc) return rc;
   h->base_T = T;
-  PG_CUDA_OK(cudaMemsetAsync(h->base, 0, need, s));  // the tap GEMMs reduce-add into zero
-  int rc = embed(h, tokens, n_tokens, nullptr, nullptr, 0, 1, T, s, 1);
+  PG_CUDA_OK(cudaMemsetAsync(h->base.p, 0, need, s));  // the tap GEMMs reduce-add into zero
+  rc = embed(h, tokens, n_tokens, nullptr, nullptr, 0, 1, T, s, 1);
   if (rc) return rc;
   // The base row of a GEMM input is its fp16 hi plane: zero the lo plane of the T rows (the tap GEMM, lin_add into the base rows,
   // then multiplies exactly that plane by the full hi/lo weights) and keep a copy of the hi plane.
@@ -743,12 +813,12 @@ int forward_progen3(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t 
   return PG_OK;
 }
 
+int forward_poet_rows(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s);
+
 int forward_ar(pg_handle h, const int32_t* ids, int B, int T, cudaStream_t s, int mode = 0, int start = 0) {
   const pg_model_desc& D = h->desc;
-  if (D.arch == PG_ARCH_PROGEN3) {
-    if (mode != 0) return set_error(PG_ERR_UNSUPPORTED, "ProGen3: wild-type prefix reuse is not implemented");
-    return forward_progen3(h, ids, B, T, s);
-  }
+  if (D.arch == PG_ARCH_PROGEN3) return forward_progen3(h, ids, B, T, s);  // mode 0 only: enter() refuses ProGen3 prefix reuse
+  if (D.arch == PG_ARCH_POET) return forward_poet_rows(h, ids, B, T, s);
   const bool progen2 = D.arch == PG_ARCH_PROGEN2;
   const bool tranception = D.arch == PG_ARCH_TRANCEPTION;  // conv'd q/k/v, grouped ALiBi, relu^2; the others: tanh-GELU, no attention bias
   const bool rotary = D.arch == PG_ARCH_RITA || progen2;
@@ -810,14 +880,11 @@ int forward_msa(pg_handle h, const int32_t* tokens, int R, int Cfull, const int3
   const size_t b_q = al(static_cast<size_t>(G) * Cp * ldt * 2), b_v = al(static_cast<size_t>(G) * Nt * ldv * 2);
   const size_t b_s = al(static_cast<size_t>(G) * Cp * lds * 4), b_p = al(static_cast<size_t>(G) * Cp * ldp * 2);
   const size_t need = 2 * b_q + b_v + b_s + b_p;
-  if (need > h->tied_bytes) {
-    if (h->tied_ws) cudaFree(h->tied_ws);
-    h->tied_ws = nullptr; h->tied_bytes = 0;
-    PG_CUDA_OK(cudaMalloc(&h->tied_ws, need));
-    h->tied_bytes = need;
-    PG_CUDA_OK(cudaMemsetAsync(h->tied_ws, 0, need, s));
+  if (need > h->tied_ws.bytes) {
+    if (int rc = h->tied_ws.grow(need, s)) return rc;
+    PG_CUDA_OK(cudaMemsetAsync(h->tied_ws.p, 0, need, s));
   }
-  uint8_t* ws = static_cast<uint8_t*>(h->tied_ws);
+  uint8_t* ws = h->tied_ws.p;
   __half* tq = reinterpret_cast<__half*>(ws);
   __half* tk = reinterpret_cast<__half*>(ws + b_q);
   __half* tv = reinterpret_cast<__half*>(ws + 2 * b_q);
@@ -909,14 +976,18 @@ HeadLaunch head_args(pg_handle h, int T) {
   return hl;
 }
 
-// Sequences per pass: as many as the workspace holds, then evened out over the passes that needs — 512 copies of a 514-token window
-// against the default 131 072-row workspace are 171 + 171 + 170, not 255 + 255 + 2 (a 2-sequence pass pays all 33 layers' launch
-// latencies and partial waves for 0.4 % of the rows). Results do not depend on the split (rows are independent; tested).
-long long balanced_per(long long total, long long cap) {
+// fn(first, count) over the passes that split `total` sequences, stopping at the first error. Sequences per pass: as many as the workspace
+// holds (`cap`), then evened out over the passes that needs — 512 copies of a 514-token window against the default 131 072-row workspace
+// are 171 + 171 + 170, not 255 + 255 + 2 (a 2-sequence pass pays all 33 layers' launch latencies and partial waves for 0.4 % of the
+// rows). Results do not depend on the split (rows are independent; tested).
+template <typename F>
+int for_passes(int total, long long cap, F fn) {
   if (cap < 1) cap = 1;
-  if (total <= cap) return total > 0 ? total : 1;
   const long long passes = (total + cap - 1) / cap;
-  return (total + passes - 1) / passes;
+  const int per = passes > 1 ? static_cast<int>((total + passes - 1) / passes) : total;
+  for (int first = 0; first < total; first += per)
+    if (int rc = fn(first, total - first < per ? total - first : per)) return rc;
+  return PG_OK;
 }
 
 // LM head on the Bc rows a pruned last layer left compacted in h->xc -> out [Bc, vocab]. `launches`: the head's own and the pass's
@@ -946,34 +1017,33 @@ int lm_head_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int B, i
   return launch_lm_head_combine(h->lm_part, (V + GEMM_BN - 1) / GEMM_BN, h->lm_tgt, ids, lens, B, T, V, f.out_logprobs, tok_logp, out_sum, s);
 }
 
-// The autoregressive head (ln_f, the handle's head matrix and bias, log-softmax) on B sequences of T rows in h->x.
+// The autoregressive head (ln_f, the handle's head matrix and bias, log-softmax) on B sequences of T rows in h->x. Of the decoders, only
+// ProGen2 and PoET load a head bias; PoET's targets equal to its mask token (23, the padding) score 0.
 int ar_head(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, const ArFusion& f, float* tok_logp, float* out_sum,
             cudaStream_t s) {
-  if (h->desc.arch == PG_ARCH_PROTGPT2) return lm_head_fused(h, ids, lens, B, T, f, tok_logp, out_sum, s);
-  return launch_ar_head(h->x, h->desc.embed_dim, B, T, h->head_vocab, ids, lens, h->lnag, h->lnab, h->outw ? h->outw : h->embed,
-                        h->desc.arch == PG_ARCH_PROGEN2 ? h->hbias : nullptr, h->label_off, f, tok_logp, out_sum, s, -1,
-                        h->desc.arch == PG_ARCH_PROGEN3 ? h->desc.rms_eps : 0.f);
+  const int arch = h->desc.arch;
+  ProfScope ps(CAT_HEAD, s, arch == PG_ARCH_PROTGPT2 ? 4 : 2);
+  if (arch == PG_ARCH_PROTGPT2) return lm_head_fused(h, ids, lens, B, T, f, tok_logp, out_sum, s);
+  return launch_ar_head(h->x, h->desc.embed_dim, B, T, h->head_vocab, ids, lens, h->lnag, h->lnab, h->outw ? h->outw : h->embed, h->hbias,
+                        h->label_off, f, tok_logp, out_sum, s, arch == PG_ARCH_POET ? 23 : -1,
+                        arch == PG_ARCH_PROGEN3 ? h->desc.rms_eps : 0.f);
 }
 
 // The decoder passes over B sequences of T rows (forward_ar mode 0, or mode 2 after the recorded prefix at `start`), as many sequences
-// per pass as the workspace holds, each followed by the head on its rows (the tied embedding, or RITA's untied lm_head).
+// per pass as the workspace holds, each followed by the head on its rows. tok_logp: the per-token log p [B, T], or null (h->tok_logp).
 int ar_passes(pg_handle h, const int32_t* ids, const int32_t* lens, int B, int T, int mode, int start, const ArFusion& fusion,
-              float* out_sum_logp, cudaStream_t s) {
-  const long long per = balanced_per(B, h->max_rows / T);
-  for (int b0 = 0; b0 < B; b0 += static_cast<int>(per)) {
-    const int Bc = (B - b0) < per ? (B - b0) : static_cast<int>(per);
+              float* out_sum_logp, cudaStream_t s, float* tok_logp = nullptr) {
+  return for_passes(B, h->max_rows / T, [&](int b0, int Bc) {
     const long long off = static_cast<long long>(b0) * T;
     int rc = forward_ar(h, ids + off, Bc, T, s, mode, start);
     if (rc) return fail(h, rc, tls_error());
-    ProfScope ps(CAT_HEAD, s, h->desc.arch == PG_ARCH_PROTGPT2 ? 4 : 2);
     ArFusion fc = fusion;
     if (fc.prior_row) fc.prior_row += off;
     if (fc.prior_row2) fc.prior_row2 += off;
     if (fc.out_logprobs) fc.out_logprobs += off * h->head_vocab;
-    rc = ar_head(h, ids + off, lens + b0, Bc, T, fc, h->tok_logp, out_sum_logp + b0, s);
-    if (rc) return fail(h, rc, tls_error());
-  }
-  return PG_OK;
+    rc = ar_head(h, ids + off, lens + b0, Bc, T, fc, tok_logp ? tok_logp + off : h->tok_logp, out_sum_logp + b0, s);
+    return rc ? fail(h, rc, tls_error()) : PG_OK;
+  });
 }
 
 // PoET (poet/models/poet.py:687-730, modules/transformer.py TieredTransformerEncoderLayer): per layer x += out(self_attn(norm1 x)),
@@ -999,7 +1069,7 @@ int forward_poet_context(pg_handle h, const int32_t* ids, int Tm, cudaStream_t s
     a.causal = 1; a.seg_start = h->ctx_seg;
     { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
     if (rc || (rc = lin_add(h, L, OUT, h->abuf, S_ATT, Tm, h->x, s))) return rc;
-    __half* mem = h->mem + static_cast<size_t>(l) * Tm * ldq;
+    __half* mem = h->mem.p + static_cast<size_t>(l) * Tm * ldq;
     if ((rc = ln(h, h->x, C.ln1g, C.ln1b, Tm, h->abuf, s))) return rc;
     if ((rc = lin(h, C, QKV, h->abuf, S_LN, Tm, mem, s, 3, 0.f, 1, 0, h->ctx_pos))) return rc;
     if (l + 1 == D.layers) break;
@@ -1031,7 +1101,7 @@ int forward_poet_rows(pg_handle h, const int32_t* ids, int B, int T, cudaStream_
       if ((rc = lin(h, A, QKV, h->abuf, S_LN, rows, h->qkv, s, 3, 0.f, T, 0))) return rc;
       AttnLaunch a = attn_args(h, h->qkv, h->abuf, B, T);
       a.causal = 1;
-      if (k && h->mem_T > 0) { a.prefix = h->mem + static_cast<size_t>(l) * h->mem_T * ldq; a.prefix_len = h->mem_T; a.prefix_mem = 1; }
+      if (k && h->mem_T > 0) { a.prefix = h->mem.p + static_cast<size_t>(l) * h->mem_T * ldq; a.prefix_len = h->mem_T; a.prefix_mem = 1; }
       { ProfScope ps(CAT_ATTN, s); rc = launch_attention_wgmma(a, s); }
       if (rc || (rc = lin_add(h, A, OUT, h->abuf, S_ATT, rows, h->x, s))) return rc;
     }
@@ -1126,9 +1196,8 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
     if (D.embed_dim != D.heads * 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: head_dim must be 64");
     if (D.embed_dim % 64 || D.ffn_dim % 64) return set_error(PG_ERR_UNSUPPORTED, "pg_create: embed_dim and ffn_dim must be multiples of 64");
   }
-  if (D.arch != PG_ARCH_ESM1B && D.arch != PG_ARCH_ESM2 && D.arch != PG_ARCH_TRANCEPTION && D.arch != PG_ARCH_MSA && D.arch != PG_ARCH_ESMC &&
-      D.arch != PG_ARCH_RITA && D.arch != PG_ARCH_PROGEN2 && D.arch != PG_ARCH_PROTGPT2 && D.arch != PG_ARCH_POET && D.arch != PG_ARCH_PROGEN3)
-    return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
+  const ArchInfo* arch = arch_info(D.arch);
+  if (!arch) return set_error(PG_ERR_UNSUPPORTED, "pg_create: unknown arch");
   if (D.arch == PG_ARCH_POET && D.vocab != 24) return set_error(PG_ERR_UNSUPPORTED, "pg_create: PoET needs the 24-token Uniprot21 vocabulary");
   if (D.arch == PG_ARCH_POET && D.max_positions <= 0)
     return set_error(PG_ERR_ARG, "pg_create: PoET needs max_positions = the rotary table rows (the longest sequence of a context or variant)");
@@ -1160,7 +1229,7 @@ int pg_create(const pg_model_desc* desc, pg_handle* out) {
   auto A = [&](auto** p, size_t n) { if (!rc) rc = dev_alloc(h, p, n); };
   if (D.arch == PG_ARCH_POET) { A(&h->ctx_pos, static_cast<size_t>(h->max_rows)); A(&h->ctx_seg, static_cast<size_t>(h->max_rows)); }
   if (D.arch == PG_ARCH_TRANCEPTION) A(&h->qkv2, static_cast<size_t>(h->max_rows) * 3 * d * np);
-  if (is_ar(D.arch) || D.arch == PG_ARCH_POET) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
+  if (arch->family == FAM_DECODER || arch->family == FAM_POET) A(&h->tok_logp, static_cast<size_t>(h->max_rows));
   if (D.arch == PG_ARCH_PROTGPT2) {  // 8 B per row and N tile: 412 MB at the default 131 072 rows and 50 257 columns
     A(&h->lm_part, static_cast<size_t>(h->max_rows) * ((D.vocab + GEMM_BN - 1) / GEMM_BN));
     A(&h->lm_tgt, static_cast<size_t>(h->max_rows));
@@ -1200,10 +1269,7 @@ int pg_destroy(pg_handle h) {
   if (!h) return PG_OK;
   cudaSetDevice(h->desc.device);
   for (void* p : h->allocs) cudaFree(p);
-  if (h->tied_ws) cudaFree(h->tied_ws);
-  if (h->base) cudaFree(h->base);
-  if (h->mem) cudaFree(h->mem);
-  delete h;
+  delete h;  // and the regrown buffers
   return PG_OK;
 }
 
@@ -1527,9 +1593,7 @@ int pg_load_weights(pg_handle h, const pg_tensor* tensors, int32_t n) {
 
 int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, const int32_t* positions, const int32_t* win_start,
                         const int32_t* out_row, int32_t P, int32_t T, float* out_logprobs, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_masked_marginals: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_masked_marginals: weights not loaded");
-  if (const char* why = not_esm(h->desc.arch)) return fail(h, PG_ERR_STATE, std::string("pg_masked_marginals: ") + why);
+  if (int rc = enter(h, "pg_masked_marginals", FAM_ESM)) return rc;
   if (!tokens || !positions || !out_logprobs) return fail(h, PG_ERR_ARG, "pg_masked_marginals: null buffer");
   if (P < 0 || T <= 0 || T > n_tokens) return fail(h, PG_ERR_ARG, "pg_masked_marginals: bad P/T");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions)
@@ -1537,34 +1601,25 @@ int pg_masked_marginals(pg_handle h, const int32_t* tokens, int32_t n_tokens, co
   if ((h->desc.arch == PG_ARCH_ESM2 || h->desc.arch == PG_ARCH_ESMC) && T > h->rot_rows)
     return fail(h, PG_ERR_ARG, "pg_masked_marginals: window longer than rotary tables");
   if (T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_masked_marginals: window longer than workspace (raise max_rows)");
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  long long per = h->max_rows / T;
-  if (per > h->head_cap) per = h->head_cap;
-  per = balanced_per(P, per);
   // delta-operand mode needs one shared window (every copy sees all n_tokens tokens) and the masked row as the emitted row
   const bool delta = h->delta && T == n_tokens && out_row == nullptr && P > 0;
   if (delta) {
     int rc = forward_base(h, tokens, n_tokens, T, s);
     if (rc) return fail(h, rc, tls_error());
   }
-  for (int p0 = 0; p0 < P; p0 += static_cast<int>(per)) {
-    const int Bc = (P - p0) < per ? (P - p0) : static_cast<int>(per);
+  return for_passes(P, std::min<long long>(h->max_rows / T, h->head_cap), [&](int p0, int Bc) {
     row_select_kernel<<<(Bc + 255) / 256, 256, 0, s>>>(positions, win_start, out_row, p0, Bc, h->row_sel);
     int rc = delta ? forward_rows_delta(h, tokens, n_tokens, positions, win_start, p0, Bc, T, s, h->row_sel)
                    : forward_rows(h, tokens, n_tokens, positions, win_start, p0, Bc, T, s, h->row_sel);
-    if (rc) return fail(h, rc, tls_error());
-    rc = compact_head(h, T, Bc, out_logprobs + static_cast<long long>(p0) * h->desc.vocab, 4, s);  // + row_select_kernel
-    if (rc) return fail(h, rc, tls_error());
-  }
-  return PG_OK;
+    if (!rc) rc = compact_head(h, T, Bc, out_logprobs + static_cast<long long>(p0) * h->desc.vocab, 4, s);  // + row_select_kernel
+    return rc ? fail(h, rc, tls_error()) : PG_OK;
+  });
 }
 
 int pg_msa_masked_marginals(pg_handle h, const int32_t* tokens, int32_t R, int32_t C_full, const int32_t* positions,
                             const int32_t* win_start, int32_t P, int32_t Cw, float* out_logprobs, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_msa_masked_marginals: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_msa_masked_marginals: weights not loaded");
-  if (h->desc.arch != PG_ARCH_MSA) return fail(h, PG_ERR_STATE, "pg_msa_masked_marginals: handle is not an MSA Transformer");
+  if (int rc = enter(h, "pg_msa_masked_marginals", FAM_MSA)) return rc;
   if (!tokens || !positions || !out_logprobs) return fail(h, PG_ERR_ARG, "pg_msa_masked_marginals: null buffer");
   if (P < 0 || R <= 0 || Cw <= 0 || Cw > C_full) return fail(h, PG_ERR_ARG, "pg_msa_masked_marginals: bad P/R/Cw");
   if (Cw > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_msa_masked_marginals: window longer than the learned position table");
@@ -1572,33 +1627,23 @@ int pg_msa_masked_marginals(pg_handle h, const int32_t* tokens, int32_t R, int32
   if (Cw < C_full && !win_start) return fail(h, PG_ERR_ARG, "pg_msa_masked_marginals: windows need win_start");
   const long long per_msa = static_cast<long long>(R) * Cw;
   if (per_msa > h->max_rows) return fail(h, PG_ERR_ARG, "pg_msa_masked_marginals: one alignment exceeds the workspace (raise max_rows)");
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  long long per = h->max_rows / per_msa;
-  if (per > h->head_cap) per = h->head_cap;
-  per = balanced_per(P, per);
-  for (int p0 = 0; p0 < P; p0 += static_cast<int>(per)) {
-    const int Bc = (P - p0) < per ? (P - p0) : static_cast<int>(per);
+  return for_passes(P, std::min<long long>(h->max_rows / per_msa, h->head_cap), [&](int p0, int Bc) {
     row_select_kernel<<<(Bc + 255) / 256, 256, 0, s>>>(positions, win_start, nullptr, p0, Bc, h->row_sel);
     int rc = forward_msa(h, tokens, R, C_full, positions, win_start, p0, Bc, Cw, s, h->row_sel);
-    if (rc) return fail(h, rc, tls_error());
-    rc = compact_head(h, 1, Bc, out_logprobs + static_cast<long long>(p0) * h->desc.vocab, 5, s);  // + row_select_kernel, row-0 gather
-    if (rc) return fail(h, rc, tls_error());
-  }
-  return PG_OK;
+    if (!rc) rc = compact_head(h, 1, Bc, out_logprobs + static_cast<long long>(p0) * h->desc.vocab, 5, s);  // + row_select_kernel, row-0 gather
+    return rc ? fail(h, rc, tls_error()) : PG_OK;
+  });
 }
 
 int pg_forward_logprobs(pg_handle h, const int32_t* tokens, int32_t n_tokens, int32_t win_start, int32_t T, int32_t mask_pos,
                         float* out_logprobs, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_forward_logprobs: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_forward_logprobs: weights not loaded");
-  if (const char* why = not_esm(h->desc.arch)) return fail(h, PG_ERR_STATE, std::string("pg_forward_logprobs: ") + why);
+  if (int rc = enter(h, "pg_forward_logprobs", FAM_ESM)) return rc;
   if (!tokens || !out_logprobs || T <= 0 || win_start < 0 || win_start + T > n_tokens) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: bad arguments");
   if (h->desc.arch == PG_ARCH_ESM1B && T > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than the learned position table");
   if ((h->desc.arch == PG_ARCH_ESM2 || h->desc.arch == PG_ARCH_ESMC) && T > h->rot_rows)
     return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than rotary tables");
   if (T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_forward_logprobs: sequence longer than workspace");
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // one row: positions / win_start as 1-element device arrays kept in row_sel scratch
   int32_t hostv[2] = {mask_pos, win_start};
@@ -1617,28 +1662,13 @@ int pg_forward_logprobs(pg_handle h, const int32_t* tokens, int32_t n_tokens, in
 }
 
 static int ar_fusion_args(pg_handle h, const pg_ar_fusion* f, ArFusion* base) {
-  if (!f) return PG_OK;
-  if ((f->log_prior == nullptr) != (f->prior_row == nullptr)) return fail(h, PG_ERR_ARG, "pg_ar_loglik: log_prior and prior_row go together");
-  if ((f->log_prior2 == nullptr) != (f->prior_row2 == nullptr)) return fail(h, PG_ERR_ARG, "pg_ar_loglik: log_prior2 and prior_row2 go together");
-  if (f->log_prior2 && !f->log_prior) return fail(h, PG_ERR_ARG, "pg_ar_loglik: the second prior needs the first (it is fused inside the MSA overlap)");
-  if (f->first_col < 0 || f->first_col > h->desc.vocab) return fail(h, PG_ERR_ARG, "pg_ar_loglik: first_col outside the vocabulary");
-  if (h->desc.arch == PG_ARCH_RITA && (f->log_prior || f->log_prior2))
-    return fail(h, PG_ERR_ARG, "pg_ar_loglik: RITA has no retrieval fusion (pass no log_prior / log_prior2)");
-  if (h->desc.arch == PG_ARCH_PROGEN2 && (f->log_prior || f->log_prior2))
-    return fail(h, PG_ERR_ARG, "pg_ar_loglik: ProGen2 has no retrieval fusion (pass no log_prior / log_prior2)");
-  if (h->desc.arch == PG_ARCH_PROTGPT2 && (f->log_prior || f->log_prior2))
-    return fail(h, PG_ERR_ARG, "pg_ar_loglik: ProtGPT2 has no retrieval fusion (pass no log_prior / log_prior2)");
-  base->log_prior = f->log_prior; base->prior_row = f->prior_row; base->alpha = f->alpha;
-  base->log_prior2 = f->log_prior2; base->prior_row2 = f->prior_row2; base->beta = f->beta;
-  base->first_col = f->first_col; base->out_logprobs = f->out_logprobs;
-  return PG_OK;
+  const int rc = fusion_args(f, h->desc.vocab, arch_info(h->desc.arch), "pg_ar_loglik", base);
+  return rc ? fail(h, rc, tls_error()) : PG_OK;
 }
 
 int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, const pg_ar_fusion* f,
                        float* out_sum_logp, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_ar_loglik: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_loglik: weights not loaded");
-  if (!is_ar(h->desc.arch)) return fail(h, PG_ERR_STATE, "pg_ar_loglik: handle is not an autoregressive model (Tranception, RITA, ProGen2)");
+  if (int rc = enter(h, "pg_ar_loglik", FAM_DECODER)) return rc;
   if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_ar_loglik: bad B/T");
   if (B == 0) return PG_OK;
   if (!ids || !lens || !out_sum_logp) return fail(h, PG_ERR_ARG, "pg_ar_loglik: null buffer");
@@ -1646,21 +1676,16 @@ int pg_ar_loglik_fused(pg_handle h, const int32_t* ids, const int32_t* lens, int
   { int frc = ar_fusion_args(h, f, &base); if (frc) return frc; }
   if (T > h->desc.max_positions) return fail(h, PG_ERR_ARG, "pg_ar_loglik: sequence longer than n_ctx");
   if (T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_ar_loglik: sequence longer than workspace");
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   return ar_passes(h, ids, lens, B, T, 0, 0, base, out_sum_logp, static_cast<cudaStream_t>(stream));
 }
 
 int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_fusion* f, float* out_tok_logp, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_ar_prefix_begin: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: weights not loaded");
-  if (!is_ar(h->desc.arch))
-    return fail(h, PG_ERR_STATE, "pg_ar_prefix_begin: handle is not an autoregressive model (Tranception, RITA, ProGen2)");
+  if (int rc = enter(h, "pg_ar_prefix_begin", FAM_DECODER, true, true)) return rc;
   if (!ids || !out_tok_logp || T < 2) return fail(h, PG_ERR_ARG, "pg_ar_prefix_begin: bad arguments");
   if (T > h->desc.max_positions || T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_ar_prefix_begin: sequence longer than n_ctx / workspace");
   ArFusion fu;
   int rc = ar_fusion_args(h, f, &fu);
   if (rc) return rc;
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t ldq = static_cast<size_t>(h->op.ldq);
   if (h->prefix_cap < h->desc.max_positions) {  // first use: [layers][n_ctx][3da*np] fp16, twice (RITA, ProGen2: once, no conv look-back)
@@ -1676,8 +1701,7 @@ int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_f
   // per-token log p(ids[t+1] | ids[<=t]) of the wild type, t = 0 .. T-2 (and the fused rows in f->out_logprobs when asked for)
   int32_t* len_dev = h->row_sel;
   PG_CUDA_OK(cudaMemcpyAsync(len_dev, &T, sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  { ProfScope ps(CAT_HEAD, s, h->desc.arch == PG_ARCH_PROTGPT2 ? 4 : 2);
-    rc = ar_head(h, ids, len_dev, 1, T, fu, out_tok_logp, h->tok_logp, s); }
+  rc = ar_head(h, ids, len_dev, 1, T, fu, out_tok_logp, h->tok_logp, s);
   if (rc) return fail(h, rc, tls_error());
   h->prefix_T = T;
   return PG_OK;
@@ -1685,10 +1709,7 @@ int pg_ar_prefix_begin(pg_handle h, const int32_t* ids, int32_t T, const pg_ar_f
 
 int pg_ar_loglik_prefix(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t start, const pg_ar_fusion* f,
                         float* out_sum_logp, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_ar_loglik_prefix: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: weights not loaded");
-  if (!is_ar(h->desc.arch))
-    return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: handle is not an autoregressive model (Tranception, RITA, ProGen2)");
+  if (int rc = enter(h, "pg_ar_loglik_prefix", FAM_DECODER)) return rc;
   if (h->prefix_T <= 0) return fail(h, PG_ERR_STATE, "pg_ar_loglik_prefix: no wild-type prefix recorded (call pg_ar_prefix_begin first)");
   if (start <= 0 || start % 128 || start >= h->prefix_T) return fail(h, PG_ERR_ARG, "pg_ar_loglik_prefix: start must be a positive multiple of 128 below the recorded length");
   if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_ar_loglik_prefix: bad B/T");
@@ -1699,17 +1720,15 @@ int pg_ar_loglik_prefix(pg_handle h, const int32_t* ids, const int32_t* lens, in
   ArFusion base;
   int rc = ar_fusion_args(h, f, &base);
   if (rc) return rc;
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   return ar_passes(h, ids, lens, B, T, 2, start, base, out_sum_logp, static_cast<cudaStream_t>(stream));
 }
 
 int pg_progen3_routing(pg_handle h, int32_t layer, int32_t* out_expert, float* out_weight, int32_t* out_rows, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_progen3_routing: null handle");
+  if (int rc = enter(h, "pg_progen3_routing", FAM_DECODER, false)) return rc;
   if (h->desc.arch != PG_ARCH_PROGEN3) return fail(h, PG_ERR_STATE, "pg_progen3_routing: handle is not a ProGen3 model");
   if (layer < 0 || layer >= h->desc.layers || !out_expert || !out_weight || !out_rows) return fail(h, PG_ERR_ARG, "pg_progen3_routing: bad arguments");
   const size_t n = static_cast<size_t>(h->route_rows) * h->desc.top_k, off = static_cast<size_t>(layer) * h->max_rows * h->desc.top_k;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   PG_CUDA_OK(cudaMemcpyAsync(out_expert, h->route_e + off, n * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
   PG_CUDA_OK(cudaMemcpyAsync(out_weight, h->route_w + off, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
   *out_rows = h->route_rows;
@@ -1724,9 +1743,7 @@ int pg_ar_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B
 }
 
 int pg_poet_context(pg_handle h, const int32_t* ids, const int32_t* seg_lens, int32_t n_seg, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_poet_context: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_poet_context: weights not loaded");
-  if (h->desc.arch != PG_ARCH_POET) return fail(h, PG_ERR_STATE, "pg_poet_context: handle is not a PoET model");
+  if (int rc = enter(h, "pg_poet_context", FAM_POET)) return rc;
   if (n_seg < 0 || (n_seg > 0 && (!ids || !seg_lens))) return fail(h, PG_ERR_ARG, "pg_poet_context: bad arguments");
   std::vector<int32_t> pos, seg;
   for (int i = 0; i < n_seg; ++i) {
@@ -1736,18 +1753,10 @@ int pg_poet_context(pg_handle h, const int32_t* ids, const int32_t* seg_lens, in
     if (static_cast<long long>(pos.size()) > h->max_rows) return fail(h, PG_ERR_ARG, "pg_poet_context: context longer than the workspace (max_rows)");
   }
   const int Tm = static_cast<int>(pos.size());
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   h->mem_T = -1;
   if (Tm == 0) { h->mem_T = 0; return PG_OK; }
-  const size_t need = static_cast<size_t>(h->desc.layers) * Tm * h->op.ldq * sizeof(__half);
-  if (need > h->mem_bytes) {
-    PG_CUDA_OK(cudaStreamSynchronize(s));  // the old record may still be read by work queued on s
-    if (h->mem) cudaFree(h->mem);
-    h->mem = nullptr; h->mem_bytes = 0;
-    PG_CUDA_OK(cudaMalloc(&h->mem, need));
-    h->mem_bytes = need;
-  }
+  if (int rc = h->mem.grow(static_cast<size_t>(h->desc.layers) * Tm * h->op.ldq * sizeof(__half), s)) return rc;
   PG_CUDA_OK(cudaMemcpyAsync(h->ctx_pos, pos.data(), Tm * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   PG_CUDA_OK(cudaMemcpyAsync(h->ctx_seg, seg.data(), Tm * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   PG_CUDA_OK(cudaStreamSynchronize(s));  // pos / seg are pageable host vectors
@@ -1758,42 +1767,26 @@ int pg_poet_context(pg_handle h, const int32_t* ids, const int32_t* seg_lens, in
 }
 
 int pg_poet_record(pg_handle h, int32_t layer, void* out, int64_t ld_bytes, pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_poet_record: null handle");
-  if (h->desc.arch != PG_ARCH_POET || h->mem_T < 0) return fail(h, PG_ERR_STATE, "pg_poet_record: no PoET context recorded");
+  if (int rc = enter(h, "pg_poet_record", FAM_POET, false)) return rc;
+  if (h->mem_T < 0) return fail(h, PG_ERR_STATE, "pg_poet_record: no PoET context recorded");
   if (layer < 0 || layer >= h->desc.layers || !out) return fail(h, PG_ERR_ARG, "pg_poet_record: bad layer or null buffer");
   const size_t row = static_cast<size_t>(h->op.ldq) * sizeof(__half);
   if (ld_bytes < static_cast<int64_t>(row)) return fail(h, PG_ERR_ARG, "pg_poet_record: pitch shorter than a record row");
   if (h->mem_T == 0) return PG_OK;
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
-  PG_CUDA_OK(cudaMemcpy2DAsync(out, ld_bytes, h->mem + static_cast<size_t>(layer) * h->mem_T * h->op.ldq, row, row, h->mem_T,
+  PG_CUDA_OK(cudaMemcpy2DAsync(out, ld_bytes, h->mem.p + static_cast<size_t>(layer) * h->mem_T * h->op.ldq, row, row, h->mem_T,
                                cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   return PG_OK;
 }
 
 int pg_poet_loglik(pg_handle h, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, float* out_sum_logp, float* out_tok_logp,
                    pg_stream stream) {
-  if (!h) return set_error(PG_ERR_ARG, "pg_poet_loglik: null handle");
-  if (!h->loaded) return fail(h, PG_ERR_STATE, "pg_poet_loglik: weights not loaded");
-  if (h->desc.arch != PG_ARCH_POET) return fail(h, PG_ERR_STATE, "pg_poet_loglik: handle is not a PoET model");
+  if (int rc = enter(h, "pg_poet_loglik", FAM_POET)) return rc;
   if (h->mem_T < 0) return fail(h, PG_ERR_STATE, "pg_poet_loglik: no context recorded (call pg_poet_context first)");
   if (B < 0 || T <= 0) return fail(h, PG_ERR_ARG, "pg_poet_loglik: bad B/T");
   if (B == 0) return PG_OK;
   if (!ids || !lens || !out_sum_logp) return fail(h, PG_ERR_ARG, "pg_poet_loglik: null buffer");
   if (T > h->rot_rows || T > h->max_rows) return fail(h, PG_ERR_ARG, "pg_poet_loglik: rows longer than max_positions / the workspace");
-  PG_CUDA_OK(cudaSetDevice(h->desc.device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const long long per = balanced_per(B, h->max_rows / T);
-  for (int b0 = 0; b0 < B; b0 += static_cast<int>(per)) {
-    const int Bc = (B - b0) < per ? (B - b0) : static_cast<int>(per);
-    const long long off = static_cast<long long>(b0) * T;
-    int rc = forward_poet_rows(h, ids + off, Bc, T, s);
-    if (rc) return fail(h, rc, tls_error());
-    ProfScope ps(CAT_HEAD, s, 2);
-    rc = launch_ar_head(h->x, h->desc.embed_dim, Bc, T, h->desc.vocab, ids + off, lens + b0, h->lnag, h->lnab,
-                        h->outw, h->hbias, 0, ArFusion{}, out_tok_logp ? out_tok_logp + off : h->tok_logp, out_sum_logp + b0, s, 23);
-    if (rc) return fail(h, rc, tls_error());
-  }
-  return PG_OK;
+  return ar_passes(h, ids, lens, B, T, 0, 0, ArFusion{}, out_sum_logp, static_cast<cudaStream_t>(stream), out_tok_logp);
 }
 
 int pg_score_mutants(const float* table, int32_t n_rows, int32_t vocab, const int32_t* site_row, const int32_t* site_wt,
@@ -1970,15 +1963,7 @@ int pg_ar_head(const pg_ar_head_args* a, const pg_ar_fusion* f, pg_stream stream
   if ((a->lnf_g == nullptr) != (a->lnf_b == nullptr)) return set_error(PG_ERR_ARG, "pg_ar_head: lnf_g and lnf_b go together");
   if (a->d + a->vocab > 12288) return set_error(PG_ERR_ARG, "pg_ar_head: d + vocab floats exceed 48 KB of shared memory");
   ArFusion fu;
-  if (f) {
-    if ((f->log_prior == nullptr) != (f->prior_row == nullptr)) return set_error(PG_ERR_ARG, "pg_ar_head: log_prior and prior_row go together");
-    if ((f->log_prior2 == nullptr) != (f->prior_row2 == nullptr)) return set_error(PG_ERR_ARG, "pg_ar_head: log_prior2 and prior_row2 go together");
-    if (f->log_prior2 && !f->log_prior) return set_error(PG_ERR_ARG, "pg_ar_head: the second prior needs the first");
-    if (f->first_col < 0 || f->first_col > a->vocab) return set_error(PG_ERR_ARG, "pg_ar_head: first_col outside the vocabulary");
-    fu.log_prior = f->log_prior; fu.prior_row = f->prior_row; fu.alpha = f->alpha;
-    fu.log_prior2 = f->log_prior2; fu.prior_row2 = f->prior_row2; fu.beta = f->beta;
-    fu.first_col = f->first_col; fu.out_logprobs = f->out_logprobs;
-  }
+  if (int rc = fusion_args(f, a->vocab, nullptr, "pg_ar_head", &fu)) return rc;
   ProfScope ps(CAT_OTHER, static_cast<cudaStream_t>(stream), 2);
   return launch_ar_head(a->x, a->d, a->B, a->T, a->vocab, a->ids, a->lens, a->lnf_g, a->lnf_b, a->wte, a->bias, a->label_off, fu,
                         a->tok_logp, a->out_sum, static_cast<cudaStream_t>(stream), a->ignore_id);

@@ -10,11 +10,30 @@ two-layer MSA Transformer table (a full and a pruned last layer) in f16x3 / f16f
 wild type's substitutions and indels with and without prefix reuse in f16f8. Every run with prefix reuse also records its token-row
 counts (reuse_rows). The load paths the runs above leave out have a run each (loads()): ESM C in f16f8 / f16x3, an ESM-1b with
 emb_layer_norm_before, an MSA Transformer without msa_position_embedding, ProGen2 with 80-wide heads (128-wide slots), RITA with an
-untied head, and PoET with and without its final norm in f16x3 / f16f8 (per-token log p and layer 0 of the context record)."""
+untied head, and PoET with and without its final norm in f16x3 / f16f8 (per-token log p and layer 0 of the context record). Runs split
+into several passes have a run each (passes()): ProGen3 in f16x3 / f16f8, PoET's per-sequence sums, and ESM-1v wt-marginals over
+overlapping 1024-token windows (pg_forward_logprobs). Every array <name> comes with <name>.launches: the library's launch count
+(pg_launch_count) over the work since the array stored before it."""
 import os
 import sys
 
 import numpy as np
+
+
+class Runs(dict):
+    """Arrays by name; storing <name> also stores <name>.launches, the launches counted since the previous store."""
+
+    def __init__(self):
+        super().__init__()
+        from proteingym_b200 import _lib
+        self.lib = _lib.load()
+        self.mark = self.lib.pg_launch_count()
+
+    def __setitem__(self, name, value):
+        n = self.lib.pg_launch_count()
+        super().__setitem__(name, value)
+        super().__setitem__(name + ".launches", np.array([n - self.mark], dtype=np.int64))
+        self.mark = n
 
 
 def collect():
@@ -22,7 +41,7 @@ def collect():
     from proteingym_b200 import checkpoint, msa_engine, synth
     from proteingym_b200.esm_engine import EsmScorer
     from proteingym_b200.tranception_engine import TranceptionScorer
-    out = {}
+    out = Runs()
     seq = synth.random_protein(200, 3)
     muts = synth.sample_mutants(seq, 400, 4, multi_frac=0.2)
     for name, arch, modes in (("esm1v", synth.EsmArch("esm1v", 3, 256, 4, 1024), ("f16x3", "f16f8", "f16d", "f16")),
@@ -69,6 +88,7 @@ def collect():
         sc.close()
     out.update(decoders())
     out.update(loads())
+    out.update(passes())
     return out
 
 
@@ -105,7 +125,7 @@ def decoders():
         ws = {k[len("transformer."):] if k.startswith("transformer.") else k: v for k, v in st.items() if k != "lm_head.weight"}
         return Protgpt2Scorer(checkpoint.Protgpt2Config(a.layers, a.embed_dim, a.heads, a.ffn_dim, a.vocab, a.n_positions), ws,
                               Protgpt2Tokenizer(os.path.join(golden, "protgpt2_tokenizer")), precision="f16f8")
-    out = {}
+    out = Runs()
     for name, make in (("rita", rita), ("progen2", progen2), ("protgpt2", protgpt2)):
         sc = make()
         for reuse in (True, False):
@@ -125,7 +145,7 @@ def loads():
     from proteingym_b200.progen2_engine import Progen2Scorer
     from proteingym_b200.rita_engine import RitaScorer, RitaTokenizer
     golden = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
-    out = {}
+    out = Runs()
     seq = synth.random_protein(150, 21)
     muts = synth.sample_mutants(seq, 200, 22, multi_frac=0.2)
     st = synth.make_esmc_state(synth.EsmcArch(2, 256, 512), seed=23)
@@ -180,6 +200,45 @@ def loads():
             out[f"poet.norm{int(norm)}.{mode}.tok"] = sc.loglik(variants, tok_logp=True)[1]
             out[f"poet.norm{int(norm)}.{mode}.record0"] = np.concatenate([k.cpu().numpy(), v.cpu().numpy()], axis=1)
             sc.close()
+    return out
+
+
+def passes():
+    """Runs with a max_rows small enough to split them into several passes, and ESM-1v wt-marginals of a 1 500-residue protein over
+    overlapping 1024-token windows."""
+    from proteingym_b200 import checkpoint, synth
+    from proteingym_b200 import poet_engine as E
+    from proteingym_b200.esm_engine import EsmScorer
+    from proteingym_b200.progen3_engine import Progen3Scorer
+    out = Runs()
+    arch = synth.Progen3Arch(2, 256, 4, 2, 512)
+    conf = checkpoint.progen3_config(arch.config())
+    st = checkpoint.normalise_progen3_state(conf, synth.make_progen3_state(arch, 41))
+    rng = np.random.default_rng(42)
+    rows = [[1] + list(rng.integers(6, 34, n - 1)) for n in (5, 70, 130, 130, 300, 301, 301)]  # one batch of T = 301: three passes
+    for mode in ("f16x3", "f16f8"):
+        sc = Progen3Scorer(conf, st, precision=mode, max_rows=700)
+        out[f"progen3.{mode}.passes"] = sc.token_sums(rows)
+        sc.close()
+
+    def row(n):
+        return np.concatenate([[E.START], rng.integers(0, 20, size=n - 2), [E.STOP]]).astype(np.int64)
+    ctx = [row(n) for n in (40, 130, 7, 90)]
+    variants = [row(n) for n in (20, 65, 128, 129, 3, 100, 129)]  # T = 129: two rows per pass, four passes
+    arch = synth.PoetArch(2, 256, 4, norm=True)
+    st = synth.make_poet_state(arch, seed=43)
+    conf = checkpoint.PoetConfig(arch.layers, arch.hidden_dim, arch.heads, 4 * arch.hidden_dim, True)
+    for mode in ("f16x3", "f16f8"):
+        sc = E.PoetScorer(conf, st, 256, precision=mode, max_rows=300)
+        sc.set_context(ctx)
+        out[f"poet.{mode}.passes.sum"] = sc.loglik(variants)
+        out[f"poet.{mode}.passes.tok"] = sc.loglik(variants, tok_logp=True)[1]
+        sc.close()
+    arch = synth.EsmArch("esm1v", 2, 256, 4, 1024)
+    sc = EsmScorer(checkpoint.config_from_synth(arch), checkpoint.normalise_synth_state(arch, synth.make_esm_state(arch, seed=44)),
+                   precision="f16x3")
+    out["esm1v.f16x3.wt_overlapping"] = sc.wt_marginal_table_overlapping(synth.random_protein(1500, 45)).cpu().numpy()
+    sc.close()
     return out
 
 

@@ -4,6 +4,7 @@ arithmetic (mean per (chunk, direction), divided by 2 * n_chunks, and the failur
 rows, the checkpoint loader's key mapping, tying and refusals, and the drop-in CLI's flags."""
 import json
 import os
+import re
 import shutil
 
 import numpy as np
@@ -171,7 +172,8 @@ def test_cli_flags_match_reference():
     assert set(got) - set(want) == {"--precision", "--device"}
 
 
-def test_refusals_are_in_the_library():
+def test_refusals_are_in_the_library_and_its_architecture_table():
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     src = open(os.path.join(root, "proteingym_b200", "csrc", "api.cu")).read()
-    assert "ProtGPT2 needs head_dim 64" in src and "ProtGPT2 has no retrieval fusion" in src
+    assert "ProtGPT2 needs head_dim 64" in src and "has no retrieval fusion" in src
+    assert re.search(r'\{PG_ARCH_PROTGPT2,\s*"ProtGPT2",\s*FAM_DECODER,\s*false,', src)  # no retrieval fusion

@@ -3,6 +3,7 @@ reference's scores, the tokenizer matches the ``tokenizers`` library on both fix
 row de-duplication and the prefix plan, the drop-in CLI's flags, the checkpoint loader's key mapping and tying rule, and refusals."""
 import json
 import os
+import re
 import warnings
 
 import numpy as np
@@ -183,9 +184,10 @@ def test_loader_key_mapping_and_tying(tmp_path):
         checkpoint.load_rita_checkpoint(str(tmp_path / "bad2"))
 
 
-def test_refusals_are_in_the_library():
+def test_refusals_are_in_the_library_and_its_architecture_table():
     src = open(os.path.join(os.path.dirname(GOLDEN), "..", "proteingym_b200", "csrc", "api.cu")).read()
-    assert "RITA needs head_dim 64" in src and "RITA has no retrieval fusion" in src
+    assert "RITA needs head_dim 64" in src and "has no retrieval fusion" in src
+    assert re.search(r'\{PG_ARCH_RITA,\s*"RITA",\s*FAM_DECODER,\s*false,', src)  # no retrieval fusion
     hdr = open(os.path.join(os.path.dirname(GOLDEN), "..", "include", "pgscore.h")).read()
     assert "PG_ARCH_RITA = 5" in hdr
 
